@@ -32,6 +32,15 @@ SYMBOLS = [
 ]
 
 
+# every option name dgb_set_option accepts (csrc/capi.cu optionSlot; defaults in csrc/common.cuh Options)
+OPTION_NAMES = [
+    "decode_fused", "decode_warps", "decode_slot_words", "encode_warps", "encode_canonical", "encode_fused",
+    "fused_stats_every", "fused_stage", "fused_chunk_blocks", "encode_wide_table", "encode_slot_words",
+    "stats_stage", "stats_stage_kb", "encode_k2_ctas", "hist_slab_kb", "hist_ctas_per_sm", "inline_members",
+    "pull_ctas", "first_part_pct", "last_part_pct", "timing", "parts",
+]
+
+
 class DietGpuError(RuntimeError):
     def __init__(self, code: int, what: str):
         super().__init__(f"dietgpu_b200: {what} failed: {error_string(code)} (code {code}"

@@ -62,6 +62,24 @@ def test_error_codes_without_gpu():
     assert capi.get_option("decode_fused") == 1
 
 
+def test_option_names_cover_every_option():
+    # capi.OPTION_NAMES is what the tests' codec_options() saves and restores: it must name every option the
+    # library accepts, so that no test can leak a changed option into the next one
+    import re
+
+    from codec_helpers import codec_options
+    from dietgpu_b200 import capi
+
+    src = open(os.path.join(ROOT, "dietgpu_b200", "csrc", "capi.cu")).read()
+    body = src[src.index("static int* optionSlot"):src.index("int dgb_set_option")]
+    assert sorted(re.findall(r'strcmp\(name, "(\w+)"\)', body)) == sorted(capi.OPTION_NAMES)
+    before = {k: capi.get_option(k) for k in capi.OPTION_NAMES}
+    with codec_options(encode_fused=1, decode_warps=4):
+        capi.set_option("parts", 3)  # set inside the body without going through codec_options
+        assert capi.get_option("encode_fused") == 1 and capi.get_option("decode_warps") == 4
+    assert {k: capi.get_option(k) for k in capi.OPTION_NAMES} == before
+
+
 def test_product_does_not_import_oracle():
     # the shipped package must never route through the CPU oracle
     pkg = os.path.join(ROOT, "dietgpu_b200")

@@ -7,52 +7,13 @@ import numpy as np
 import pytest
 import torch
 
+from codec_helpers import (KINDS, ans_roundtrip, assert_pdf_matches, codec_options, dg, exact_histogram, float_roundtrip,
+                           guarded_compress, guarded_decode, oracle_archive, to_dev_bytes, words_to_tensor)
+from codec_helpers import options  # noqa: F401  (fixture)
 from conftest import exp_bytes, normal_words, zipf_bytes
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
-
-KINDS = {"f16": (O.F16, torch.float16, np.uint16), "bf16": (O.BF16, torch.bfloat16, np.uint16),
-         "f32": (O.F32, torch.float32, np.uint32)}
-
-
-def dg():
-    import dietgpu_b200
-
-    return dietgpu_b200
-
-
-def to_dev_bytes(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def words_to_tensor(w, kind):
-    _, tdt, _ = KINDS[kind]
-    t = torch.from_numpy(w.view(np.int16 if w.dtype == np.uint16 else np.int32).copy())
-    return t.view(tdt).cuda()
-
-
-def ans_roundtrip(arrays, pb, checksum=False):
-    ts = [to_dev_bytes(a) for a in arrays]
-    comp, sizes, _ = dg().compress_data(False, ts, checksum, prob_bits=pb)
-    hs = sizes.cpu().tolist()
-    rows = []
-    for i, a in enumerate(arrays):
-        want = O.ans_encode(a, pb, checksum)
-        got = comp[i, :hs[i]].cpu().numpy()
-        assert hs[i] == want.size, f"member {i}: size {hs[i]} != oracle {want.size}"
-        assert hs[i] % 16 == 0  # ans/ANSTest.cu:131-135
-        O.assert_same_ans(got, want, f"member {i}")
-        rows.append(comp[i, :hs[i]].clone())  # exactly-truncated buffers (ans_test.py:21-26)
-    outs = [torch.empty_like(t) for t in ts]
-    status = torch.zeros(len(ts), dtype=torch.uint8, device="cuda")
-    osz = torch.zeros(len(ts), dtype=torch.int32, device="cuda")
-    dg().decompress_data(False, rows, outs, checksum, None, status, osz, prob_bits=pb)
-    assert status.cpu().tolist() == [1] * len(ts)
-    assert osz.cpu().tolist() == [a.size for a in arrays]
-    for t, o in zip(ts, outs):
-        assert torch.equal(t, o)
-
 
 @pytest.mark.parametrize("pb", [9, 10, 11])
 @pytest.mark.parametrize("lam", [1.0, 10.0, 100.0, 1000.0])
@@ -201,35 +162,6 @@ def test_ans_stride_api():
 
 # ------------------------------------------------------------------ floats ----
 
-def float_roundtrip(kind, word_arrays, pb=10, checksum=False, offsets=None):
-    ft, tdt, _ = KINDS[kind]
-    ts = []
-    for i, w in enumerate(word_arrays):
-        off = 0 if offsets is None else offsets[i]
-        full = words_to_tensor(np.concatenate([np.zeros(off, w.dtype), w]), kind)
-        ts.append(full[off:])  # element-aligned but possibly not 16 B aligned (float/FloatTest.cu:276-282)
-    comp, sizes, _ = dg().compress_data(True, ts, checksum, prob_bits=pb)
-    hs = sizes.cpu().tolist()
-    rows = []
-    for i, w in enumerate(word_arrays):
-        want = O.float_compress(ft, w, pb, checksum)
-        assert hs[i] == want.size, f"member {i}: size {hs[i]} != oracle {want.size}"
-        O.assert_same_float(comp[i, :hs[i]].cpu().numpy(), want, ft, f"member {i}")
-        rows.append(comp[i, :hs[i]].clone())
-    outs = []
-    for i, t in enumerate(ts):
-        off = 0 if offsets is None else (offsets[i] + 1) % 5
-        outs.append(torch.empty(t.numel() + off, dtype=tdt, device="cuda")[off:])
-    status = torch.zeros(len(ts), dtype=torch.uint8, device="cuda")
-    osz = torch.zeros(len(ts), dtype=torch.int32, device="cuda")
-    dg().decompress_data(True, rows, outs, checksum, None, status, osz, prob_bits=pb)
-    assert status.cpu().tolist() == [1] * len(ts)
-    assert osz.cpu().tolist() == [w.size for w in word_arrays]
-    it = torch.int16 if kind != "f32" else torch.int32
-    for t, o in zip(ts, outs):
-        assert torch.equal(t.view(it), o.view(it))
-
-
 @pytest.mark.parametrize("kind", ["f16", "bf16", "f32"])
 @pytest.mark.parametrize("pb", [9, 10])
 def test_float_batch(kind, pb):
@@ -300,123 +232,107 @@ def test_float_capacity_failure():
 
 # ------------------------------------------- full-size configs (properties) ----
 
+def _full_batch_parity(kind, uniq, ts, pb, what):
+    """Batch parity for the large configurations: every member's stored pdf against O.normalize of its
+    exact histogram, every distinct input's whole archive against the oracle, every repeated member
+    semantically equal to its first copy; then a guard-banded decode of the whole batch."""
+    as_float = kind != "bytes"
+    comp, hs = guarded_compress(as_float, ts, False, pb)
+    nu = len(uniq)
+    for i, t in enumerate(ts):
+        assert_pdf_matches(comp[i, :hs[i]].cpu().numpy(), t, kind, pb, f"{what} member {i}")
+    first = [comp[i, :hs[i]].cpu().numpy() for i in range(nu)]
+    for i, u in enumerate(uniq):
+        want = oracle_archive(kind, u, pb)
+        assert hs[i] == want.size, f"{what} member {i}: size {hs[i]} != oracle {want.size}"
+        if as_float:
+            O.assert_same_float(first[i], want, KINDS[kind][0], f"{what} member {i}")
+        else:
+            O.assert_same_ans(first[i], want, f"{what} member {i}")
+    for i in range(nu, len(ts)):
+        got = comp[i, :hs[i]].cpu().numpy()
+        if as_float:
+            O.assert_same_float(got, first[i % nu], KINDS[kind][0], f"{what} member {i} vs member {i % nu}")
+        else:
+            O.assert_same_ans(got, first[i % nu], f"{what} member {i} vs member {i % nu}")
+    guarded_decode(as_float, [comp[i, :hs[i]] for i in range(len(ts))], [t.numel() for t in ts], ts[0].dtype, pb,
+                   False, ts, what)
+
+
 def test_config2_zipf_256mib_roundtrip():
-    # BASELINE configs[1]: 64 x 4 MiB Zipf bytes, prec 10 and 11: round trip + size == oracle on a sample
-    members = [to_dev_bytes(zipf_bytes(4 << 20, 1.0 if i % 2 == 0 else 1.5, 1234 + i)) for i in range(8)]
+    # BASELINE configs[1]: 64 x 4 MiB Zipf bytes (8 distinct members, each repeated 8 times), prec 10 and 11
+    uniq = [zipf_bytes(4 << 20, 1.0 if i % 2 == 0 else 1.5, 1234 + i) for i in range(8)]
+    members = [to_dev_bytes(u) for u in uniq]
     ts = [members[i % 8] for i in range(64)]
     for pb in (10, 11):
-        comp, sizes, _ = dg().compress_data(False, ts, prob_bits=pb)
-        hs = sizes.cpu().tolist()
-        for i in (0, 1):
-            want = O.ans_encode(members[i].cpu().numpy(), pb)
-            assert hs[i] == want.size
-            O.assert_same_ans(comp[i, :hs[i]].cpu().numpy(), want)
-        assert hs[:8] * 8 == hs
-        outs = [torch.empty_like(t) for t in ts]
-        dg().decompress_data(False, [comp[i, :hs[i]] for i in range(64)], outs, prob_bits=pb)
-        for i in range(64):
-            assert torch.equal(outs[i], ts[i])
+        _full_batch_parity("bytes", uniq, ts, pb, f"c2 pb {pb}")
 
 
 @pytest.mark.parametrize("kind,batch,relu", [("bf16", 64, False), ("f16", 256, True)])
 def test_config3_4_float_256mib_roundtrip(kind, batch, relu):
-    # BASELINE configs[2]/[3]: 256 MiB of 16-bit floats; round trip + oracle equality on one member
+    # BASELINE configs[2]/[3]: 256 MiB of 16-bit floats (4 distinct members, repeated)
     per = (128 << 20) // batch
     uniq = [normal_words(per, kind, 1234 + i, relu=relu) for i in range(4)]
     dev = [words_to_tensor(u, kind) for u in uniq]
     ts = [dev[i % 4] for i in range(batch)]
-    comp, sizes, _ = dg().compress_data(True, ts)
-    hs = sizes.cpu().tolist()
-    want = O.float_compress(KINDS[kind][0], uniq[0], 10)
-    assert hs[0] == want.size
-    O.assert_same_float(comp[0, :hs[0]].cpu().numpy(), want, KINDS[kind][0])
-    outs = [torch.empty_like(t) for t in ts]
-    dg().decompress_data(True, [comp[i, :hs[i]] for i in range(batch)], outs)
-    for i in range(batch):
-        assert torch.equal(outs[i].view(torch.int16), ts[i].view(torch.int16))
+    _full_batch_parity(kind, uniq, ts, 10, f"{kind} x {batch}")
 
 
 def test_single_member_256mib_bf16():
-    # bs = 1 x 128 Mi floats: 32768 blocks in one member (look-back across many tickets)
-    w = words_to_tensor(normal_words(128 << 20, "bf16", 99), "bf16")
-    comp, sizes, _ = dg().compress_data(True, [w])
-    n = int(sizes[0])
+    # bs = 1 x 128 Mi floats: 32768 blocks in one member (look-back across many tickets), 2^27 symbols in
+    # one histogram (fp32 conversion of the counts rounds)
+    u = normal_words(128 << 20, "bf16", 99)
+    w = words_to_tensor(u, "bf16")
+    comp, hs = guarded_compress(True, [w], False, 10)
+    n = hs[0]
     ratio = n / (w.numel() * 2)
     assert 0.66 < ratio < 0.69  # README: ~0.673
-    out = torch.empty_like(w)
-    dg().decompress_data(True, [comp[0, :n]], [out])
-    assert torch.equal(out.view(torch.int16), w.view(torch.int16))
+    got = comp[0, :n].cpu().numpy()
+    assert_pdf_matches(got, w, "bf16", 10, "128 Mi bf16")
+    want = oracle_archive("bf16", u, 10)
+    assert n == want.size
+    O.assert_same_float(got, want, O.BF16, "128 Mi bf16")
+    guarded_decode(True, [comp[0, :n]], [w.numel()], torch.bfloat16, 10, False, [w], "128 Mi bf16")
 
 
-def test_canonical_layout_is_byte_exact():
+def test_canonical_layout_is_byte_exact(options):
     # option encode_canonical: streams packed in block order -> archives equal the oracle's byte for byte
-    from dietgpu_b200 import capi
-
-    capi.set_option("encode_canonical", 1)
-    try:
-        arrays = [zipf_bytes(300000, 1.1, 5), exp_bytes(4097, 50, 6), exp_bytes(70000, 10, 7), np.zeros(0, np.uint8)]
-        for pb in (9, 10, 11):
-            ts = [to_dev_bytes(a) for a in arrays]
-            comp, sizes, _ = dg().compress_data(False, ts, True, prob_bits=pb)
-            hs = sizes.cpu().tolist()
-            for i, a in enumerate(arrays):
-                assert np.array_equal(comp[i, :hs[i]].cpu().numpy(), O.ans_encode(a, pb, True))
-        for kind in ("bf16", "f16", "f32"):
-            ws = [normal_words(n, kind, n) for n in (100000, 4096, 33)]
-            ts = [words_to_tensor(w, kind) for w in ws]
-            comp, sizes, _ = dg().compress_data(True, ts, True)
-            hs = sizes.cpu().tolist()
-            for i, w in enumerate(ws):
-                assert np.array_equal(comp[i, :hs[i]].cpu().numpy(), O.float_compress(KINDS[kind][0], w, 10, True))
-            outs = [torch.empty_like(t) for t in ts]
-            dg().decompress_data(True, [comp[i, :hs[i]] for i in range(len(ts))], outs, True)
-            it = torch.int16 if kind != "f32" else torch.int32
-            for t, o in zip(ts, outs):
-                assert torch.equal(t.view(it), o.view(it))
-    finally:
-        capi.set_option("encode_canonical", 0)
+    options(encode_canonical=1)
+    arrays = [zipf_bytes(300000, 1.1, 5), exp_bytes(4097, 50, 6), exp_bytes(70000, 10, 7), np.zeros(0, np.uint8)]
+    for pb in (9, 10, 11):
+        ans_roundtrip(arrays, pb, True, exact=True)
+    for kind in ("bf16", "f16", "f32"):
+        float_roundtrip(kind, [normal_words(n, kind, n) for n in (100000, 4096, 33)], 10, True, exact=True)
 
 
-def test_small_staging_slot_spills():
+def test_small_staging_slot_spills(options):
     # the fast encoder's staging slot can be smaller than a block's worst-case stream; force the
     # spill path with the smallest slot on incompressible and on ragged inputs
-    from dietgpu_b200 import capi
-
-    capi.set_option("encode_slot_words", 776)
-    try:
-        arrays = [np.random.default_rng(5).integers(0, 256, 300000, dtype=np.uint8), zipf_bytes(123457, 1.0, 3),
-                  exp_bytes(4097, 2, 4), exp_bytes(31, 1, 5)]
-        for pb in (9, 10, 11):
-            ans_roundtrip(arrays, pb, checksum=True)
-        float_roundtrip("f32", [np.random.default_rng(6).integers(0, 2**32, 100000, dtype=np.uint32)], 10)
-        float_roundtrip("bf16", [np.random.default_rng(7).integers(0, 2**16, 200001, dtype=np.uint16)], 11)
-    finally:
-        capi.set_option("encode_slot_words", 0)
+    options(encode_slot_words=776)
+    arrays = [np.random.default_rng(5).integers(0, 256, 300000, dtype=np.uint8), zipf_bytes(123457, 1.0, 3),
+              exp_bytes(4097, 2, 4), exp_bytes(31, 1, 5)]
+    for pb in (9, 10, 11):
+        ans_roundtrip(arrays, pb, checksum=True)
+    float_roundtrip("f32", [np.random.default_rng(6).integers(0, 2**32, 100000, dtype=np.uint32)], 10)
+    float_roundtrip("bf16", [np.random.default_rng(7).integers(0, 2**16, 200001, dtype=np.uint16)], 11)
 
 
-def test_sub_batch_streams():
+def test_sub_batch_streams(options):
     # large batches are cut into sub-batches that run on internal streams; force 1/2/4 parts on
     # batches of 1, 3 and many members (incl. empty members) and check parity each time
-    from dietgpu_b200 import capi
-
-    try:
-        for parts in (1, 2, 4):
-            capi.set_option("parts", parts)
-            ans_roundtrip([zipf_bytes(50000, 1.0, 1)], 10)
-            ans_roundtrip([exp_bytes(9000, 5, 2), np.zeros(0, np.uint8), exp_bytes(70000, 50, 3)], 10, checksum=True)
-            ans_roundtrip([exp_bytes(1000 + 513 * i, 20, i) for i in range(37)], 11)
-            float_roundtrip("bf16", [normal_words(3000 + 1111 * i, "bf16", i) for i in range(19)], 10, checksum=True)
-            float_roundtrip("f32", [normal_words(5000, "f32", 1), normal_words(0, "f32", 2)], 10)
-    finally:
-        capi.set_option("parts", 0)
+    for parts in (1, 2, 4):
+        options(parts=parts)
+        ans_roundtrip([zipf_bytes(50000, 1.0, 1)], 10)
+        ans_roundtrip([exp_bytes(9000, 5, 2), np.zeros(0, np.uint8), exp_bytes(70000, 50, 3)], 10, checksum=True)
+        ans_roundtrip([exp_bytes(1000 + 513 * i, 20, i) for i in range(37)], 11)
+        float_roundtrip("bf16", [normal_words(3000 + 1111 * i, "bf16", i) for i in range(19)], 10, checksum=True)
+        float_roundtrip("f32", [normal_words(5000, "f32", 1), normal_words(0, "f32", 2)], 10)
 
 
-def test_two_host_threads_with_sub_batches():
+def test_two_host_threads_with_sub_batches(options):
     # two host threads, each on its own CUDA stream, both forcing sub-batch streams: the internal
     # fork/join streams and events are per thread, so the calls must not disturb each other
     import threading
-
-    from dietgpu_b200 import capi
 
     errs = []
 
@@ -430,45 +346,32 @@ def test_two_host_threads_with_sub_batches():
         except Exception as e:  # noqa: BLE001
             errs.append(repr(e))
 
-    try:
-        capi.set_option("parts", 3)
-        th = [threading.Thread(target=worker, args=(100 * k,)) for k in range(2)]
-        for t in th:
-            t.start()
-        for t in th:
-            t.join()
-    finally:
-        capi.set_option("parts", 0)
+    options(parts=3)
+    th = [threading.Thread(target=worker, args=(100 * k,)) for k in range(2)]
+    for t in th:
+        t.start()
+    for t in th:
+        t.join()
     assert not errs, errs
 
 
-def test_encoder_table_formats():
+def test_encoder_table_formats(options):
     # the encoder symbol table has a 16-byte and an 8-byte entry format (chosen by data kind);
     # force each one on every kind, all precisions, incl. pdf == 1 symbols and a single-symbol input
-    from dietgpu_b200 import capi
-
-    try:
-        for wide in (0, 1):
-            capi.set_option("encode_wide_table", wide)
-            for pb in (9, 10, 11):
-                ans_roundtrip([zipf_bytes(200000, 1.0, 1), exp_bytes(4097, 3, 2), np.full(5000, 7, np.uint8),
-                               np.random.default_rng(3).integers(0, 256, 70001, dtype=np.uint8)], pb, checksum=True)
-            for ft in ("f16", "bf16", "f32"):
-                float_roundtrip(ft, [normal_words(100000 + 7 * i, ft, i) for i in range(3)], 10, checksum=True)
-    finally:
-        capi.set_option("encode_wide_table", -1)
+    for wide in (0, 1):
+        options(encode_wide_table=wide)
+        for pb in (9, 10, 11):
+            ans_roundtrip([zipf_bytes(200000, 1.0, 1), exp_bytes(4097, 3, 2), np.full(5000, 7, np.uint8),
+                           np.random.default_rng(3).integers(0, 256, 70001, dtype=np.uint8)], pb, checksum=True)
+        for ft in ("f16", "bf16", "f32"):
+            float_roundtrip(ft, [normal_words(100000 + 7 * i, ft, i) for i in range(3)], 10, checksum=True)
 
 
 def test_kernel_variants_agree():
     # every tuning variant produces identical results: single-launch vs two-kernel paths in both
     # directions, chunk sizes, statistics-CTA share, warps per CTA, canonical packing
-    from dietgpu_b200 import capi
-
     a = [zipf_bytes(300000, 1.1, 5), exp_bytes(4097, 50, 6), zipf_bytes(1, 1.0, 7), np.zeros(0, np.uint8)]
     f = [normal_words(50000 + 13 * i, "bf16", i) for i in range(5)]
-    names = ("encode_fused", "decode_fused", "fused_chunk_blocks", "fused_stats_every", "fused_stage",
-             "encode_warps", "encode_canonical", "inline_members", "decode_warps")
-    defaults = {k: capi.get_option(k) for k in names}
     variants = [
         dict(encode_fused=0, decode_fused=0),
         dict(encode_fused=1, decode_fused=0),
@@ -488,15 +391,10 @@ def test_kernel_variants_agree():
         dict(decode_warps=4),
         dict(inline_members=0),  # member table uploaded to scratch instead of travelling in the kernel parameters
     ]
-    try:
-        for v in variants:
-            for k, d in defaults.items():
-                capi.set_option(k, v.get(k, d))
+    for v in variants:
+        with codec_options(**v):
             ans_roundtrip(a, 10)
             float_roundtrip("bf16", f, 10)
-    finally:
-        for k, d in defaults.items():
-            capi.set_option(k, d)
 
 
 def test_more_members_than_fit_the_kernel_parameters():
@@ -585,7 +483,8 @@ def test_archive_mover_copies_exactly_the_archive():
 def test_members_near_the_format_limit():
     # one member of 1.5 Gi + 1 symbols: the largest round size whose worst-case archive still fits the format's
     # 32-bit sizes (dgb_*_max_compressed_size != 0); 393 217 blocks, block offsets above 2^31 bytes in the
-    # float output.  Round trip, status, reported size against the archive's own header fields.
+    # float output.  Round trip, status, reported size against the archive's own header fields, and the
+    # stored pdf against O.normalize of the exact histogram.
     from dietgpu_b200 import ops
 
     n = (3 << 29) + 1
@@ -611,6 +510,10 @@ def test_members_near_the_format_limit():
         else:
             ans = words
         h = ans[:16].view(torch.int32).cpu().tolist()
+        # counts far above 2^24: the stored pdf against O.normalize of the exact histogram
+        hist = exact_histogram(x, "bf16" if as_float else "bytes")
+        assert np.array_equal(ans[32:544].cpu().numpy().view(np.uint16).astype(np.uint32),
+                              O.normalize(hist.astype(np.uint32), n, 10))
         nb = (n + 4095) // 4096
         assert (h[0] & 0xffffffff) == 0xd00d0001 and h[1] == nb and h[2] == n
         total_words = h[3] & 0xffffffff
