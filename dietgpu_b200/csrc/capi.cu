@@ -43,8 +43,69 @@ cudaEvent_t takeEvent() {
 thread_local TimedLaunch tlsOpen[kNumSlots];
 }  // namespace
 
+HostStage& hostStage() {
+  static thread_local HostStage h;
+  return h;
+}
+
+int smCount() {
+  // per device (a process may drive several); racing first calls write the same value
+  static int cached[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (!cached[dev]) {
+    int v = 0;
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    cached[dev] = v > 0 ? v : 132;
+  }
+  return cached[dev];
+}
+
+int residentCtasPerSm(const void* kernel, int threads, size_t smemBytes, int maxDynamicSmem, int* out) {
+  // function attributes are per device; a thread that drives several devices keeps an entry per device.
+  // A full cache overwrites its oldest entry, which costs one recomputation later.
+  struct Entry {
+    const void* kernel;
+    int dev, threads;
+    size_t smem;
+    int perSm;  // 0: only the shared-memory limit is set
+  };
+  constexpr int kEntries = 64;
+  static thread_local Entry cache[kEntries];
+  static thread_local int nextEntry = 0;
+  int dev = 0;
+  DGB_CUDA_TRY(cudaGetDevice(&dev));
+  bool limitSet = false;
+  for (const Entry& e : cache) {
+    if (e.kernel != kernel || e.dev != dev) continue;
+    limitSet = true;
+    if (!out) return DGB_OK;
+    if (e.perSm && e.threads == threads && e.smem == smemBytes) {
+      *out = e.perSm;
+      return DGB_OK;
+    }
+  }
+  if (!limitSet) DGB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, maxDynamicSmem));
+  int perSm = 0;
+  if (out) {
+    DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smemBytes));
+    perSm = std::max(perSm, 1);
+    *out = perSm;
+  }
+  cache[nextEntry] = Entry{kernel, dev, threads, smemBytes, perSm};
+  nextEntry = (nextEntry + 1) % kEntries;
+  return DGB_OK;
+}
+
+// ---- sub-batches -------------------------------------------------------------
+struct StreamPool {
+  cudaStream_t s[kMaxParts];
+  cudaEvent_t start, done[kMaxParts];
+};
+
+namespace {
 // One pool per (host thread, device): the fork/join events of a call must not be shared with a call
-// that another thread, or the same thread on another device, makes at the same time.
+// that another thread, or the same thread on another device, makes at the same time.  Lazily created.
 int streamPool(StreamPool** out) {
   constexpr int kMaxDevices = 64;
   struct Slot {
@@ -80,30 +141,32 @@ int streamPool(StreamPool** out) {
   return DGB_OK;
 }
 
-void splitParts(const uint64_t* weight, uint32_t n, int parts, uint32_t* bounds) {
+// cuts members [0,n) into `parts` contiguous ranges of roughly equal bytes; bounds has parts+1 entries
+void splitParts(const MemberDesc* members, uint32_t n, uint32_t wordBytes, int parts, const Options& opt,
+                uint32_t* bounds) {
+  auto weight = [&](uint32_t i) { return (uint64_t)members[i].size * wordBytes; };
   uint64_t total = 0;
-  for (uint32_t i = 0; i < n; ++i) total += weight[i];
+  for (uint32_t i = 0; i < n; ++i) total += weight(i);
   bounds[0] = 0;
   uint64_t acc = 0;
   uint32_t idx = 0;
   // options first_part_pct / last_part_pct: size of the first / last sub-batch in percent of an equal share
   // (100 = equal); the middle sub-batches share the rest equally
-  const int fp = parts > 2 ? std::max(10, std::min(200, options().first_part_pct)) : 100;
-  const int lp = parts > 2 ? std::max(10, std::min(200, options().last_part_pct)) : 100;
+  const int fp = parts > 2 ? std::max(10, std::min(200, opt.first_part_pct)) : 100;
+  const int lp = parts > 2 ? std::max(10, std::min(200, opt.last_part_pct)) : 100;
   const uint64_t eq = total / (uint64_t)parts;
   const uint64_t first = eq * (uint64_t)fp / 100u, last = eq * (uint64_t)lp / 100u;
   const uint64_t mid = parts > 2 && total > first + last ? (total - first - last) / (uint64_t)(parts - 2) : eq;
   for (int p = 1; p < parts; ++p) {
     const uint64_t target = (parts > 2 && (fp != 100 || lp != 100)) ? first + mid * (uint64_t)(p - 1) : eq * (uint64_t)p;
     const uint32_t mustLeave = (uint32_t)(parts - p);  // one member for every later part
-    while (idx + mustLeave < n && (idx < bounds[p - 1] + 1 || acc + weight[idx] / 2 <= target)) acc += weight[idx++];
+    while (idx + mustLeave < n && (idx < bounds[p - 1] + 1 || acc + weight(idx) / 2 <= target)) acc += weight(idx++);
     bounds[p] = idx;
   }
   bounds[parts] = n;
 }
 
-int autoParts(int kind, uint32_t n, uint64_t totalBytes, bool decode) {
-  const Options& o = options();
+int autoParts(int kind, uint32_t n, uint64_t totalBytes, const Options& o) {
   if (o.timing) return 1;  // per-kernel timing wants un-overlapped launches
   int p = o.parts;
   // float encode of large batches runs in sub-batches so that the bandwidth-bound statistics kernel of
@@ -117,19 +180,54 @@ int autoParts(int kind, uint32_t n, uint64_t totalBytes, bool decode) {
   p = std::min(p, kMaxParts);
   return (int)std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)p, n));
 }
+}  // namespace
+
+SubBatches::SubBatches(int kind, const MemberDesc* members, uint32_t n, const Options& opt, bool split,
+                       cudaStream_t stream)
+    : stream_(stream) {
+  const uint32_t wb = wordBytes(kind);
+  uint64_t totalBytes = 0;
+  for (uint32_t i = 0; i < n; ++i) totalBytes += (uint64_t)members[i].size * wb;
+  parts_ = split ? autoParts(kind, n, totalBytes, opt) : 1;
+  splitParts(members, n, wb, parts_, opt, bounds_);
+}
+
+int SubBatches::fork() {
+  if (parts_ == 1) return DGB_OK;
+  const int rc = streamPool(&pool_);
+  if (rc != DGB_OK) return rc;
+  DGB_CUDA_TRY(cudaEventRecord(pool_->start, stream_));
+  return DGB_OK;
+}
+
+int SubBatches::stream(int k, cudaStream_t* out) {
+  *out = stream_;
+  if (parts_ == 1) return DGB_OK;
+  DGB_CUDA_TRY(cudaStreamWaitEvent(pool_->s[k], pool_->start, 0));
+  forked_[k] = true;
+  *out = pool_->s[k];
+  return DGB_OK;
+}
+
+SubBatches::~SubBatches() {
+  if (!pool_) return;
+  for (int k = 0; k < kMaxParts; ++k)
+    if (forked_[k] && cudaEventRecord(pool_->done[k], pool_->s[k]) == cudaSuccess)
+      cudaStreamWaitEvent(stream_, pool_->done[k], 0);
+}
 
 // kernels launched by this library since load (every codec launch site calls timerBegin first)
 static std::atomic<int> gLaunches{0};
 
-void timerBegin(int slot, cudaStream_t stream) {
+void timerBegin(const Options& opt, int slot, cudaStream_t stream) {
   gLaunches.fetch_add(1, std::memory_order_relaxed);
-  if (!options().timing) return;
+  if (!opt.timing) return;
   TimedLaunch t{slot, takeEvent(), takeEvent()};
   cudaEventRecord(t.a, stream);
   tlsOpen[slot] = t;
 }
-void timerEnd(int slot, cudaStream_t stream) {
-  if (!options().timing) return;
+void timerEnd(const Options& opt, int slot, cudaStream_t stream) {
+  if (!opt.timing) return;
   cudaEventRecord(tlsOpen[slot].b, stream);
   std::lock_guard<std::mutex> lock(timerMutex());
   timedLaunches().push_back(tlsOpen[slot]);
@@ -138,13 +236,18 @@ void timerEnd(int slot, cudaStream_t stream) {
 namespace {
 
 bool validFloatType(int ft) { return ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32; }
-uint32_t wordBytes(int kind) { return kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u); }
+
+// the calling thread's member list, sized for n members
+HostMember* stageMembers(uint32_t n) {
+  std::vector<HostMember>& v = hostStage().members;
+  v.resize(n);
+  return v.data();
+}
 
 // pointer form
-int buildPointer(uint32_t n, const void* const* in, const uint32_t* size, void* const* out,
-                 std::vector<HostMember>& v) {
+int buildPointer(uint32_t n, const void* const* in, const uint32_t* size, void* const* out, HostMember** members) {
   if (n && (!in || !size || !out)) return DGB_ERR_INVALID_ARG;
-  v.resize(n);
+  HostMember* v = *members = stageMembers(n);
   for (uint32_t i = 0; i < n; ++i) v[i] = HostMember{in[i], out[i], size[i]};
   return DGB_OK;
 }
@@ -208,10 +311,10 @@ int dgb_ans_encode_pointer(void* temp, size_t tempBytes, int pb, int useChecksum
                            const void* const* in, const uint32_t* inSize,
                            const uint32_t* histogram_dev, void* const* out, uint32_t* outSize_dev,
                            void* stream) {
-  std::vector<HostMember> v;
-  int rc = buildPointer(n, in, inSize, out, v);
+  HostMember* v = nullptr;
+  int rc = buildPointer(n, in, inSize, out, &v);
   if (rc) return rc;
-  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v.data(), histogram_dev,
+  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v, histogram_dev,
                      outSize_dev, (cudaStream_t)stream);
 }
 
@@ -220,11 +323,11 @@ int dgb_ans_encode_stride(void* temp, size_t tempBytes, int pb, int useChecksum,
                           const uint32_t* histogram_dev, void* out_dev, uint32_t outStride,
                           uint32_t* outSize_dev, void* stream) {
   if (n && (!out_dev || (inSize && !in_dev))) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
+  HostMember* v = stageMembers(n);
   for (uint32_t i = 0; i < n; ++i)
     v[i] = HostMember{static_cast<const uint8_t*>(in_dev) + (size_t)i * inStride,
                       static_cast<uint8_t*>(out_dev) + (size_t)i * outStride, inSize};
-  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v.data(), histogram_dev,
+  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v, histogram_dev,
                      outSize_dev, (cudaStream_t)stream);
 }
 
@@ -233,7 +336,7 @@ int dgb_ans_encode_split_size(void* temp, size_t tempBytes, int pb, int useCheck
                               const uint32_t* histogram_dev, void* out_dev, uint32_t outStride,
                               uint32_t* outSize_dev, void* stream) {
   if (n && (!splitSizes || !out_dev)) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
+  HostMember* v = stageMembers(n);
   size_t off = 0;
   for (uint32_t i = 0; i < n; ++i) {
     // ans/GpuANSEncode.cu:132-140: interior splits must keep 4 B alignment
@@ -242,7 +345,7 @@ int dgb_ans_encode_split_size(void* temp, size_t tempBytes, int pb, int useCheck
                       static_cast<uint8_t*>(out_dev) + (size_t)i * outStride, splitSizes[i]};
     off += splitSizes[i];
   }
-  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v.data(), histogram_dev,
+  return encodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v, histogram_dev,
                      outSize_dev, (cudaStream_t)stream);
 }
 
@@ -250,10 +353,10 @@ int dgb_float_compress_pointer(void* temp, size_t tempBytes, int ft, int pb, int
                                uint32_t n, const void* const* in, const uint32_t* inSize,
                                void* const* out, uint32_t* outSize_dev, void* stream) {
   if (!validFloatType(ft)) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v;
-  int rc = buildPointer(n, in, inSize, out, v);
+  HostMember* v = nullptr;
+  int rc = buildPointer(n, in, inSize, out, &v);
   if (rc) return rc;
-  return encodeBatch(ft, temp, tempBytes, pb, useChecksum != 0, n, v.data(), nullptr, outSize_dev,
+  return encodeBatch(ft, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev,
                      (cudaStream_t)stream);
 }
 
@@ -263,14 +366,14 @@ int dgb_float_compress_split_size(void* temp, size_t tempBytes, int ft, int pb, 
                                   void* stream) {
   if (!validFloatType(ft)) return DGB_ERR_INVALID_ARG;
   if (n && (!splitSizes || !out_dev)) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
+  HostMember* v = stageMembers(n);
   size_t off = 0;
   for (uint32_t i = 0; i < n; ++i) {
     v[i] = HostMember{static_cast<const uint8_t*>(in_dev) + off * wordBytes(ft),
                       static_cast<uint8_t*>(out_dev) + (size_t)i * outStride, splitSizes[i]};
     off += splitSizes[i];
   }
-  return encodeBatch(ft, temp, tempBytes, pb, useChecksum != 0, n, v.data(), nullptr, outSize_dev,
+  return encodeBatch(ft, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev,
                      (cudaStream_t)stream);
 }
 
@@ -280,10 +383,10 @@ static int decodePointerCommon(int kind, void* temp, size_t tempBytes, int pb, i
                                uint32_t n, const void* const* in, void* const* out,
                                const uint32_t* cap, uint8_t* outSuccess_dev, uint32_t* outSize_dev,
                                uint8_t* mismatchHost, void* stream) {
-  if (n && (!in || !out || !cap)) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
-  for (uint32_t i = 0; i < n; ++i) v[i] = HostMember{in[i], out[i], cap[i]};
-  return decodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v.data(), outSuccess_dev,
+  HostMember* v = nullptr;
+  int rc = buildPointer(n, in, cap, out, &v);
+  if (rc) return rc;
+  return decodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, outSuccess_dev,
                      outSize_dev, mismatchHost, (cudaStream_t)stream);
 }
 
@@ -292,13 +395,13 @@ static int decodeSplitCommon(int kind, void* temp, size_t tempBytes, int pb, int
                              const uint32_t* splitSizes, uint8_t* outSuccess_dev,
                              uint32_t* outSize_dev, uint8_t* mismatchHost, void* stream) {
   if (n && (!in || !splitSizes)) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
+  HostMember* v = stageMembers(n);
   size_t off = 0;
   for (uint32_t i = 0; i < n; ++i) {
     v[i] = HostMember{in[i], static_cast<uint8_t*>(out_dev) + off * wordBytes(kind), splitSizes[i]};
     off += splitSizes[i];
   }
-  return decodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v.data(), outSuccess_dev,
+  return decodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, outSuccess_dev,
                      outSize_dev, mismatchHost, (cudaStream_t)stream);
 }
 
@@ -315,11 +418,11 @@ int dgb_ans_decode_stride(void* temp, size_t tempBytes, int pb, int useChecksum,
                           uint32_t outCapacity, uint8_t* outSuccess_dev, uint32_t* outSize_dev,
                           uint8_t* mismatchHost, void* stream) {
   if (n && !in_dev) return DGB_ERR_INVALID_ARG;
-  std::vector<HostMember> v(n);
+  HostMember* v = stageMembers(n);
   for (uint32_t i = 0; i < n; ++i)
     v[i] = HostMember{static_cast<const uint8_t*>(in_dev) + (size_t)i * inStride,
                       static_cast<uint8_t*>(out_dev) + (size_t)i * outStride, outCapacity};
-  return decodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v.data(), outSuccess_dev,
+  return decodeBatch(kKindBytes, temp, tempBytes, pb, useChecksum != 0, n, v, outSuccess_dev,
                      outSize_dev, mismatchHost, (cudaStream_t)stream);
 }
 

@@ -8,6 +8,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+#include <vector>
+
 #include "../../include/dietgpu_b200.h"
 
 namespace dgb {
@@ -137,24 +140,89 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
 
 void setLastCudaError(cudaError_t e);
 
-// Per-kernel timing (options().timing): slots are stable indices reported by
+inline uint32_t wordBytes(int kind) { return kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u); }
+inline size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
+int smCount();  // SMs of the current device, cached per device
+
+// Resident CTAs per SM of `kernel` with `threads` threads and `smemBytes` of dynamic shared memory, into
+// *out.  The kernel's dynamic shared-memory limit is raised to `maxDynamicSmem` once per (kernel, device);
+// with out == nullptr that is all it does.  Cached per host thread: once warm it makes no CUDA call
+// beyond cudaGetDevice and allocates nothing.
+int residentCtasPerSm(const void* kernel, int threads, size_t smemBytes, int maxDynamicSmem, int* out);
+
+// Per-thread host staging of the codec calls, reused: no allocation on the steady-state call path.
+// The uploaded member tables have a buffer per direction: a CUDA graph that captured an encode and a
+// decode copies from both host buffers again at every replay.
+struct HostStage {
+  std::vector<HostMember> members;      // the entry point's member list (capi.cu)
+  std::vector<uint8_t> encodeUpload;    // encoder member table + work index, uploaded in one copy
+  std::vector<MemberDesc> decodeTable;  // decoder member table
+  std::vector<uint32_t> checksum;       // decoder checksum pass: computed, stored and decoded size per member
+};
+HostStage& hostStage();
+
+// Per-kernel timing (Options::timing of the call): slots are stable indices reported by
 // dgb_kernel_times().  No-ops when timing is off.
 enum TimerSlot : int { kSlotStats = 0, kSlotEncode = 1, kSlotPlan = 2, kSlotDecode = 3, kSlotChecksum = 4, kSlotFused = 5, kSlotPull = 6, kNumSlots = 7 };
-// Internal helper streams: a large batch is cut into up to kMaxParts contiguous sub-batches whose
-// kernels run on separate streams (forked from / joined to the caller's stream with events), so the
-// HBM-bound and the issue-bound kernels of different sub-batches overlap and launch gaps hide.
-constexpr int kMaxParts = 8;
-struct StreamPool {
-  cudaStream_t s[kMaxParts];
-  cudaEvent_t start, done[kMaxParts];
-};
-int streamPool(StreamPool** out);  // lazily created; DGB_OK or DGB_ERR_CUDA
-// cuts members [0,n) into `parts` contiguous ranges of roughly equal `weight`; bounds has parts+1 entries
-void splitParts(const uint64_t* weight, uint32_t n, int parts, uint32_t* bounds);
-int autoParts(int kind, uint32_t n, uint64_t totalBytes, bool decode);
+void timerBegin(const Options& opt, int slot, cudaStream_t stream);
+void timerEnd(const Options& opt, int slot, cudaStream_t stream);
 
-void timerBegin(int slot, cudaStream_t stream);
-void timerEnd(int slot, cudaStream_t stream);
+// Sub-batches of one call: a large batch is cut into up to kMaxParts contiguous member ranges of
+// roughly equal bytes whose kernels run on internal streams forked from the caller's stream, so the
+// HBM-bound and the issue-bound kernels of different sub-batches overlap and launch gaps hide.  The
+// destructor joins every forked stream back to the caller's stream, on every exit path: the caller
+// frees / reuses its scratch when the call returns, so work queued on a helper stream must be ordered
+// before whatever it enqueues next -- also when a later launch of the same call failed.
+constexpr int kMaxParts = 8;
+struct StreamPool;
+class SubBatches {
+ public:
+  // `split` false: one sub-batch on the caller's stream
+  SubBatches(int kind, const MemberDesc* members, uint32_t n, const Options& opt, bool split, cudaStream_t stream);
+  ~SubBatches();
+  SubBatches(const SubBatches&) = delete;
+  SubBatches& operator=(const SubBatches&) = delete;
+  int fork();  // records the fork point on the caller's stream (nothing to do for one sub-batch)
+  int count() const { return parts_; }
+  uint32_t begin(int k) const { return bounds_[k]; }
+  uint32_t end(int k) const { return bounds_[k + 1]; }
+  int stream(int k, cudaStream_t* out);  // the stream of sub-batch k, forked on first use
+
+ private:
+  int parts_;
+  uint32_t bounds_[kMaxParts + 1];
+  cudaStream_t stream_;
+  StreamPool* pool_ = nullptr;
+  bool forked_[kMaxParts] = {};
+};
+
+// Runtime data kind / probBits / flag turned into a template argument: f(std::integral_constant)
+// with the matching value (read it as decltype(arg)::value).
+template <int V>
+using IntC = std::integral_constant<int, V>;
+template <class F>
+int withKind(int kind, F&& f) {
+  switch (kind) {
+    case kKindBytes: return f(IntC<kKindBytes>{});
+    case kKindF16: return f(IntC<kKindF16>{});
+    case kKindBF16: return f(IntC<kKindBF16>{});
+    case kKindF32: return f(IntC<kKindF32>{});
+    default: return DGB_ERR_INVALID_ARG;
+  }
+}
+template <class F>
+int withPb(int pb, F&& f) {
+  switch (pb) {
+    case 9: return f(IntC<9>{});
+    case 10: return f(IntC<10>{});
+    case 11: return f(IntC<11>{});
+    default: return DGB_ERR_INVALID_ARG;
+  }
+}
+template <class F>
+int withBool(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
+}
 
 #define DGB_CUDA_TRY(expr)                    \
   do {                                        \
@@ -221,6 +289,28 @@ __device__ __forceinline__ void bulkLoad(uint32_t dstSmem, const void* src, uint
           "r"(dstSmem),
       "l"(src), "r"(bytes), "r"(bar)
       : "memory");
+}
+
+// ---- cp.async (LDGSTS) 16 B copies and shared-memory loads at a constant offset ----
+__device__ __forceinline__ void cpAsync16(uint32_t dstSmem, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dstSmem), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cpAsyncWait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+template <int OFF>
+__device__ __forceinline__ uint32_t ldsU8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
+  return v;
+}
+template <int OFF>
+__device__ __forceinline__ uint32_t ldsU16(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u16 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
+  return v;
 }
 // block-wide exclusive scan of one value per thread for THREADS threads
 // (THREADS multiple of 32, <= 1024).  `warpSums` is smem of THREADS/32 words.

@@ -131,27 +131,6 @@ planKernel(DecodeScratch sc, uint32_t m0, uint32_t m1, uint32_t part, int pb,
 constexpr int kGroupRows = DGB_DEC_GROUP_ROWS;  // rows per prefetch group (8 or 16)
 constexpr uint32_t kRingSlots = 3;              // groups resident per warp: current + 2 in flight
 
-__device__ __forceinline__ void cpAsync16(uint32_t dstSmem, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dstSmem), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cpAsyncWait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-template <int OFF>
-__device__ __forceinline__ uint32_t ldsU8(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
-  return v;
-}
-template <int OFF>
-__device__ __forceinline__ uint32_t ldsU16(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u16 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
-  return v;
-}
-
 template <int KIND>
 struct RowWriter;
 
@@ -765,8 +744,6 @@ checksumKernel(DecodeScratch sc) {
   if ((threadIdx.x & 31) == 0 && x) atomicXor(sc.checksum + m, x & 0xffu);
 }
 
-size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
-
 struct DecodePlan {
   size_t members, next, totals, checksum, archiveChecksum, sizes, total;
 };
@@ -784,160 +761,67 @@ DecodePlan planDecodeScratch(uint32_t n) {
   return p;
 }
 
-int smCountD() {
-  // per device (a process may drive several); racing first calls write the same value
-  static int cached[64] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-  if (!cached[dev]) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = v > 0 ? v : 132;
-  }
-  return cached[dev];
+// Staging slot per warp (u16 words) and dynamic shared memory of a decoder CTA of `warps` warps.  The slot
+// covers the worst case for raw bytes; float kinds code exponent-like bytes that compress well, so a
+// smaller slot (more resident warps) covers them and rare larger blocks take the direct-from-global path
+// inside the kernel.
+template <int KIND, int PB>
+size_t decoderSmem(int warps, const Options& opt, uint32_t* slotWords) {
+  uint32_t slot = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words : (KIND == kKindBytes ? maxBlockWords(PB) : 1536u);
+  slot = std::min(roundUp(slot, 8u), maxBlockWords(PB));
+  *slotWords = slot;
+  return (2 * kNumSymbols + 64) * 4 + ((warps + 1) & ~1) * 8 + (size_t)warps * kRingSlots * RowWriter<KIND>::kRingSlotBytes +
+         (size_t)warps * (128u + slot * 2u);
 }
 
-template <int KIND, int PB, int WARPS, bool STAGE, bool LUT64>
-int launchDecode(const DecodeScratch& sc, uint32_t m0, uint32_t m1, uint32_t part, uint64_t blockBound,
-                 cudaStream_t stream) {
-  auto kern = decodeKernel<KIND, PB, WARPS, STAGE, LUT64>;
-  const Options& opt = options();
-  // staging slot per warp: worst case for raw bytes; float kinds code exponent-like bytes that
-  // compress well, so a smaller slot (more resident warps) covers them and rare larger blocks
-  // take the direct-from-global path inside the kernel
-  uint32_t slotWords = 0;
-  if (STAGE) {
-    slotWords = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words
-                                          : (KIND == kKindBytes ? maxBlockWords(PB) : 1536u);
-    slotWords = std::min(roundUp(slotWords, 8u), maxBlockWords(PB));
-  }
-  size_t smemBytes = (2 * kNumSymbols + 64) * 4 + ((WARPS + 1) & ~1) * 8 +
-                     (size_t)WARPS * kRingSlots * RowWriter<KIND>::kRingSlotBytes;
-  if (STAGE) smemBytes += (size_t)WARPS * (128u + slotWords * 2u);
-  // per instantiation and host thread; re-done when the thread's current device changes (function
-  // attributes are per device)
-  static thread_local int perSm = 0;
-  static thread_local size_t perSmKey = 0;
-  int devOrdinal = 0;
-  DGB_CUDA_TRY(cudaGetDevice(&devOrdinal));
-  const size_t occKey = smemBytes | ((size_t)(devOrdinal + 1) << 40);
-  if (perSm == 0 || perSmKey != occKey) {
-    DGB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    int occ = 0;
-    DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WARPS * 32, smemBytes));
-    perSm = std::max(occ, 1);
-    perSmKey = occKey;
-  }
+// Two-kernel path (option decode_fused=0) for members [m0, m1): planKernel, then decodeKernel.  One
+// decoder variant is shipped per (kind, probBits): 8 warps per CTA, TMA-staged streams, 4-byte LUT
+// entries (4 warps, direct-from-global streams and 8-byte LUT entries are not instantiated).
+template <int KIND, int PB>
+int launchPlanDecode(const Options& opt, const DecodeScratch& sc, bool checksum, uint32_t m0, uint32_t m1, uint32_t part,
+                     uint64_t blockBound, uint8_t* outSuccess, uint32_t* outSize, cudaStream_t stream) {
+  timerBegin(opt, kSlotPlan, stream);
+  planKernel<KIND><<<1, 1024, 0, stream>>>(sc, m0, m1, part, PB, outSuccess, outSize, checksum);
+  DGB_CUDA_TRY(cudaGetLastError());
+  timerEnd(opt, kSlotPlan, stream);
+
+  constexpr int kWarps = 8;
+  auto kern = decodeKernel<KIND, PB, kWarps, true, false>;
+  uint32_t slotWords;
+  const size_t smemBytes = decoderSmem<KIND, PB>(kWarps, opt, &slotWords);
+  int perSm = 1;
+  const int rc = residentCtasPerSm((const void*)kern, kWarps * 32, smemBytes, 160 * 1024, &perSm);
+  if (rc != DGB_OK) return rc;
   // one resident wave; every warp gets the same number of blocks (rounds) when the batch is
   // large, so no warp idles at the CTA barrier waiting for a neighbour's extra block
-  const uint64_t resident = (uint64_t)perSm * smCountD();
-  const uint64_t rounds = std::max<uint64_t>(1, (blockBound + resident * WARPS - 1) / (resident * WARPS));
-  const uint64_t want = (blockBound + WARPS * rounds - 1) / (WARPS * rounds);
+  const uint64_t resident = (uint64_t)perSm * smCount();
+  const uint64_t rounds = std::max<uint64_t>(1, (blockBound + resident * kWarps - 1) / (resident * kWarps));
+  const uint64_t want = (blockBound + kWarps * rounds - 1) / (kWarps * rounds);
   const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, resident));
-  timerBegin(kSlotDecode, stream);
-  kern<<<grid, WARPS * 32, smemBytes, stream>>>(sc, m0, m1, part, slotWords);
+  timerBegin(opt, kSlotDecode, stream);
+  kern<<<grid, kWarps * 32, smemBytes, stream>>>(sc, m0, m1, part, slotWords);
   DGB_CUDA_TRY(cudaGetLastError());
-  timerEnd(kSlotDecode, stream);
+  timerEnd(opt, kSlotDecode, stream);
   return DGB_OK;
 }
 
-// One variant is shipped per (kind, probBits): 8 warps per CTA, TMA-staged streams, 4-byte LUT
-// entries.  The alternatives (4 warps, direct-from-global streams, 8-byte LUT entries) are no longer
-// instantiated: this two-kernel path is kept behind option decode_fused=0 only.
-template <int KIND, int PB>
-int launchDecodeW(const DecodeScratch& sc, uint32_t m0, uint32_t m1, uint32_t part, uint64_t blockBound,
-                  cudaStream_t stream) {
-  return launchDecode<KIND, PB, 8, true, false>(sc, m0, m1, part, blockBound, stream);
-}
-
-// member table of the call in flight on this thread (decodeBatch fills it; count == 0: table in scratch)
-InlineMembers& decodeInline() {
-  static thread_local InlineMembers im;
-  return im;
-}
-
+// Single-launch decoder (the default) with WARPS warps per CTA.
 template <int KIND, int PB, int WARPS>
-int launchDecodeFusedW(const DecodeScratch& sc, uint32_t n, uint64_t totalChunks,
-                       uint32_t slotWordsOpt, uint8_t* outSuccess, uint32_t* outSize, bool checksum,
-                       cudaStream_t stream) {
+int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineMembers& im, uint32_t n,
+                      uint64_t totalChunks, uint8_t* outSuccess, uint32_t* outSize, bool checksum, cudaStream_t stream) {
   auto kern = decodeFusedKernel<KIND, PB, WARPS>;
-  // staging slot per warp: worst case for raw bytes; float kinds code exponent-like bytes that
-  // compress well, so a smaller slot (more resident warps) covers them and rare larger blocks
-  // take the direct-from-global path inside the kernel
-  uint32_t slotWords = slotWordsOpt > 0 ? slotWordsOpt : (KIND == kKindBytes ? maxBlockWords(PB) : 1536u);
-  slotWords = std::min(roundUp(slotWords, 8u), maxBlockWords(PB));
-  const size_t smemBytes = (2 * kNumSymbols + 64) * 4 + ((WARPS + 1) & ~1) * 8 +
-                           (size_t)WARPS * kRingSlots * RowWriter<KIND>::kRingSlotBytes +
-                           (size_t)WARPS * (128u + slotWords * 2u);
-  static thread_local int perSm = 0;
-  static thread_local size_t perSmKey = 0;
-  int devOrdinal = 0;
-  DGB_CUDA_TRY(cudaGetDevice(&devOrdinal));
-  const size_t occKey = smemBytes | ((size_t)(devOrdinal + 1) << 40);
-  if (perSm == 0 || perSmKey != occKey) {
-    DGB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    int occ = 0;
-    DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WARPS * 32, smemBytes));
-    perSm = std::max(occ, 1);
-    perSmKey = occKey;
-  }
-  const uint64_t resident = (uint64_t)perSm * smCountD();
+  uint32_t slotWords;
+  const size_t smemBytes = decoderSmem<KIND, PB>(WARPS, opt, &slotWords);
+  int perSm = 1;
+  const int rc = residentCtasPerSm((const void*)kern, WARPS * 32, smemBytes, 160 * 1024, &perSm);
+  if (rc != DGB_OK) return rc;
+  const uint64_t resident = (uint64_t)perSm * smCount();
   const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(resident, totalChunks));
-  timerBegin(kSlotDecode, stream);
-  kern<<<grid, WARPS * 32, smemBytes, stream>>>(sc, decodeInline(), n, slotWords, outSuccess, outSize, checksum);
+  timerBegin(opt, kSlotDecode, stream);
+  kern<<<grid, WARPS * 32, smemBytes, stream>>>(sc, im, n, slotWords, outSuccess, outSize, checksum);
   DGB_CUDA_TRY(cudaGetLastError());
-  timerEnd(kSlotDecode, stream);
+  timerEnd(opt, kSlotDecode, stream);
   return DGB_OK;
-}
-
-template <int KIND, int PB>
-int launchDecodeFused(const DecodeScratch& sc, uint32_t n, uint64_t totalChunks,
-                      uint32_t slotWordsOpt, uint8_t* outSuccess, uint32_t* outSize, bool checksum,
-                      cudaStream_t stream) {
-  // warps per CTA = warps that share one LUT and meet at the barrier when a lease ends.  Float kinds: 8 (4 is
-  // equal: c3 decode 190 us either way on an H100 at 700 W, tools/walltime.py).  Byte archives need the worst-case
-  // staging slot (5.1 KiB per warp), which caps 8-warp CTAs at 32 resident warps per SM; 20-warp CTAs reach 40
-  // (same H100: c2 decode 249 us against 271 with 8 warps) -- used when the members are long enough to keep 20
-  // warps busy through a lease.
-  int w = options().decode_warps;
-  // (at 11 bits the LUT is 8 KiB and the slot 5.6 KiB per warp: a 20-warp CTA needs 126 KiB and fits once per
-  // SM and gains nothing -- c2p11 decode 248 us with 20 or 8 warps on the same H100 -- so the wide CTA is used
-  // up to 10 bits only)
-  if (w == 0) w = (KIND == kKindBytes && PB <= 10 && totalChunks * 8u >= 160ull * n) ? 20 : 8;
-  if (w == 4)
-    return launchDecodeFusedW<KIND, PB, 4>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-  if constexpr (KIND == kKindBytes) {
-    if (w == 20)
-      return launchDecodeFusedW<KIND, PB, 20>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-  }
-  return launchDecodeFusedW<KIND, PB, 8>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-}
-
-template <int KIND>
-int decodeFusedKind(const DecodeScratch& sc, int pb, uint32_t n, uint64_t totalChunks,
-                    uint32_t slotWordsOpt, uint8_t* outSuccess, uint32_t* outSize, bool checksum,
-                    cudaStream_t stream) {
-  switch (pb) {
-    case 9: return launchDecodeFused<KIND, 9>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-    case 10: return launchDecodeFused<KIND, 10>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-    case 11: return launchDecodeFused<KIND, 11>(sc, n, totalChunks, slotWordsOpt, outSuccess, outSize, checksum, stream);
-    default: return DGB_ERR_INVALID_ARG;
-  }
-}
-
-template <int KIND>
-int decodeKind(const DecodeScratch& sc, int pb, bool checksum, uint32_t m0, uint32_t m1, uint32_t part,
-               uint64_t blockBound, uint8_t* outSuccess, uint32_t* outSize, cudaStream_t stream) {
-  timerBegin(kSlotPlan, stream);
-  planKernel<KIND><<<1, 1024, 0, stream>>>(sc, m0, m1, part, pb, outSuccess, outSize, checksum);
-  DGB_CUDA_TRY(cudaGetLastError());
-  timerEnd(kSlotPlan, stream);
-  switch (pb) {
-    case 9: return launchDecodeW<KIND, 9>(sc, m0, m1, part, blockBound, stream);
-    case 10: return launchDecodeW<KIND, 10>(sc, m0, m1, part, blockBound, stream);
-    case 11: return launchDecodeW<KIND, 11>(sc, m0, m1, part, blockBound, stream);
-    default: return DGB_ERR_INVALID_ARG;
-  }
 }
 
 }  // namespace
@@ -955,17 +839,16 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 
   const Options opt = options();  // one snapshot per call
   const bool fused = opt.decode_fused != 0;
-  static thread_local std::vector<MemberDesc> descStage;  // reused: no allocation on the steady-state path
-  static thread_local std::vector<uint64_t> weightStage;
-  descStage.resize(n);
-  MemberDesc* desc = descStage.data();
-  const uint32_t wordBytes = kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u);
+  HostStage& hs = hostStage();
+  hs.decodeTable.resize(n);
+  MemberDesc* desc = hs.decodeTable.data();
+  const uint32_t elemBytes = wordBytes(kind);
   uint64_t totalChunks = 0;
   for (uint32_t i = 0; i < n; ++i) {
     if (!members[i].in || (members[i].size && !members[i].out)) return DGB_ERR_INVALID_ARG;
     // headers are read as 16 B vectors; the reference imposes the same alignment
     if (reinterpret_cast<uintptr_t>(members[i].in) & 15u) return DGB_ERR_INVALID_ARG;
-    if (reinterpret_cast<uintptr_t>(members[i].out) & (wordBytes - 1u)) return DGB_ERR_INVALID_ARG;
+    if (reinterpret_cast<uintptr_t>(members[i].out) & (elemBytes - 1u)) return DGB_ERR_INVALID_ARG;
     desc[i].in = members[i].in;
     desc[i].out = members[i].out;
     desc[i].size = members[i].size;  // capacity
@@ -984,7 +867,7 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   sc.archiveChecksum = reinterpret_cast<uint32_t*>(base + dp.archiveChecksum);
   sc.sizes = reinterpret_cast<uint32_t*>(base + dp.sizes);
   // member table: inside the kernel parameters when it fits (the checksum pass reads it from scratch)
-  InlineMembers& im = decodeInline();
+  static thread_local InlineMembers im;
   const bool inlined = opt.inline_members != 0 && fused && !checksum && n <= kInlineMembers;
   im.count = inlined ? n : 0u;
   if (inlined) {
@@ -996,80 +879,65 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 
   if (fused) {
     DGB_CUDA_TRY(cudaMemsetAsync(sc.next, 0, 8 * (size_t)n, stream));
-    const uint32_t slotOpt = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words : 0u;
-    int rc;
-    switch (kind) {
-      case kKindBytes: rc = decodeFusedKind<kKindBytes>(sc, pb, n, totalChunks, slotOpt, outSuccess_dev, outSize_dev, checksum, stream); break;
-      case kKindF16: rc = decodeFusedKind<kKindF16>(sc, pb, n, totalChunks, slotOpt, outSuccess_dev, outSize_dev, checksum, stream); break;
-      case kKindBF16: rc = decodeFusedKind<kKindBF16>(sc, pb, n, totalChunks, slotOpt, outSuccess_dev, outSize_dev, checksum, stream); break;
-      case kKindF32: rc = decodeFusedKind<kKindF32>(sc, pb, n, totalChunks, slotOpt, outSuccess_dev, outSize_dev, checksum, stream); break;
-      default: return DGB_ERR_INVALID_ARG;
-    }
+    const int rc = withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
+      constexpr int KIND = decltype(K)::value, PB = decltype(P)::value;
+      // warps per CTA = warps that share one LUT and meet at the barrier when a lease ends.  Float kinds: 8 (4 is
+      // equal: c3 decode 190 us either way on an H100 at 700 W, tools/walltime.py).  Byte archives need the worst-case
+      // staging slot (5.1 KiB per warp), which caps 8-warp CTAs at 32 resident warps per SM; 20-warp CTAs reach 40
+      // (same H100: c2 decode 249 us against 271 with 8 warps) -- used when the members are long enough to keep 20
+      // warps busy through a lease.
+      int w = opt.decode_warps;
+      // (at 11 bits the LUT is 8 KiB and the slot 5.6 KiB per warp: a 20-warp CTA needs 126 KiB and fits once per
+      // SM and gains nothing -- c2p11 decode 248 us with 20 or 8 warps on the same H100 -- so the wide CTA is used
+      // up to 10 bits only)
+      if (w == 0) w = (KIND == kKindBytes && PB <= 10 && totalChunks * 8u >= 160ull * n) ? 20 : 8;
+      if (w == 4) return launchDecodeFused<KIND, PB, 4>(opt, sc, im, n, totalChunks, outSuccess_dev, outSize_dev, checksum, stream);
+      if constexpr (KIND == kKindBytes) {
+        if (w == 20)
+          return launchDecodeFused<KIND, PB, 20>(opt, sc, im, n, totalChunks, outSuccess_dev, outSize_dev, checksum, stream);
+      }
+      return launchDecodeFused<KIND, PB, 8>(opt, sc, im, n, totalChunks, outSuccess_dev, outSize_dev, checksum, stream);
+    }); });
     if (rc != DGB_OK) return rc;
   } else {
     // two-kernel path: sub-batches on internal streams: the plan kernel (pure latency) of one part
     // hides behind the decode kernel of another, and the tail of one decode kernel overlaps the next
-    weightStage.resize(n);
-    uint64_t totalBytes = 0;
-    for (uint32_t i = 0; i < n; ++i) { weightStage[i] = (uint64_t)desc[i].size * wordBytes; totalBytes += weightStage[i]; }
-    const int parts = autoParts(kind, n, totalBytes, true);
-    uint32_t bounds[kMaxParts + 1];
-    splitParts(weightStage.data(), n, parts, bounds);
-    // joins the helper streams on every exit path (the caller reuses its scratch on return)
-    struct Join {
-      StreamPool* pool = nullptr;
-      cudaStream_t stream = nullptr;
-      bool forked[kMaxParts] = {};
-      ~Join() {
-        if (!pool) return;
-        for (int k = 0; k < kMaxParts; ++k)
-          if (forked[k] && cudaEventRecord(pool->done[k], pool->s[k]) == cudaSuccess) cudaStreamWaitEvent(stream, pool->done[k], 0);
+    SubBatches parts(kind, desc, n, opt, true, stream);
+    if (const int rc = parts.fork(); rc != DGB_OK) return rc;
+    const int rc = withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
+      for (int part = 0; part < parts.count(); ++part) {
+        const uint32_t m0 = parts.begin(part), m1 = parts.end(part);
+        if (m1 == m0) continue;
+        cudaStream_t ps;
+        int prc = parts.stream(part, &ps);
+        if (prc != DGB_OK) return prc;
+        uint64_t partBound = 0;
+        for (uint32_t i = m0; i < m1; ++i) partBound += divUp(desc[i].size, kBlockBytes);
+        prc = launchPlanDecode<decltype(K)::value, decltype(P)::value>(opt, sc, checksum, m0, m1, part, partBound,
+                                                                      outSuccess_dev, outSize_dev, ps);
+        if (prc != DGB_OK) return prc;
       }
-    } join;
-    StreamPool* pool = nullptr;
-    if (parts > 1) {
-      int prc = streamPool(&pool);
-      if (prc != DGB_OK) return prc;
-      DGB_CUDA_TRY(cudaEventRecord(pool->start, stream));
-      join.pool = pool;
-      join.stream = stream;
-    }
-    for (int part = 0; part < parts; ++part) {
-      const uint32_t m0 = bounds[part], m1 = bounds[part + 1];
-      if (m1 == m0) continue;
-      cudaStream_t ps = stream;
-      if (parts > 1) {
-        ps = pool->s[part];
-        DGB_CUDA_TRY(cudaStreamWaitEvent(ps, pool->start, 0));
-        join.forked[part] = true;
-      }
-      uint64_t partBound = 0;
-      for (uint32_t i = m0; i < m1; ++i) partBound += divUp(desc[i].size, kBlockBytes);
-      int rc;
-      switch (kind) {
-        case kKindBytes: rc = decodeKind<kKindBytes>(sc, pb, checksum, m0, m1, part, partBound, outSuccess_dev, outSize_dev, ps); break;
-        case kKindF16: rc = decodeKind<kKindF16>(sc, pb, checksum, m0, m1, part, partBound, outSuccess_dev, outSize_dev, ps); break;
-        case kKindBF16: rc = decodeKind<kKindBF16>(sc, pb, checksum, m0, m1, part, partBound, outSuccess_dev, outSize_dev, ps); break;
-        case kKindF32: rc = decodeKind<kKindF32>(sc, pb, checksum, m0, m1, part, partBound, outSuccess_dev, outSize_dev, ps); break;
-        default: return DGB_ERR_INVALID_ARG;
-      }
-      if (rc != DGB_OK) return rc;
-    }
-  }  // ~Join orders the helper streams before the caller's stream
+      return DGB_OK;
+    }); });
+    if (rc != DGB_OK) return rc;
+  }  // ~SubBatches orders the helper streams before the caller's stream
 
   if (checksum) {
     // ans/GpuANSDecode.cuh:555-591 / float/GpuFloatDecompress.cuh:698-733: checksum the
     // output, compare with the archive's on the host (this path synchronises).
     // Float kinds: the checksum covers the first `size` BYTES (SURVEY A.6/B6); sc.sizes holds
     // the word count, which is exactly that byte count.
-    const int sms = smCountD();
+    const int sms = smCount();
     dim3 grid(n, std::max(1, std::min(64, 4 * sms / (int)std::max(1u, n))));
     checksumKernel<<<grid, 256, 0, stream>>>(sc);
     DGB_CUDA_TRY(cudaGetLastError());
-    std::vector<uint32_t> got(n), want(n), sizes(n);
-    DGB_CUDA_TRY(cudaMemcpyAsync(got.data(), sc.checksum, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
-    DGB_CUDA_TRY(cudaMemcpyAsync(want.data(), sc.archiveChecksum, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
-    DGB_CUDA_TRY(cudaMemcpyAsync(sizes.data(), sc.sizes, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
+    hs.checksum.resize(3 * (size_t)n);
+    uint32_t* got = hs.checksum.data();
+    uint32_t* want = got + n;
+    uint32_t* sizes = want + n;
+    DGB_CUDA_TRY(cudaMemcpyAsync(got, sc.checksum, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
+    DGB_CUDA_TRY(cudaMemcpyAsync(want, sc.archiveChecksum, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
+    DGB_CUDA_TRY(cudaMemcpyAsync(sizes, sc.sizes, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream));
     DGB_CUDA_TRY(cudaStreamSynchronize(stream));
     bool bad = false;
     for (uint32_t i = 0; i < n; ++i) {
@@ -1177,7 +1045,8 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
                  uint32_t* outBytes_dev, cudaStream_t stream) {
   if (n == 0) return DGB_OK;
   if (!src || !dst || !capacity) return DGB_ERR_INVALID_ARG;
-  const int ctas = std::max(1, options().pull_ctas);
+  const Options opt = options();  // one snapshot per call
+  const int ctas = std::max(1, opt.pull_ctas);
   static thread_local InlineMembers im;
   for (uint32_t i0 = 0; i0 < n; i0 += kInlineMembers) {
     const uint32_t k = std::min(kInlineMembers, n - i0);
@@ -1190,10 +1059,10 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
       im.m[i].size = capacity[i0 + i];
       im.m[i].work0 = 0;
     }
-    timerBegin(kSlotPull, stream);
+    timerBegin(opt, kSlotPull, stream);
     pullArchivesKernel<<<ctas, kPullThreads, 0, stream>>>(im, kind, outBytes_dev ? outBytes_dev + i0 : nullptr);
     DGB_CUDA_TRY(cudaGetLastError());
-    timerEnd(kSlotPull, stream);
+    timerEnd(opt, kSlotPull, stream);
   }
   return DGB_OK;
 }

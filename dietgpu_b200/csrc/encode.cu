@@ -518,21 +518,6 @@ statsFloatStagedKernel(EncodeScratch sc, int pb, bool useChecksum, uint32_t slab
 #endif
 constexpr int kEncGroupRows = DGB_ENC_GROUP_ROWS;  // rows per cp.async group
 
-__device__ __forceinline__ void cpAsync16(uint32_t dstSmem, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dstSmem), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cpAsyncWait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-template <int OFF>
-__device__ __forceinline__ uint32_t ldsU8(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
-  return v;
-}
-
 // ---------------------------------------------------------------------------
 // Input side of the coder, per data kind.  The coder reads the member's RAW words (bytes, or the
 // fp16 / bf16 / fp32 words themselves): for float kinds it takes the coded byte out of each word on
@@ -1440,21 +1425,6 @@ encodeFusedKernel(EncodeScratch sc, const uint32_t* __restrict__ histogramGiven,
   }
 }
 
-size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
-
-int smCount() {
-  // per device (a process may drive several); racing first calls write the same value
-  static int cached[64] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-  if (!cached[dev]) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = v > 0 ? v : 132;
-  }
-  return cached[dev];
-}
-
 struct ScratchPlan {
   size_t members, workIdx, uploadEnd, zeroBegin, hist, histDone, checksum, ticket, allocDone, ready, zeroEnd, lookback,
       lookbackEnd, table, spill, total;
@@ -1499,114 +1469,6 @@ ScratchPlan planScratch(int kind, uint32_t n, uint32_t maxSize, uint32_t totalTi
 
 uint32_t ticketsFor(uint32_t size) { return divUp(size, kBlockBytes); }
 
-// Joins the internal streams on every exit path: the caller frees / reuses its scratch when the
-// call returns, so work already queued on a helper stream must be ordered before whatever the
-// caller enqueues next on its own stream -- also when a later launch of the same call failed.
-struct ForkGuard {
-  StreamPool* pool = nullptr;
-  cudaStream_t stream = nullptr;
-  bool forked[kMaxParts] = {};
-  ~ForkGuard() {
-    if (!pool) return;
-    for (int k = 0; k < kMaxParts; ++k) {
-      if (!forked[k]) continue;
-      if (cudaEventRecord(pool->done[k], pool->s[k]) == cudaSuccess) cudaStreamWaitEvent(stream, pool->done[k], 0);
-    }
-  }
-};
-
-// per-thread reusable host staging (no allocation on the steady-state call path)
-struct HostStage {
-  std::vector<uint8_t> upload;
-  std::vector<uint64_t> weight;
-};
-HostStage& hostStage() {
-  static thread_local HostStage h;
-  return h;
-}
-
-template <int KIND, bool WIDE, bool STAGED>
-int launchFused(const EncodeScratch& sc, const uint32_t* histogram_dev, int pb, bool checksum, uint32_t n,
-                uint32_t totalItems, uint32_t totalChunks, uint32_t slabVecs, uint32_t chunkBlocks,
-                uint32_t slotWords, uint32_t statsEvery, uint32_t spillWarps, uint32_t* outSize_dev,
-                cudaStream_t stream) {
-  auto kern = encodeFusedKernel<KIND, WIDE, STAGED>;
-  constexpr uint32_t W = kStatsThreads / 32;
-  const size_t smemBytes = (size_t)W * encFastWarpSmem(slotWords, KIND);
-  static thread_local int perSm = 0;
-  static thread_local size_t perSmKey = 0;
-  int devOrdinal = 0;
-  DGB_CUDA_TRY(cudaGetDevice(&devOrdinal));
-  const size_t occKey = smemBytes | ((size_t)(devOrdinal + 1) << 40);
-  if (perSm == 0 || perSmKey != occKey) {
-    DGB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-    int occ = 0;
-    DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)kStatsThreads, smemBytes));
-    perSm = std::max(occ, 1);
-    perSmKey = occKey;
-  }
-  uint64_t grid = (uint64_t)perSm * (uint64_t)smCount();
-  grid = std::min<uint64_t>(grid, (uint64_t)totalItems + totalChunks);
-  grid = std::min<uint64_t>(grid, spillWarps / W);  // every warp owns a spill slot
-  grid = std::max<uint64_t>(grid, 1);
-  timerBegin(kSlotFused, stream);
-  kern<<<(uint32_t)grid, kStatsThreads, smemBytes, stream>>>(sc, histogram_dev, pb, checksum, n, totalItems, totalChunks,
-                                                             slabVecs, chunkBlocks, slotWords, statsEvery, outSize_dev);
-  DGB_CUDA_TRY(cudaGetLastError());
-  timerEnd(kSlotFused, stream);
-  return DGB_OK;
-}
-
-// K2 of the two-kernel path for one data kind: variant 0 = canonical (ordered, packed table),
-// 1 = fast + packed table, 2 = fast + wide table.  Launch attributes and occupancy are cached per
-// host thread and (variant, shared-memory size, device).
-template <int KIND>
-struct K2Launcher {
-  static int residentPerSm(int variant, uint32_t W, size_t smemBytes, int* out) {
-    static thread_local size_t keySmem = 0;
-    static thread_local uint32_t keyW = 0;
-    static thread_local int keyVariant = -1, keyDev = -1, perSm = 1;
-    int dev = 0;
-    DGB_CUDA_TRY(cudaGetDevice(&dev));
-    if (keySmem != smemBytes || keyW != W || keyVariant != variant || keyDev != dev) {
-      int occ = 0;
-      if (variant == 0) {
-        DGB_CUDA_TRY(cudaFuncSetAttribute(encodeKernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-        DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, encodeKernel<KIND>, (int)(W * 32), smemBytes));
-      } else if (variant == 1) {
-        DGB_CUDA_TRY(cudaFuncSetAttribute(encodeKernelFast<false, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-        DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, encodeKernelFast<false, KIND>, (int)(W * 32), smemBytes));
-      } else {
-        DGB_CUDA_TRY(cudaFuncSetAttribute(encodeKernelFast<true, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-        DGB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, encodeKernelFast<true, KIND>, (int)(W * 32), smemBytes));
-      }
-      perSm = std::max(occ, 1);
-      keySmem = smemBytes; keyW = W; keyVariant = variant; keyDev = dev;
-    }
-    *out = perSm;
-    return DGB_OK;
-  }
-  static void launch(int variant, uint32_t grid, uint32_t W, size_t smemBytes, cudaStream_t ps, const EncodeScratch& sc,
-                     const InlineMembers& im, int pb, bool checksum, uint32_t n, uint32_t totalTickets, uint32_t blockBegin, uint32_t blockEnd,
-                     uint32_t slotWords, uint32_t spillWarpBase, uint32_t* outSize_dev) {
-    if (variant == 0) {
-      encodeKernel<KIND><<<grid, W * 32, smemBytes, ps>>>(sc, pb, checksum, n, totalTickets, outSize_dev);
-    } else if (variant == 1) {
-      encodeKernelFast<false, KIND><<<grid, W * 32, smemBytes, ps>>>(sc, im, pb, checksum, n, blockBegin, blockEnd, slotWords,
-                                                                    spillWarpBase, outSize_dev);
-    } else {
-      encodeKernelFast<true, KIND><<<grid, W * 32, smemBytes, ps>>>(sc, im, pb, checksum, n, blockBegin, blockEnd, slotWords,
-                                                                   spillWarpBase, outSize_dev);
-    }
-  }
-};
-
-#define DGB_BY_KIND(kind, CALL)                             \
-  ((kind) == kKindBytes ? K2Launcher<kKindBytes>::CALL      \
-   : (kind) == kKindF16 ? K2Launcher<kKindF16>::CALL        \
-   : (kind) == kKindBF16 ? K2Launcher<kKindBF16>::CALL      \
-                         : K2Launcher<kKindF32>::CALL)
-
 }  // namespace
 
 size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize) {
@@ -1624,7 +1486,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   if (kind != kKindBytes && histogram_dev) return DGB_ERR_INVALID_ARG;
   const Options opt = options();  // one snapshot per call
   const uint32_t W = (uint32_t)std::max(1, std::min(opt.encode_warps, 8));  // warps per CTA (two-kernel path)
-  const uint32_t elemBytes = kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u);
+  const uint32_t elemBytes = wordBytes(kind);
   const bool canonical = opt.encode_canonical != 0;
   const bool fused = !canonical && opt.encode_fused != 0;
   // staging slot of the fast / fused encoder (spills to global scratch when a block needs more)
@@ -1647,9 +1509,9 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   HostStage& hs = hostStage();
   const size_t descBytes = sizeof(MemberDesc) * (size_t)n;
   const size_t idxOff = (descBytes + 15) & ~size_t(15);
-  hs.upload.resize(idxOff + sizeof(uint2) * ((size_t)n + 1));
-  MemberDesc* desc = reinterpret_cast<MemberDesc*>(hs.upload.data());
-  uint2* workIdx = reinterpret_cast<uint2*>(hs.upload.data() + idxOff);
+  hs.encodeUpload.resize(idxOff + sizeof(uint2) * ((size_t)n + 1));
+  MemberDesc* desc = reinterpret_cast<MemberDesc*>(hs.encodeUpload.data());
+  uint2* workIdx = reinterpret_cast<uint2*>(hs.encodeUpload.data() + idxOff);
   uint32_t maxSize = 0;
   uint64_t tickets = 0, items = 0, chunks = 0;
   for (uint32_t i = 0; i < n; ++i) {
@@ -1703,7 +1565,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   if (inlined) {
     std::memcpy(im.m, desc, descBytes);
   } else {
-    DGB_CUDA_TRY(cudaMemcpyAsync(base + sp.members, hs.upload.data(), hs.upload.size(), cudaMemcpyHostToDevice, stream));
+    DGB_CUDA_TRY(cudaMemcpyAsync(base + sp.members, hs.encodeUpload.data(), hs.encodeUpload.size(), cudaMemcpyHostToDevice, stream));
   }
   DGB_CUDA_TRY(cudaMemsetAsync(base + sp.zeroBegin, 0, (canonical ? sp.lookbackEnd : sp.zeroEnd) - sp.zeroBegin, stream));
 
@@ -1716,132 +1578,105 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   if (fused) {
     // ---- one persistent launch: statistics items and encode chunks from two counters ----
     const uint32_t statsEvery = (uint32_t)std::max(0, opt.fused_stats_every);
-    const uint32_t ti = (uint32_t)items, tc = (uint32_t)chunks;
-#define DGB_FUSED(K, WD)                                                                                          \
-  (staged ? launchFused<K, WD, true>(sc, histogram_dev, pb, checksum, n, ti, tc, slabVecs, chunkBlocks, slotWords, \
-                                     statsEvery, sp.spillWarps, outSize_dev, stream)                               \
-          : launchFused<K, WD, false>(sc, histogram_dev, pb, checksum, n, ti, tc, slabVecs, chunkBlocks, slotWords, \
-                                      statsEvery, sp.spillWarps, outSize_dev, stream))
-    switch (kind) {
-      case kKindBytes: return wideTable ? DGB_FUSED(kKindBytes, true) : DGB_FUSED(kKindBytes, false);
-      case kKindF16: return wideTable ? DGB_FUSED(kKindF16, true) : DGB_FUSED(kKindF16, false);
-      case kKindBF16: return wideTable ? DGB_FUSED(kKindBF16, true) : DGB_FUSED(kKindBF16, false);
-      case kKindF32: return wideTable ? DGB_FUSED(kKindF32, true) : DGB_FUSED(kKindF32, false);
-      default: return DGB_ERR_INVALID_ARG;
-    }
-#undef DGB_FUSED
+    return withKind(kind, [&](auto K) { return withBool(wideTable, [&](auto WD) { return withBool(staged, [&](auto ST) {
+      auto kern = encodeFusedKernel<decltype(K)::value, decltype(WD)::value, decltype(ST)::value>;
+      constexpr uint32_t W = kStatsThreads / 32;
+      const size_t smemBytes = (size_t)W * encFastWarpSmem(slotWords, kind);
+      int perSm = 1;
+      const int rc = residentCtasPerSm((const void*)kern, kStatsThreads, smemBytes, 200 * 1024, &perSm);
+      if (rc != DGB_OK) return rc;
+      uint64_t grid = (uint64_t)perSm * (uint64_t)sms;
+      grid = std::min<uint64_t>(grid, items + chunks);
+      grid = std::min<uint64_t>(grid, sp.spillWarps / W);  // every warp owns a spill slot
+      grid = std::max<uint64_t>(grid, 1);
+      timerBegin(opt, kSlotFused, stream);
+      kern<<<(uint32_t)grid, kStatsThreads, smemBytes, stream>>>(sc, histogram_dev, pb, checksum, n, (uint32_t)items,
+                                                                 (uint32_t)chunks, slabVecs, chunkBlocks, slotWords,
+                                                                 statsEvery, outSize_dev);
+      DGB_CUDA_TRY(cudaGetLastError());
+      timerEnd(opt, kSlotFused, stream);
+      return DGB_OK;
+    }); }); });
   }
 
   // ---- two-kernel path: sub-batches on internal streams (the ordered canonical encoder stays on one) ----
-  hs.weight.resize(n);
-  uint64_t totalBytes = 0;
-  for (uint32_t i = 0; i < n; ++i) { hs.weight[i] = (uint64_t)desc[i].size * elemBytes; totalBytes += hs.weight[i]; }
   // byte inputs gain nothing from splitting (their stats kernel is atomics-bound, not HBM-bound; capi.cu autoParts)
-  const int parts = canonical ? 1 : autoParts(kind, n, totalBytes, false);
-  uint32_t bounds[kMaxParts + 1];
-  splitParts(hs.weight.data(), n, parts, bounds);
-  ForkGuard guard;
-  StreamPool* pool = nullptr;
-  if (parts > 1) {
-    int rc = streamPool(&pool);
-    if (rc != DGB_OK) return rc;
-    DGB_CUDA_TRY(cudaEventRecord(pool->start, stream));
-    guard.pool = pool;
-    guard.stream = stream;
-  }
-
+  SubBatches parts(kind, desc, n, opt, !canonical, stream);
+  if (const int rc = parts.fork(); rc != DGB_OK) return rc;
+  const uint32_t spillWarpsPerPart = sp.spillWarps / (uint32_t)parts.count();
+  const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0;
+  const uint32_t slabVecsK1 = stagedK1 ? std::min<uint32_t>(slabVecs, (uint32_t)std::max(1, opt.stats_stage_kb) * 64u) : slabVecs;
   // K2 launch configuration (same for every part)
   const size_t smemBytes = (size_t)W * (canonical ? encWarpSmem(pb, kind) : encFastWarpSmem(slotWords, kind));
-  // 0: canonical kernel (packed table), 1: fast kernel + packed table, 2: fast kernel + wide table
-  const int variant = canonical ? 0 : (wideTable ? 2 : 1);
-  int perSm = 1;
-  {
-    const int rc = DGB_BY_KIND(kind, residentPerSm(variant, W, smemBytes, &perSm));
+
+  return withKind(kind, [&](auto K) { return withBool(wideTable, [&](auto WD) {
+    constexpr int KIND = decltype(K)::value;
+    constexpr bool WIDE = decltype(WD)::value;
+    // K2: the canonical coder (ordered, packed table; wideTable is false) or the fast coder
+    const void* coder = canonical ? (const void*)encodeKernel<KIND> : (const void*)encodeKernelFast<WIDE, KIND>;
+    int perSm = 1;
+    int rc = residentCtasPerSm(coder, (int)(W * 32), smemBytes, 200 * 1024, &perSm);
     if (rc != DGB_OK) return rc;
-  }
-  // option encode_k2_ctas caps the coder's CTAs per SM so that the statistics kernel of the next
-  // sub-batch finds room beside it (0 = as many as fit)
-  if (opt.encode_k2_ctas > 0) perSm = std::min(perSm, opt.encode_k2_ctas);
-  const uint64_t resident = (uint64_t)perSm * sms;
-  int devForAttr = 0;
-  DGB_CUDA_TRY(cudaGetDevice(&devForAttr));
-  const uint32_t spillWarpsPerPart = sp.spillWarps / (uint32_t)parts;
+    // option encode_k2_ctas caps the coder's CTAs per SM so that the statistics kernel of the next
+    // sub-batch finds room beside it (0 = as many as fit)
+    if (opt.encode_k2_ctas > 0) perSm = std::min(perSm, opt.encode_k2_ctas);
+    const uint64_t resident = (uint64_t)perSm * sms;
 
-  for (int part = 0; part < parts; ++part) {
-    const uint32_t m0 = bounds[part], m1 = bounds[part + 1];
-    if (m1 == m0) continue;
-    cudaStream_t ps = stream;
-    if (parts > 1) {
-      ps = pool->s[part];
-      DGB_CUDA_TRY(cudaStreamWaitEvent(ps, pool->start, 0));
-      guard.forked[part] = true;
-    }
-    // ---- K1 ----
-    uint32_t partMax = 0;
-    for (uint32_t i = m0; i < m1; ++i) partMax = std::max(partMax, desc[i].size);
-    const uint64_t maxVecs = ((uint64_t)partMax * elemBytes) / 16u;
-    const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0;
-    const uint32_t slabVecsK1 = stagedK1 ? std::min<uint32_t>(slabVecs, (uint32_t)std::max(1, opt.stats_stage_kb) * 64u) : slabVecs;
-    uint32_t gridY = (uint32_t)std::max<uint64_t>(1, (maxVecs + slabVecsK1 - 1) / slabVecsK1);
-    if (!stagedK1) {
-      // enough CTAs to fill the machine a few times, never more than the slabs
-      const uint32_t wantY = std::max(1u, (uint32_t)(std::max(1, opt.hist_ctas_per_sm) * sms) / (m1 - m0));
-      gridY = std::min(gridY, wantY);
-    }
-    gridY = std::min(gridY, 65535u);
-    dim3 grid1(m1 - m0, gridY);
-    timerBegin(kSlotStats, ps);
-    if (stagedK1 && gridY * (uint64_t)slabVecsK1 >= maxVecs) {
-      const size_t stageBytes = (size_t)slabVecsK1 * 16u;
-      static thread_local int stagedDev = -1;
-      if (stagedDev != devForAttr) {
-        DGB_CUDA_TRY(cudaFuncSetAttribute(statsFloatStagedKernel<DGB_FLOAT16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-        DGB_CUDA_TRY(cudaFuncSetAttribute(statsFloatStagedKernel<DGB_BFLOAT16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-        DGB_CUDA_TRY(cudaFuncSetAttribute(statsFloatStagedKernel<DGB_FLOAT32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-        stagedDev = devForAttr;
+    for (int part = 0; part < parts.count(); ++part) {
+      const uint32_t m0 = parts.begin(part), m1 = parts.end(part);
+      if (m1 == m0) continue;
+      cudaStream_t ps;
+      rc = parts.stream(part, &ps);
+      if (rc != DGB_OK) return rc;
+      // ---- K1 ----
+      uint32_t partMax = 0;
+      for (uint32_t i = m0; i < m1; ++i) partMax = std::max(partMax, desc[i].size);
+      const uint64_t maxVecs = ((uint64_t)partMax * elemBytes) / 16u;
+      uint32_t gridY = (uint32_t)std::max<uint64_t>(1, (maxVecs + slabVecsK1 - 1) / slabVecsK1);
+      if (!stagedK1) {
+        // enough CTAs to fill the machine a few times, never more than the slabs
+        const uint32_t wantY = std::max(1u, (uint32_t)(std::max(1, opt.hist_ctas_per_sm) * sms) / (m1 - m0));
+        gridY = std::min(gridY, wantY);
       }
-      if (kind == kKindF16) {
-        statsFloatStagedKernel<DGB_FLOAT16><<<grid1, kStatsThreads, stageBytes, ps>>>(sc, pb, checksum, slabVecsK1, m0, outSize_dev);
-      } else if (kind == kKindBF16) {
-        statsFloatStagedKernel<DGB_BFLOAT16><<<grid1, kStatsThreads, stageBytes, ps>>>(sc, pb, checksum, slabVecsK1, m0, outSize_dev);
+      gridY = std::min(gridY, 65535u);
+      dim3 grid1(m1 - m0, gridY);
+      timerBegin(opt, kSlotStats, ps);
+      if constexpr (KIND == kKindBytes) {
+        statsBytesKernel<<<grid1, kStatsThreads, 0, ps>>>(sc, im, histogram_dev, pb, checksum, slabVecs, m0, outSize_dev);
+      } else if (stagedK1 && gridY * (uint64_t)slabVecsK1 >= maxVecs) {
+        rc = residentCtasPerSm((const void*)statsFloatStagedKernel<KIND>, kStatsThreads, 0, 128 * 1024, nullptr);
+        if (rc != DGB_OK) return rc;
+        statsFloatStagedKernel<KIND><<<grid1, kStatsThreads, (size_t)slabVecsK1 * 16u, ps>>>(sc, pb, checksum, slabVecsK1, m0,
+                                                                                            outSize_dev);
       } else {
-        statsFloatStagedKernel<DGB_FLOAT32><<<grid1, kStatsThreads, stageBytes, ps>>>(sc, pb, checksum, slabVecsK1, m0, outSize_dev);
+        statsFloatKernel<KIND><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
       }
-    } else if (kind == kKindBytes) {
-      statsBytesKernel<<<grid1, kStatsThreads, 0, ps>>>(sc, im, histogram_dev, pb, checksum, slabVecs, m0, outSize_dev);
-    } else if (kind == kKindF16) {
-      statsFloatKernel<DGB_FLOAT16><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
-    } else if (kind == kKindBF16) {
-      statsFloatKernel<DGB_BFLOAT16><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
-    } else {
-      statsFloatKernel<DGB_FLOAT32><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
-    }
-    DGB_CUDA_TRY(cudaGetLastError());
-    timerEnd(kSlotStats, ps);
+      DGB_CUDA_TRY(cudaGetLastError());
+      timerEnd(opt, kSlotStats, ps);
 
-    // ---- K2 ----
-    const uint32_t blockBegin = desc[m0].work0;
-    const uint32_t blockEnd = m1 < n ? desc[m1].work0 : totalTickets;
-    const uint32_t partBlocks = blockEnd - blockBegin;
-    if (partBlocks > 0) {
-      timerBegin(kSlotEncode, ps);
-      uint32_t grid2;
+      // ---- K2 ----
+      const uint32_t blockBegin = desc[m0].work0;
+      const uint32_t blockEnd = m1 < n ? desc[m1].work0 : totalTickets;
+      const uint32_t partBlocks = blockEnd - blockBegin;
+      if (partBlocks == 0) continue;
+      timerBegin(opt, kSlotEncode, ps);
       if (canonical) {
-        grid2 = std::min<uint32_t>(divUp(totalTickets, W), (uint32_t)resident);
+        const uint32_t grid2 = std::min<uint32_t>(divUp(totalTickets, W), (uint32_t)resident);
+        encodeKernel<KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, pb, checksum, n, totalTickets, outSize_dev);
       } else {
-        // one resident wave, equal rounds per warp (see launchDecode)
+        // one resident wave, equal rounds per warp (see launchPlanDecode)
         const uint64_t rounds = std::max<uint64_t>(1, (partBlocks + resident * W - 1) / (resident * W));
         const uint64_t want = ((uint64_t)partBlocks + W * rounds - 1) / (W * rounds);
-        grid2 = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, resident));
+        uint32_t grid2 = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, resident));
         grid2 = std::max(1u, std::min(grid2, spillWarpsPerPart / W));  // every warp owns a spill slot
+        encodeKernelFast<WIDE, KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, im, pb, checksum, n, blockBegin, blockEnd, slotWords,
+                                                                      (uint32_t)part * spillWarpsPerPart, outSize_dev);
       }
-      DGB_BY_KIND(kind, launch(variant, grid2, W, smemBytes, ps, sc, im, pb, checksum, n, totalTickets, blockBegin, blockEnd,
-                               slotWords, (uint32_t)part * spillWarpsPerPart, outSize_dev));
       DGB_CUDA_TRY(cudaGetLastError());
-      timerEnd(kSlotEncode, ps);
+      timerEnd(opt, kSlotEncode, ps);
     }
-  }
-  return DGB_OK;  // ~ForkGuard joins the helper streams
+    return DGB_OK;  // ~SubBatches joins the helper streams
+  }); });
 }
 
 }  // namespace dgb
