@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DIETGPU_B200_LIB selects an experiment build of the same library (tools/ only); default = the shipped one
 LIB_PATH = os.environ.get("DIETGPU_B200_LIB") or os.path.join(_HERE, "libdietgpu_b200.so")
 
-OK, ERR_INVALID_ARG, ERR_TEMP_TOO_SMALL, ERR_CUDA, ERR_CHECKSUM, ERR_TOO_LARGE = range(6)
+OK, ERR_INVALID_ARG, ERR_TEMP_TOO_SMALL, ERR_CUDA, ERR_CHECKSUM, ERR_TOO_LARGE, ERR_CAPTURING = range(7)
 FLOAT16, BFLOAT16, FLOAT32 = 1, 2, 3
 
 # every symbol include/dietgpu_b200.h declares (tests check the .so exports all of them)

@@ -1,7 +1,7 @@
 // capi.cu -- the extern "C" boundary declared in include/dietgpu_b200.h.
 // Maps the reference's three batch-addressing forms (pointer / stride / split
 // size; ans/BatchProvider.cuh) onto one internal member list, so every kernel
-// sees a single descriptor table uploaded in one copy.
+// sees a single descriptor table.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -46,6 +46,64 @@ thread_local TimedLaunch tlsOpen[kNumSlots];
 HostStage& hostStage() {
   static thread_local HostStage h;
   return h;
+}
+
+namespace {
+// uploadTable while capturing: up to kTableWords 8-byte words per launch, in the kernel parameters (32 KiB are allowed
+// since CUDA 12.1); most tables fit the small form, which keeps the parameter block of a launch at 4 KiB
+template <uint32_t WORDS>
+struct TableChunk {
+  unsigned long long* dst;
+  uint32_t words;
+  uint32_t pad;
+  unsigned long long w[WORDS];
+};
+constexpr uint32_t kTableWordsSmall = 500, kTableWords = 4080;
+static_assert(sizeof(TableChunk<kTableWordsSmall>) <= 4096 && sizeof(TableChunk<kTableWords>) <= 32764, "");
+
+template <uint32_t WORDS>
+__global__ void __launch_bounds__(256) tableKernel(const __grid_constant__ TableChunk<WORDS> c) {
+  for (uint32_t i = threadIdx.x; i < c.words; i += blockDim.x) c.dst[i] = c.w[i];
+}
+
+template <uint32_t WORDS>
+int launchTable(unsigned long long* dst, const unsigned long long* src, uint32_t words, cudaStream_t stream) {
+  static thread_local TableChunk<WORDS> c;
+  c.dst = dst;
+  c.words = words;
+  std::memcpy(c.w, src, (size_t)words * 8u);
+  tableKernel<WORDS><<<1, 256, 0, stream>>>(c);
+  DGB_CUDA_TRY(cudaGetLastError());
+  return DGB_OK;
+}
+}  // namespace
+
+int uploadTable(void* dst, const void* src, size_t bytes, cudaStream_t stream) {
+  if ((bytes | reinterpret_cast<uintptr_t>(dst)) & 7u) return DGB_ERR_INVALID_ARG;
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  DGB_CUDA_TRY(cudaStreamIsCapturing(stream, &st));
+  if (st == cudaStreamCaptureStatusNone) {
+    // an ordinary call: a copy from pageable memory has staged `src` when it returns, and it costs the device
+    // less than a copy kernel whose parameter block holds the table (256 members, c4 in tools/walltime.py on an
+    // H100 at 400 W: encode and decode each 2-5 us faster).  A captured copy would read `src` at every replay.
+    DGB_CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
+    return DGB_OK;
+  }
+  auto* d = static_cast<unsigned long long*>(dst);
+  const auto* s = static_cast<const unsigned long long*>(src);
+  for (size_t w = 0, words = bytes / 8u; w < words; w += kTableWords) {
+    const uint32_t k = (uint32_t)std::min<size_t>(kTableWords, words - w);
+    const int rc = k <= kTableWordsSmall ? launchTable<kTableWordsSmall>(d + w, s + w, k, stream)
+                                         : launchTable<kTableWords>(d + w, s + w, k, stream);
+    if (rc != DGB_OK) return rc;
+  }
+  return DGB_OK;
+}
+
+int checkNotCapturing(cudaStream_t stream) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  DGB_CUDA_TRY(cudaStreamIsCapturing(stream, &st));
+  return st == cudaStreamCaptureStatusNone ? DGB_OK : DGB_ERR_CAPTURING;
 }
 
 int smCount() {
@@ -269,6 +327,7 @@ const char* dgb_error_string(int code) {
     case DGB_ERR_CUDA: return "CUDA runtime error";
     case DGB_ERR_CHECKSUM: return "checksum mismatch";
     case DGB_ERR_TOO_LARGE: return "size exceeds format limits";
+    case DGB_ERR_CAPTURING: return "checksum verification synchronises the stream and cannot be captured into a CUDA graph";
     default: return "unknown error";
   }
 }

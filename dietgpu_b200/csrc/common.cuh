@@ -45,7 +45,7 @@ __host__ __device__ constexpr uint32_t floatNonCompBytes(int ft, uint32_t n) {
 // probBits bits (a symbol of pdf 1), so 4096*pb/16 words; +8 for 16 B padding.
 __host__ __device__ constexpr uint32_t maxBlockWords(int pb) { return 256u * (uint32_t)pb + 8u; }
 
-// ---- per-member descriptor (device), built on the host in one upload -------
+// ---- per-member descriptor (device), built on the host ----------------------
 enum CodecKind : int { kKindBytes = 0, kKindF16 = DGB_FLOAT16, kKindBF16 = DGB_BFLOAT16, kKindF32 = DGB_FLOAT32 };
 
 struct MemberDesc {
@@ -57,10 +57,9 @@ struct MemberDesc {
 static_assert(sizeof(MemberDesc) == 24, "");
 
 // Batches of up to kInlineMembers members travel to the default kernels INSIDE the kernel parameters
-// (constant bank, 1.5 KB) instead of through a host-to-device copy in front of the first launch: one
-// dependent DMA less per call, nothing of the caller's host memory is read after the call returns,
-// and the whole call can be captured into a CUDA graph.  Larger batches (and the optional kernel
-// flavours) read the same table from the scratch buffer.
+// (constant bank, 1.5 KB) instead of through a copy in front of the first launch: one dependent
+// operation less per call.  Larger batches (and the optional kernel flavours) read the same table from the
+// scratch buffer, where uploadTable puts it; either way no host memory is read after the call returns.
 constexpr uint32_t kInlineMembers = 64;
 struct InlineMembers {
   uint32_t count;  // 0: the table is in global memory (scratch)
@@ -151,15 +150,25 @@ int smCount();  // SMs of the current device, cached per device
 int residentCtasPerSm(const void* kernel, int threads, size_t smemBytes, int maxDynamicSmem, int* out);
 
 // Per-thread host staging of the codec calls, reused: no allocation on the steady-state call path.
-// The uploaded member tables have a buffer per direction: a CUDA graph that captured an encode and a
-// decode copies from both host buffers again at every replay.
+// Nothing here is read after the call returns (uploadTable), so a later call, or a graph capture, may
+// overwrite every buffer.
 struct HostStage {
   std::vector<HostMember> members;      // the entry point's member list (capi.cu)
-  std::vector<uint8_t> encodeUpload;    // encoder member table + work index, uploaded in one copy
+  std::vector<uint8_t> encodeUpload;    // encoder member table + work index, uploaded together
   std::vector<MemberDesc> decodeTable;  // decoder member table
   std::vector<uint32_t> checksum;       // decoder checksum pass: computed, stored and decoded size per member
 };
 HostStage& hostStage();
+
+// Enqueues on `stream` a copy of `bytes` (a multiple of 8) of host memory at `src` to `dst` (device, 8 B
+// aligned).  `src` is read before this returns, so the caller may reuse it at once: an ordinary call copies
+// from pageable memory, which stages the bytes; on a capturing stream the bytes travel inside the parameters
+// of small copy kernels, so a graph replays the bytes it captured, not whatever `src` holds at replay time.
+int uploadTable(void* dst, const void* src, size_t bytes, cudaStream_t stream);
+
+// DGB_ERR_CAPTURING when `stream` is being captured into a CUDA graph, else DGB_OK; for calls that
+// synchronise the stream, which a capture cannot hold
+int checkNotCapturing(cudaStream_t stream);
 
 // Per-kernel timing (Options::timing of the call): slots are stable indices reported by
 // dgb_kernel_times().  No-ops when timing is off.

@@ -836,6 +836,10 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const DecodePlan dp = planDecodeScratch(n);
   if (!temp || tempBytes < dp.total) return DGB_ERR_TEMP_TOO_SMALL;
   if (reinterpret_cast<uintptr_t>(temp) & 255u) return DGB_ERR_INVALID_ARG;
+  if (checksum) {
+    const int rc = checkNotCapturing(stream);  // the verification below synchronises the stream
+    if (rc != DGB_OK) return rc;
+  }
 
   const Options opt = options();  // one snapshot per call
   const bool fused = opt.decode_fused != 0;
@@ -873,7 +877,8 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   if (inlined) {
     std::memcpy(im.m, desc, sizeof(MemberDesc) * n);
   } else {
-    DGB_CUDA_TRY(cudaMemcpyAsync(sc.members, desc, sizeof(MemberDesc) * n, cudaMemcpyHostToDevice, stream));
+    const int rc = uploadTable(sc.members, desc, sizeof(MemberDesc) * n, stream);
+    if (rc != DGB_OK) return rc;
   }
   if (checksum) DGB_CUDA_TRY(cudaMemsetAsync(sc.checksum, 0, 4 * (size_t)n, stream));
 
@@ -1075,7 +1080,8 @@ int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool 
   const void* const* in_dev = in;
   if (!inIsDevice) {
     if (!temp || tempBytes < sizeof(void*) * (size_t)n) return DGB_ERR_TEMP_TOO_SMALL;
-    DGB_CUDA_TRY(cudaMemcpyAsync(temp, in, sizeof(void*) * (size_t)n, cudaMemcpyHostToDevice, stream));
+    const int rc = uploadTable(temp, in, sizeof(void*) * (size_t)n, stream);
+    if (rc != DGB_OK) return rc;
     in_dev = static_cast<const void* const*>(temp);
   }
   infoKernel<<<divUp(n, 128), 128, 0, stream>>>(kind, in_dev, n, outSizes, outTypes, outChecksum);

@@ -1443,7 +1443,7 @@ uint32_t spillWarpBound(uint32_t n, uint64_t totalBlocks) {
 ScratchPlan planScratch(int kind, uint32_t n, uint32_t maxSize, uint32_t totalTickets, uint32_t spillWarps) {
   ScratchPlan p{};
   size_t o = 0;
-  // uploaded in one copy: member descriptors, then the fused launch's work index
+  // uploaded together: member descriptors, then the fused launch's work index
   p.members = o; o += sizeof(MemberDesc) * (size_t)n;
   o = (o + 15) & ~size_t(15);
   p.workIdx = o; o += sizeof(uint2) * ((size_t)n + 1);
@@ -1505,7 +1505,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const uint32_t chunkBlocks = (uint32_t)std::max(1, std::min(opt.fused_chunk_blocks, 4096));
   const bool doPass = histogram_dev == nullptr || checksum;
 
-  // ---- member table + work index (host staging, one upload) ----
+  // ---- member table + work index (host staging, uploaded together) ----
   HostStage& hs = hostStage();
   const size_t descBytes = sizeof(MemberDesc) * (size_t)n;
   const size_t idxOff = (descBytes + 15) & ~size_t(15);
@@ -1557,7 +1557,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   sc.spill = base + sp.spill;
   sc.table = reinterpret_cast<uint4*>(base + sp.table);
 
-  // member table: inside the kernel parameters when it fits and the default kernels run, else one upload
+  // member table: inside the kernel parameters when it fits and the default kernels run, else uploaded to scratch
   static thread_local InlineMembers im;
   const bool inlined = opt.inline_members != 0 && n <= kInlineMembers && !fused && !canonical &&
                        !(kind != kKindBytes && opt.stats_stage != 0);
@@ -1565,7 +1565,8 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   if (inlined) {
     std::memcpy(im.m, desc, descBytes);
   } else {
-    DGB_CUDA_TRY(cudaMemcpyAsync(base + sp.members, hs.encodeUpload.data(), hs.encodeUpload.size(), cudaMemcpyHostToDevice, stream));
+    const int rc = uploadTable(base + sp.members, hs.encodeUpload.data(), hs.encodeUpload.size(), stream);
+    if (rc != DGB_OK) return rc;
   }
   DGB_CUDA_TRY(cudaMemsetAsync(base + sp.zeroBegin, 0, (canonical ? sp.lookbackEnd : sp.zeroEnd) - sp.zeroBegin, stream));
 

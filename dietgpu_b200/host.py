@@ -24,16 +24,25 @@ def _nbytes(t: torch.Tensor) -> int:
     return t.numel() * t.element_size()
 
 
+def _storage(t: torch.Tensor) -> int:
+    """Identity of the allocation a tensor views."""
+    return t.untyped_storage().data_ptr()
+
+
 def _copy_runs(dst: Sequence[torch.Tensor], src: Sequence[torch.Tensor], stream: torch.cuda.Stream) -> None:
     """dst[i] <- src[i] (same byte sizes), one DMA per maximal run of members that are byte-adjacent on
-    BOTH sides (e.g. slices of one pinned buffer -> the packed device staging buffer)."""
+    BOTH sides (e.g. slices of one pinned buffer -> the packed device staging buffer).  A run never spans
+    two allocations: separately pinned tensors may happen to sit back to back, and one copy across both is
+    invalid."""
     L, st = capi.lib(), stream.cuda_stream
     i, n = 0, len(dst)
     while i < n:
         d0, s0 = dst[i].data_ptr(), src[i].data_ptr()
+        ds, ss = _storage(dst[i]), _storage(src[i])
         total = _nbytes(src[i])
         j = i + 1
-        while j < n and dst[j].data_ptr() == d0 + total and src[j].data_ptr() == s0 + total:
+        while (j < n and dst[j].data_ptr() == d0 + total and src[j].data_ptr() == s0 + total
+               and _storage(dst[j]) == ds and _storage(src[j]) == ss):
             total += _nbytes(src[j])
             j += 1
         capi.check(L.dgb_copy_async(d0, s0, total, st), "copy")
@@ -47,16 +56,17 @@ def _row_room(rows: Sequence[torch.Tensor]) -> int:
 
 
 def _copy_rows(dst_ptrs: Sequence[int], src_ptrs: Sequence[int], sizes: Sequence[int], dst_cap: int, src_cap: int,
-               stream: torch.cuda.Stream) -> None:
+               stream: torch.cuda.Stream, one_allocation: bool = True) -> None:
     """Row i: sizes[i] bytes from src_ptrs[i] to dst_ptrs[i].  When the rows sit at a constant pitch on both
-    sides (rows of two [n, cols] matrices) and have similar sizes, one pitched DMA moves the whole group
-    (every row copies max(sizes) bytes: rows have dst_cap / src_cap bytes of room); else one copy per row."""
+    sides (rows of two [n, cols] matrices; `one_allocation`: all rows of each side lie in one allocation) and
+    have similar sizes, one pitched DMA moves the whole group (every row copies max(sizes) bytes: rows have
+    dst_cap / src_cap bytes of room); else one copy per row."""
     L, st = capi.lib(), stream.cuda_stream
     n = len(sizes)
     if n == 0:
         return
     w = max(sizes)
-    if n > 1 and w > 0:
+    if n > 1 and w > 0 and one_allocation:
         dp, sp = dst_ptrs[1] - dst_ptrs[0], src_ptrs[1] - src_ptrs[0]
         pitched = dp >= w and sp >= w and w <= dst_cap and w <= src_cap and all(
             dst_ptrs[k + 1] - dst_ptrs[k] == dp and src_ptrs[k + 1] - src_ptrs[k] == sp for k in range(n - 1))
@@ -236,7 +246,8 @@ class HostCodec:
                     szs.append(sz)
                 # rows of one pinned [n, cols] matrix go up as one pitched DMA per group
                 _copy_rows([self.comp_in[i].data_ptr() for i in range(a, b)], [host_rows[i].data_ptr() for i in range(a, b)],
-                           szs, self.cols, _row_room(host_rows[a:b]), self.up)
+                           szs, self.cols, _row_room(host_rows[a:b]), self.up,
+                           len({_storage(r) for r in host_rows[a:b]}) == 1)
                 ev_up = torch.cuda.Event()
                 ev_up.record(self.up)
                 with torch.cuda.stream(self.k):

@@ -16,7 +16,9 @@
  *     returns; "_dev" = device memory; `stream` is a cudaStream_t passed as
  *     void* (NULL = the legacy default stream);
  *   - all device work is enqueued on `stream`; calls are asynchronous unless
- *     a checksum has to be verified (decode with use_checksum != 0);
+ *     a checksum has to be verified (decode with use_checksum != 0).  No
+ *     device work reads a host array after the call returns, so every call
+ *     but checksum-verifying decodes can be captured into a CUDA graph;
  *   - temp_dev/temp_bytes: caller-owned device scratch, 256 B aligned, at
  *     least dgb_*_temp_bytes(...) bytes; it may be reused by the next call on
  *     the same stream.  The library allocates nothing (no cudaMalloc);
@@ -46,6 +48,7 @@ extern "C" {
 #define DGB_ERR_CUDA 3            /* a CUDA runtime call failed (see dgb_last_cuda_error) */
 #define DGB_ERR_CHECKSUM 4        /* decode: stored checksum != recomputed checksum */
 #define DGB_ERR_TOO_LARGE 5       /* a size exceeds the format's 32-bit limits */
+#define DGB_ERR_CAPTURING 6       /* decode with checksum verification on a stream that is being captured */
 
 /* float/GpuFloatCodec.h:18-23 FloatType */
 #define DGB_FLOAT16 1
@@ -112,7 +115,9 @@ int dgb_ans_encode_split_size(void* temp_dev, size_t temp_bytes, int prob_bits, 
  * skipped (size = required bytes, or 0 for an invalid header).
  * With use_checksum != 0 the call synchronises `stream`, compares checksums
  * and returns DGB_ERR_CHECKSUM on mismatch; checksum_mismatch_host (optional
- * host u8[n]) then flags the failing members. */
+ * host u8[n]) then flags the failing members.  That synchronisation cannot be
+ * captured into a CUDA graph: on a capturing stream such a call returns
+ * DGB_ERR_CAPTURING before it enqueues anything, and the capture stays valid. */
 int dgb_ans_decode_pointer(void* temp_dev, size_t temp_bytes, int prob_bits, int use_checksum,
                            uint32_t num_in_batch, const void* const* in, void* const* out,
                            const uint32_t* out_capacity, uint8_t* out_success_dev,

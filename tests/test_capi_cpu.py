@@ -48,6 +48,8 @@ def test_error_codes_without_gpu():
     L = capi.lib()
     assert capi.error_string(capi.OK) == "ok"
     assert "temporary" in capi.error_string(capi.ERR_TEMP_TOO_SMALL)
+    assert "cannot be captured" in capi.error_string(capi.ERR_CAPTURING)
+    assert capi.error_string(capi.ERR_CAPTURING + 1) == "unknown error"
     # empty batches are no-ops and need no device
     assert L.dgb_ans_encode_pointer(None, 0, 10, 0, 0, None, None, None, None, None, None) == capi.OK
     assert L.dgb_ans_decode_pointer(None, 0, 10, 0, 0, None, None, None, None, None, None, None) == capi.OK
