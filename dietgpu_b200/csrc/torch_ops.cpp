@@ -4,7 +4,14 @@
 // (/root/reference/dietgpu/DietGpu.cpp:915-937) so that code written against
 // `torch.ops.load_library(<dietgpu>)` works by loading this library instead.  Argument validation,
 // return values and error behaviour follow DietGpu.cpp:149-911; tensors are only handles to device
-// memory -- all compute is in the CUDA library behind include/dietgpu_b200_compat.hpp.
+// memory -- all compute is in the CUDA library (include/dietgpu_b200.h).
+//
+// Every codec call goes to a dgb_* entry point and every return code becomes a TORCH_CHECK, so input the C ABI
+// refuses raises RuntimeError instead of aborting the process (the compat header keeps the reference's abort for
+// C++ callers; here only its StackDeviceMemory leases the scratch).  Where the reference would write or read
+// memory the caller did not hand over, these operators differ on purpose, as dietgpu_b200/ops.py does: byte
+// batches of mixed dtypes get rows sized by their largest member in bytes, split sizes must fit the tensor they
+// index, float outputs must share one dtype, and archives and output rows must be 16 B aligned.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/library.h>
@@ -42,14 +49,34 @@ at::ScalarType dtypeOf(FloatType ft) {
   return at::ScalarType::Half;
 }
 
-std::tuple<int64_t, int64_t> totalAndMax(const std::vector<Tensor>& ts) {
-  int64_t total = 0, mx = 0;
+// largest member in elements and, separately, in bytes (a byte batch may mix dtypes)
+std::tuple<int64_t, int64_t> maxNumelAndBytes(const std::vector<Tensor>& ts) {
+  int64_t mx = 0, mxBytes = 0;
   for (auto& t : ts) {
     TORCH_CHECK((uint64_t)t.numel() * t.element_size() <= std::numeric_limits<uint32_t>::max());
-    total += t.numel();
     mx = std::max<int64_t>(mx, t.numel());
+    mxBytes = std::max<int64_t>(mxBytes, t.numel() * t.element_size());
   }
-  return {total, mx};
+  return {mx, mxBytes};
+}
+
+void checkRc(int rc, const char* what) {
+  TORCH_CHECK(rc == DGB_OK, "dietgpu: ", what, " failed: ", dgb_error_string(rc), " (code ", rc,
+              rc == DGB_ERR_CUDA ? ", cudaError " + std::to_string(dgb_last_cuda_error()) : std::string(), ")");
+}
+void checkDecodeRc(int rc, bool asFloat, const char* what) {
+  TORCH_CHECK(rc != DGB_ERR_CHECKSUM, asFloat ? "floatDecompress" : "ANSDecode",
+              ": checksum mismatch seen on decoded data; archive cannot be unpacked");
+  checkRc(rc, what);
+}
+void checkArchiveAligned(const Tensor& t) {
+  TORCH_CHECK(uintptr_t(t.data_ptr()) % 16 == 0, "dietgpu: compressed input is not 16 B aligned");
+}
+void checkSplitTotal(const std::vector<uint32_t>& split, int64_t capacity, const char* what) {
+  int64_t total = 0;
+  for (auto s : split) total += s;
+  TORCH_CHECK(total <= capacity, "dietgpu: split sizes sum to ", total, ", more than ", what, " holds (", capacity,
+              ")");
 }
 
 StackDeviceMemory makeRes(const std::optional<Tensor>& temp, const Tensor& like) {
@@ -61,18 +88,26 @@ StackDeviceMemory makeRes(const std::optional<Tensor>& temp, const Tensor& like)
   return StackDeviceMemory(like.get_device(), nullptr, 0);
 }
 
-// The reference falls back to cudaMalloc inside StackDeviceMemory when scratch is missing; here
-// the op first tries a stream-ordered torch allocation so the common "no temp_mem" call stays
-// asynchronous.
+// The scratch of one codec call: `need` bytes leased from temp_mem when it holds them at a 256 B boundary.
+// The reference falls back to cudaMalloc inside StackDeviceMemory when scratch is missing; here the op
+// uses a stream-ordered torch allocation instead, so the common "no temp_mem" call stays asynchronous
+// and the lease never takes StackDeviceMemory's cudaMalloc path.
 struct Scratch {
   Tensor owned;
   StackDeviceMemory res;
-  Scratch(const std::optional<Tensor>& temp, const Tensor& like, size_t need) : res(makeRes(temp, like)) {
-    if (res.getSizeAvailable() < need) {
-      owned = torch::empty({(int64_t)need + 256}, at::TensorOptions().device(like.device()).dtype(torch::kByte));
-      res = StackDeviceMemory(like.get_device(), owned.data_ptr(), need + 256);
+  StackDeviceMemory::Lease lease;  // declared last: released before `res` goes away
+  Scratch(const std::optional<Tensor>& temp, const Tensor& like, size_t need, cudaStream_t stream)
+      : res(makeRes(temp, like)) {
+    const size_t granular = (std::max<size_t>(need, 1) + kSDMAlignment - 1) / kSDMAlignment * kSDMAlignment;
+    if (res.getSizeAvailable() < granular) {
+      owned = torch::empty({(int64_t)granular + 256}, at::TensorOptions().device(like.device()).dtype(torch::kByte));
+      res = StackDeviceMemory(like.get_device(), owned.data_ptr(), granular + 256);
     }
+    lease = res.lease(need, stream);
   }
+  void* ptr() const { return lease.ptr; }
+  size_t bytes() const { return lease.bytes; }
+  int64_t used() const { return (int64_t)res.getMaxMemoryUsage(); }
 };
 
 // ---- sizes ----------------------------------------------------------------
@@ -84,16 +119,18 @@ int64_t bound(uint32_t v) {
 }
 std::tuple<int64_t, int64_t> max_float_compressed_output_size(const std::vector<Tensor>& ts) {
   TORCH_CHECK(!ts.empty());
-  auto s = totalAndMax(ts);
-  return {(int64_t)ts.size(), bound(getMaxFloatCompressedSize(floatTypeOf(ts[0]), std::get<1>(s)))};
+  auto s = maxNumelAndBytes(ts);
+  return {(int64_t)ts.size(), bound(getMaxFloatCompressedSize(floatTypeOf(ts[0]), std::get<0>(s)))};
 }
 int64_t max_float_compressed_size(const Tensor& dtype, int64_t size) {
   return bound(getMaxFloatCompressedSize(floatTypeOf(dtype), size));
 }
 std::tuple<int64_t, int64_t> max_any_compressed_output_size(const std::vector<Tensor>& ts) {
   TORCH_CHECK(!ts.empty());
-  auto s = totalAndMax(ts);
-  return {(int64_t)ts.size(), bound(getMaxCompressedSize(std::get<1>(s) * ts[0].element_size()))};
+  // rows sized by the largest member in bytes; the reference multiplies the largest element count by the
+  // first member's element size (DietGpu.cpp:134), too small for a batch of mixed dtypes
+  auto s = maxNumelAndBytes(ts);
+  return {(int64_t)ts.size(), bound(getMaxCompressedSize(std::get<1>(s)))};
 }
 int64_t max_any_compressed_size(int64_t bytes) { return bound(getMaxCompressedSize(bytes)); }
 
@@ -104,6 +141,8 @@ void validateOut(const std::optional<Tensor>& outCompressed, const std::optional
     TORCH_CHECK(outCompressed->dtype() == torch::kByte && outCompressed->is_cuda() && outCompressed->is_contiguous());
     TORCH_CHECK(outCompressed->dim() == 2 && outCompressed->size(0) >= n && outCompressed->size(1) >= cols);
     TORCH_CHECK(outCompressed->get_device() == like.get_device());
+    TORCH_CHECK(uintptr_t(outCompressed->data_ptr()) % 16 == 0 && (n <= 1 || outCompressed->size(1) % 16 == 0),
+                "dietgpu: out_compressed rows are not 16 B aligned");
     comp = *outCompressed;
   } else {
     comp = torch::empty({n, cols}, at::TensorOptions().device(like.device()).dtype(torch::kByte));
@@ -144,18 +183,20 @@ std::tuple<Tensor, Tensor, int64_t> compress_data(bool asFloat, const std::vecto
     out[i] = (uint8_t*)comp.data_ptr() + i * comp.size(1);
     maxSize = std::max(maxSize, inSize[i]);
   }
-  auto stream = at::cuda::getCurrentCUDAStream();
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (asFloat) {
-    auto ft = floatTypeOf(tIns[0]);
-    Scratch sc(tempMem, tIns[0], dgb_float_compress_temp_bytes((int)ft, n, maxSize));
-    FloatCompressConfig cfg(ft, ANSCodecConfig(kPrecision, false), false, checksum);
-    floatCompress(sc.res, cfg, n, in.data(), inSize.data(), out.data(), (uint32_t*)sizes.data_ptr(), stream);
-    return {comp, sizes, (int64_t)sc.res.getMaxMemoryUsage()};
+    const int ft = (int)floatTypeOf(tIns[0]);
+    Scratch sc(tempMem, tIns[0], dgb_float_compress_temp_bytes(ft, n, maxSize), stream);
+    checkRc(dgb_float_compress_pointer(sc.ptr(), sc.bytes(), ft, kPrecision, checksum, n, in.data(), inSize.data(),
+                                       out.data(), (uint32_t*)sizes.data_ptr(), stream),
+            "compress_data");
+    return {comp, sizes, sc.used()};
   }
-  Scratch sc(tempMem, tIns[0], dgb_ans_encode_temp_bytes(n, maxSize));
-  ansEncodeBatchPointer(sc.res, ANSCodecConfig(kPrecision, checksum), n, in.data(), inSize.data(), nullptr, out.data(),
-                        (uint32_t*)sizes.data_ptr(), stream);
-  return {comp, sizes, (int64_t)sc.res.getMaxMemoryUsage()};
+  Scratch sc(tempMem, tIns[0], dgb_ans_encode_temp_bytes(n, maxSize), stream);
+  checkRc(dgb_ans_encode_pointer(sc.ptr(), sc.bytes(), kPrecision, checksum, n, in.data(), inSize.data(), nullptr,
+                                 out.data(), (uint32_t*)sizes.data_ptr(), stream),
+          "compress_data");
+  return {comp, sizes, sc.used()};
 }
 
 std::vector<Tensor> matrixToTensors(int64_t n, Tensor& matrix, Tensor& sizes) {
@@ -176,31 +217,36 @@ std::tuple<std::vector<Tensor>, Tensor, int64_t> compress_data_split_size(
   if (!asFloat) TORCH_CHECK(uintptr_t(tIn.data_ptr()) % kANSRequiredAlignment == 0, "start pointer is not aligned");
   TORCH_CHECK(tSplit.is_contiguous() && tSplit.device().type() == at::kCPU && tSplit.dtype() == torch::kInt);
   const int64_t n = tSplit.numel();
+  std::vector<uint32_t> split(n);
   uint32_t maxSize = 0;
   for (int64_t i = 0; i < n; ++i) {
     auto size = tSplit.data_ptr<int32_t>()[i];
     TORCH_CHECK(size > 0);
+    split[i] = size;
     maxSize = std::max<uint32_t>(maxSize, size);
     if (!asFloat && i != n - 1)
       TORCH_CHECK(size % kANSRequiredAlignment == 0, "the size of an interior split is not a multiple of 4 bytes");
   }
-  const int64_t cols = asFloat ? getMaxFloatCompressedSize(ft, maxSize) : getMaxCompressedSize(maxSize);
+  // splits count words of tIn's dtype for floats, bytes otherwise
+  checkSplitTotal(split, asFloat ? tIn.numel() : tIn.numel() * tIn.element_size(), "t_in");
+  const int64_t cols = bound(asFloat ? getMaxFloatCompressedSize(ft, maxSize) : getMaxCompressedSize(maxSize));
   Tensor comp, sizes;
   validateOut(outCompressed, outSizes, n, cols, tIn, comp, sizes);
-  auto stream = at::cuda::getCurrentCUDAStream();
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   int64_t used = 0;
   if (asFloat) {
-    Scratch sc(tempMem, tIn, dgb_float_compress_temp_bytes((int)ft, n, maxSize));
-    FloatCompressConfig cfg(ft, ANSCodecConfig(kPrecision, false), false, checksum);
-    floatCompressSplitSize(sc.res, cfg, n, tIn.data_ptr(), (const uint32_t*)tSplit.data_ptr(), comp.data_ptr(),
-                           comp.size(1), (uint32_t*)sizes.data_ptr(), stream);
-    used = sc.res.getMaxMemoryUsage();
+    Scratch sc(tempMem, tIn, dgb_float_compress_temp_bytes((int)ft, n, maxSize), stream);
+    checkRc(dgb_float_compress_split_size(sc.ptr(), sc.bytes(), (int)ft, kPrecision, checksum, n, tIn.data_ptr(),
+                                          split.data(), comp.data_ptr(), comp.size(1), (uint32_t*)sizes.data_ptr(),
+                                          stream),
+            "compress_data_split_size");
+    used = sc.used();
   } else {
-    Scratch sc(tempMem, tIn, dgb_ans_encode_temp_bytes(n, maxSize));
-    ansEncodeBatchSplitSize(sc.res, ANSCodecConfig(kPrecision, checksum), n, tIn.data_ptr(),
-                            (const uint32_t*)tSplit.data_ptr(), nullptr, comp.data_ptr(), comp.size(1),
-                            (uint32_t*)sizes.data_ptr(), stream);
-    used = sc.res.getMaxMemoryUsage();
+    Scratch sc(tempMem, tIn, dgb_ans_encode_temp_bytes(n, maxSize), stream);
+    checkRc(dgb_ans_encode_split_size(sc.ptr(), sc.bytes(), kPrecision, checksum, n, tIn.data_ptr(), split.data(),
+                                      nullptr, comp.data_ptr(), comp.size(1), (uint32_t*)sizes.data_ptr(), stream),
+            "compress_data_split_size");
+    used = sc.used();
   }
   return {matrixToTensors(n, comp, sizes), sizes, used};
 }
@@ -244,8 +290,14 @@ int64_t decompressImpl(bool asFloat, const std::vector<Tensor>& tIns, const std:
     auto& ti = tIns[i];
     auto& to = tOuts[i];
     TORCH_CHECK(ti.is_cuda() && ti.is_contiguous() && ti.dtype() == torch::kByte);
+    TORCH_CHECK(ti.get_device() == tIns[0].get_device());
+    checkArchiveAligned(ti);
     TORCH_CHECK(to.is_cuda() && to.is_contiguous() && to.get_device() == ti.get_device());
-    if (asFloat) floatTypeOf(to);
+    if (asFloat) {
+      floatTypeOf(to);
+      // capacities are counted in words of one float type
+      TORCH_CHECK(to.dtype() == tOuts[0].dtype(), "dietgpu: float outputs must all have the same dtype");
+    }
     in[i] = ti.data_ptr();
     out[i] = to.data_ptr();
     auto c = asFloat ? to.numel() : to.numel() * to.element_size();
@@ -255,22 +307,20 @@ int64_t decompressImpl(bool asFloat, const std::vector<Tensor>& tIns, const std:
   validateStatus(outStatus, outSizes, n, tIns[0]);
   auto st = (uint8_t*)(outStatus ? outStatus->data_ptr() : nullptr);
   auto sz = (uint32_t*)(outSizes ? outSizes->data_ptr() : nullptr);
-  auto stream = at::cuda::getCurrentCUDAStream();
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (asFloat) {
-    auto ft = floatTypeOf(tOuts[0]);
-    Scratch sc(tempMem, tIns[0], dgb_float_decompress_temp_bytes((int)ft, n, 0));
-    FloatDecompressConfig cfg(ft, ANSCodecConfig(kPrecision, false), false, checksum);
-    auto status = floatDecompress(sc.res, cfg, n, in.data(), out.data(), cap.data(), st, sz, stream);
-    TORCH_CHECK(status.error != FloatDecompressError::ChecksumMismatch,
-                "floatDecompress: checksum mismatch seen on decoded data; archive cannot be unpacked");
-    return sc.res.getMaxMemoryUsage();
+    const int ft = (int)floatTypeOf(tOuts[0]);
+    Scratch sc(tempMem, tIns[0], dgb_float_decompress_temp_bytes(ft, n, 0), stream);
+    checkDecodeRc(dgb_float_decompress_pointer(sc.ptr(), sc.bytes(), ft, kPrecision, checksum, n, in.data(),
+                                               out.data(), cap.data(), st, sz, nullptr, stream),
+                  true, "decompress_data");
+    return sc.used();
   }
-  Scratch sc(tempMem, tIns[0], dgb_ans_decode_temp_bytes(n));
-  auto status = ansDecodeBatchPointer(sc.res, ANSCodecConfig(kPrecision, checksum), n, in.data(), out.data(),
-                                      cap.data(), st, sz, stream);
-  TORCH_CHECK(status.error != ANSDecodeError::ChecksumMismatch,
-              "ANSDecode: checksum mismatch seen on decoded data; archive cannot be unpacked");
-  return sc.res.getMaxMemoryUsage();
+  Scratch sc(tempMem, tIns[0], dgb_ans_decode_temp_bytes(n), stream);
+  checkDecodeRc(dgb_ans_decode_pointer(sc.ptr(), sc.bytes(), kPrecision, checksum, n, in.data(), out.data(),
+                                       cap.data(), st, sz, nullptr, stream),
+                false, "decompress_data");
+  return sc.used();
 }
 
 int64_t decompress_data(bool asFloat, const std::vector<Tensor>& tIns, const std::vector<Tensor>& tOuts, bool checksum,
@@ -291,31 +341,33 @@ int64_t decompress_data_split_size(bool asFloat, const std::vector<Tensor>& tIns
   std::vector<uint32_t> split(n);
   for (int64_t i = 0; i < n; ++i) {
     TORCH_CHECK(tIns[i].is_cuda() && tIns[i].is_contiguous() && tIns[i].dtype() == torch::kByte);
+    TORCH_CHECK(tIns[i].get_device() == tIns[0].get_device());
+    checkArchiveAligned(tIns[i]);
     in[i] = tIns[i].data_ptr();
     auto s = tSplit.data_ptr<int32_t>()[i];
     TORCH_CHECK(s > 0);
     split[i] = s;
   }
   TORCH_CHECK(tOut.is_cuda() && tOut.is_contiguous());
+  TORCH_CHECK(tOut.get_device() == tIns[0].get_device(), "dietgpu: t_out is not on the device of the compressed inputs");
+  const int ft = asFloat ? (int)floatTypeOf(tOut) : 0;
+  checkSplitTotal(split, asFloat ? tOut.numel() : tOut.numel() * tOut.element_size(), "t_out");
   validateStatus(outStatus, outSizes, n, tIns[0]);
   auto st = (uint8_t*)(outStatus ? outStatus->data_ptr() : nullptr);
   auto sz = (uint32_t*)(outSizes ? outSizes->data_ptr() : nullptr);
-  auto stream = at::cuda::getCurrentCUDAStream();
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (asFloat) {
-    auto ft = floatTypeOf(tOut);
-    Scratch sc(tempMem, tIns[0], dgb_float_decompress_temp_bytes((int)ft, n, 0));
-    FloatDecompressConfig cfg(ft, ANSCodecConfig(kPrecision, false), false, checksum);
-    auto status = floatDecompressSplitSize(sc.res, cfg, n, in.data(), tOut.data_ptr(), split.data(), st, sz, stream);
-    TORCH_CHECK(status.error != FloatDecompressError::ChecksumMismatch,
-                "floatDecompress: checksum mismatch seen on decoded data; archive cannot be unpacked");
-    return sc.res.getMaxMemoryUsage();
+    Scratch sc(tempMem, tIns[0], dgb_float_decompress_temp_bytes(ft, n, 0), stream);
+    checkDecodeRc(dgb_float_decompress_split_size(sc.ptr(), sc.bytes(), ft, kPrecision, checksum, n, in.data(),
+                                                  tOut.data_ptr(), split.data(), st, sz, nullptr, stream),
+                  true, "decompress_data_split_size");
+    return sc.used();
   }
-  Scratch sc(tempMem, tIns[0], dgb_ans_decode_temp_bytes(n));
-  auto status = ansDecodeBatchSplitSize(sc.res, ANSCodecConfig(kPrecision, checksum), n, in.data(), tOut.data_ptr(),
-                                        split.data(), st, sz, stream);
-  TORCH_CHECK(status.error != ANSDecodeError::ChecksumMismatch,
-              "ANSDecode: checksum mismatch seen on decoded data; archive cannot be unpacked");
-  return sc.res.getMaxMemoryUsage();
+  Scratch sc(tempMem, tIns[0], dgb_ans_decode_temp_bytes(n), stream);
+  checkDecodeRc(dgb_ans_decode_split_size(sc.ptr(), sc.bytes(), kPrecision, checksum, n, in.data(), tOut.data_ptr(),
+                                          split.data(), st, sz, nullptr, stream),
+                false, "decompress_data_split_size");
+  return sc.used();
 }
 
 std::vector<Tensor> decompress_data_simple(bool asFloat, const std::vector<Tensor>& tIns, bool checksum,
@@ -329,22 +381,25 @@ std::vector<Tensor> decompress_data_simple(bool asFloat, const std::vector<Tenso
   std::vector<const void*> in(n);
   for (int64_t i = 0; i < n; ++i) {
     TORCH_CHECK(tIns[i].is_cuda() && tIns[i].get_device() == tIns[0].get_device());
+    checkArchiveAligned(tIns[i]);
     in[i] = tIns[i].data_ptr();
   }
   {
-    Scratch sc(std::nullopt, tIns[0], sizeof(void*) * n + 512);
-    auto stream = at::cuda::getCurrentCUDAStream();
-    if (asFloat)
-      floatGetCompressedInfo(sc.res, in.data(), n, (uint32_t*)sizes.data_ptr(), (uint32_t*)types.data_ptr(), nullptr, stream);
-    else
-      ansGetCompressedInfo(sc.res, in.data(), n, (uint32_t*)sizes.data_ptr(), nullptr, stream);
+    cudaStream_t stream = at::cuda::getCurrentCUDAStream();
+    Scratch sc(std::nullopt, tIns[0], sizeof(void*) * n + 256, stream);
+    checkRc(asFloat ? dgb_float_get_compressed_info(sc.ptr(), sc.bytes(), in.data(), 0, n, (uint32_t*)sizes.data_ptr(),
+                                                    (uint32_t*)types.data_ptr(), nullptr, stream)
+                    : dgb_ans_get_compressed_info(sc.ptr(), sc.bytes(), in.data(), 0, n, (uint32_t*)sizes.data_ptr(),
+                                                  nullptr, stream),
+            "get_compressed_info");
   }
   auto hs = sizes.to(torch::kCPU), ht = types.to(torch::kCPU);
   std::vector<Tensor> outs;
   for (int64_t i = 0; i < n; ++i) {
     auto size = hs.data_ptr<int32_t>()[i];
     if (asFloat) {
-      TORCH_CHECK(ht.data_ptr<int32_t>()[i] == ht.data_ptr<int32_t>()[0]);
+      TORCH_CHECK(ht.data_ptr<int32_t>()[i] == ht.data_ptr<int32_t>()[0],
+                  "dietgpu: inconsistent / invalid float type in archives");
       outs.push_back(torch::empty({size}, opts.dtype(dtypeOf((FloatType)ht.data_ptr<int32_t>()[i]))));
     } else {
       outs.push_back(torch::empty({size}, opts.dtype(torch::kByte)));

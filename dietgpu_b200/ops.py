@@ -13,6 +13,11 @@ memory, streams and dtypes; all compute is in libdietgpu_b200.so.
 
 Python's precision is fixed at 10 bits as in the reference (DietGpu.cpp:114);
 `prob_bits=` is an extension used by the parity tests (C++ API parity).
+
+Where the reference would write or read memory the caller did not hand over, this layer (and the C++
+operators, which raise for the same inputs) differs on purpose: byte batches of mixed dtypes get rows sized
+by their largest member in bytes, split sizes must fit the tensor they index, float outputs must share one
+dtype, and archives and output rows must be 16 B aligned.
 """
 from __future__ import annotations
 
@@ -42,13 +47,23 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-def _total_and_max(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
-    total = mx = 0
+def _max_numel_and_bytes(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
+    """Largest member in elements and, separately, in bytes (a byte batch may mix dtypes)."""
+    mx = mx_bytes = 0
     for t in ts:
         _check(t.numel() * t.element_size() <= 0xFFFFFFFF, "tensor exceeds 4 GiB - 1")
-        total += t.numel()
         mx = max(mx, t.numel())
-    return total, mx
+        mx_bytes = max(mx_bytes, t.numel() * t.element_size())
+    return mx, mx_bytes
+
+
+def _check_archive_aligned(t: torch.Tensor) -> None:
+    _check(t.data_ptr() % 16 == 0, "compressed input is not 16 B aligned")
+
+
+def _split_total(splits: Sequence[int], capacity: int, what: str) -> None:
+    total = sum(splits)
+    _check(total <= capacity, f"split sizes sum to {total}, more than {what} holds ({capacity})")
 
 
 class _Temp:
@@ -83,7 +98,7 @@ def _bound(v: int, size: int) -> int:
 
 
 def max_float_compressed_output_size(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
-    _, mx = _total_and_max(ts)
+    mx, _ = _max_numel_and_bytes(ts)
     return len(ts), _bound(capi.lib().dgb_float_max_compressed_size(_float_type(ts[0]), mx), mx)
 
 
@@ -92,8 +107,10 @@ def max_float_compressed_size(dtype: torch.Tensor, size: int) -> int:
 
 
 def max_any_compressed_output_size(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
-    _, mx = _total_and_max(ts)
-    return len(ts), _bound(capi.lib().dgb_ans_max_compressed_size(mx * ts[0].element_size()), mx)
+    # rows sized by the largest member in bytes; the reference multiplies the largest element count by
+    # the first member's element size (DietGpu.cpp:134), too small for a batch of mixed dtypes
+    _, mx_bytes = _max_numel_and_bytes(ts)
+    return len(ts), _bound(capi.lib().dgb_ans_max_compressed_size(mx_bytes), mx_bytes)
 
 
 def max_any_compressed_size(nbytes: int) -> int:
@@ -108,6 +125,8 @@ def _validate_out(out_compressed, out_sizes, n: int, cols: int, dev):
                and out_compressed.is_contiguous() and out_compressed.dim() == 2)
         _check(out_compressed.size(0) >= n and out_compressed.size(1) >= cols)
         _check(out_compressed.device == dev)
+        _check(out_compressed.data_ptr() % 16 == 0 and (n <= 1 or out_compressed.size(1) % 16 == 0),
+               "out_compressed rows are not 16 B aligned")
         comp = out_compressed
     else:
         comp = torch.empty((n, cols), dtype=torch.uint8, device=dev)
@@ -182,6 +201,8 @@ def compress_data_split_size(compress_as_float: bool, t_in: torch.Tensor, t_in_s
         _check(s > 0)
         if not compress_as_float and i != n - 1:
             _check(s % 4 == 0, "the size of an interior split is not a multiple of 4 bytes")
+    # splits count words of t_in's dtype for floats, bytes otherwise
+    _split_total(splits, t_in.numel() if compress_as_float else t_in.numel() * t_in.element_size(), "t_in")
     mx = max(splits)
     L = capi.lib()
     cols = _bound(L.dgb_float_max_compressed_size(ft, mx) if compress_as_float else L.dgb_ans_max_compressed_size(mx), mx)
@@ -267,9 +288,12 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
     caps = []
     for ti, to in zip(ts_in, ts_out):
         _check(ti.is_cuda and ti.device == dev and ti.is_contiguous() and ti.dtype == torch.uint8)
+        _check_archive_aligned(ti)
         _check(to.is_cuda and to.device == dev and to.is_contiguous())
         if compress_as_float:
             _float_type(to)
+            # capacities are counted in words of one float type
+            _check(to.dtype == ts_out[0].dtype, "float outputs must all have the same dtype")
         cap = to.numel() if compress_as_float else to.numel() * to.element_size()
         _check(cap <= 0xFFFFFFFF)
         caps.append(cap)
@@ -309,9 +333,12 @@ def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Te
     splits = t_out_split_sizes.tolist()
     for ti, s in zip(ts_in, splits):
         _check(ti.is_cuda and ti.device == dev and ti.is_contiguous() and ti.dtype == torch.uint8)
+        _check_archive_aligned(ti)
         _check(s > 0)
-    _check(t_out.is_cuda and t_out.device == dev and t_out.is_contiguous())
+    _check(t_out.is_cuda and t_out.is_contiguous())
+    _check(t_out.device == dev, "t_out is not on the device of the compressed inputs")
     ft = _float_type(t_out) if compress_as_float else 0
+    _split_total(splits, t_out.numel() if compress_as_float else t_out.numel() * t_out.element_size(), "t_out")
     st_ptr, sz_ptr = _validate_status(out_status, out_decompressed_words, n, dev)
     L = capi.lib()
     in_ptrs = capi.ptr_array([t.data_ptr() for t in ts_in])
@@ -338,6 +365,7 @@ def decompress_data_simple(compress_as_float: bool, ts_in: Sequence[torch.Tensor
     n = len(ts_in)
     for t in ts_in:
         _check(t.is_cuda and t.device == dev)
+        _check_archive_aligned(t)
     L = capi.lib()
     sizes = torch.empty(n, dtype=torch.int32, device=dev)
     types = torch.zeros(n, dtype=torch.int32, device=dev)
