@@ -293,7 +293,7 @@ void timerEnd(const Options& opt, int slot, cudaStream_t stream) {
 
 namespace {
 
-bool validFloatType(int ft) { return ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32; }
+bool validFloatType(int ft) { return ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32 || ft == DGB_FLOAT64; }
 
 // the calling thread's member list, sized for n members
 HostMember* stageMembers(uint32_t n) {
@@ -348,8 +348,7 @@ uint32_t dgb_float_max_compressed_size(int ft, uint32_t n) {
   if (!validFloatType(ft)) return 0;
   const uint32_t ans = dgb_ans_max_compressed_size(n);
   if (ans == 0u) return 0u;  // too large (see above)
-  const uint64_t non = ft == DGB_FLOAT32 ? 2ull * roundUp64(n, 8) + roundUp64(n, 16) : roundUp64(n, 16);
-  const uint64_t total = (uint64_t)kFloatHeaderBytes + ans + non;
+  const uint64_t total = (uint64_t)kFloatHeaderBytes + ans + floatPlanesBytes<uint64_t>(ft, n);
   return total <= 0xffffffffull ? (uint32_t)total : 0u;
 }
 
@@ -546,8 +545,7 @@ int dgb_copy_rows_async(void* dst, size_t dst_pitch, const void* src, size_t src
 
 int dgb_archives_pull(int float_type, uint32_t num_in_batch, const void* const* src, void* const* dst,
                       const uint32_t* dst_capacity, uint32_t* out_bytes_dev, void* stream) {
-  if (float_type != 0 && float_type != DGB_FLOAT16 && float_type != DGB_BFLOAT16 && float_type != DGB_FLOAT32)
-    return DGB_ERR_INVALID_ARG;
+  if (float_type != 0 && !validFloatType(float_type)) return DGB_ERR_INVALID_ARG;
   return dgb::pullArchives(float_type, num_in_batch, src, dst, dst_capacity, out_bytes_dev, (cudaStream_t)stream);
 }
 

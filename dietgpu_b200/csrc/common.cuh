@@ -35,18 +35,45 @@ __host__ __device__ constexpr uint32_t ansOverhead(uint32_t numBlocks) {
   return kAnsHeaderBytes + kAnsPdfBytes + 128u * numBlocks + 8u * roundUp(numBlocks, 2u);
 }
 
-// float/GpuFloatUtils.cuh:123-127,163-167,194-203 (bytes of the stored,
-// non-compressed part, 16 B padded)
-__host__ __device__ constexpr uint32_t floatNonCompBytes(int ft, uint32_t n) {
-  return ft == DGB_FLOAT32 ? 2u * roundUp(n, 8u) + roundUp(n, 16u) : roundUp(n, 16u);
+// Stored ("non-compressed") planes of a float archive, in this order after the 16 B float header, each
+// starting 16 B aligned and zero padded (float/GpuFloatUtils.cuh:123-127,163-167,194-203 for types 1-3):
+//   fp16, bf16 : u8 plane
+//   fp32       : u16 plane, u8 plane
+//   fp64       : u32 plane, u16 plane, u8 plane  (type 4, an extension the reference does not have)
+// Byte offsets relative to the first plane, in T: uint32_t on the device (every offset inside an archive
+// fits 32 bits), uint64_t for the host's size bounds, which must see totals that do not.
+template <class T>
+__host__ __device__ constexpr T roundUpT(T a, T b) { return (a + b - 1) / b * b; }
+template <class T>
+__host__ __device__ constexpr T floatU16PlaneOffset(int ft, T n) {  // fp32, fp64
+  return ft == DGB_FLOAT64 ? T(4) * roundUpT<T>(n, 4) : T(0);
 }
+template <class T>
+__host__ __device__ constexpr T floatU8PlaneOffset(int ft, T n) {
+  return ft == DGB_FLOAT64   ? T(4) * roundUpT<T>(n, 4) + T(2) * roundUpT<T>(n, 8)
+         : ft == DGB_FLOAT32 ? T(2) * roundUpT<T>(n, 8)
+                             : T(0);
+}
+template <class T>
+__host__ __device__ constexpr T floatPlanesBytes(int ft, T n) {
+  return ft == DGB_FLOAT64   ? T(4) * roundUpT<T>(n, 4) + T(2) * roundUpT<T>(n, 8) + roundUpT<T>(n, 16)
+         : ft == DGB_FLOAT32 ? T(2) * roundUpT<T>(n, 8) + roundUpT<T>(n, 16)
+                             : roundUpT<T>(n, 16);
+}
+__host__ __device__ constexpr uint32_t floatNonCompBytes(int ft, uint32_t n) { return floatPlanesBytes<uint32_t>(ft, n); }
 
 // Worst-case u16 words one 4 KiB block can emit: every symbol costs at most
 // probBits bits (a symbol of pdf 1), so 4096*pb/16 words; +8 for 16 B padding.
 __host__ __device__ constexpr uint32_t maxBlockWords(int pb) { return 256u * (uint32_t)pb + 8u; }
 
 // ---- per-member descriptor (device), built on the host ----------------------
-enum CodecKind : int { kKindBytes = 0, kKindF16 = DGB_FLOAT16, kKindBF16 = DGB_BFLOAT16, kKindF32 = DGB_FLOAT32 };
+enum CodecKind : int {
+  kKindBytes = 0,
+  kKindF16 = DGB_FLOAT16,
+  kKindBF16 = DGB_BFLOAT16,
+  kKindF32 = DGB_FLOAT32,
+  kKindF64 = DGB_FLOAT64
+};
 
 struct MemberDesc {
   const void* in;     // encode: raw input (bytes / float words); decode: archive
@@ -139,7 +166,9 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
 
 void setLastCudaError(cudaError_t e);
 
-inline uint32_t wordBytes(int kind) { return kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u); }
+inline uint32_t wordBytes(int kind) {
+  return kind == kKindF64 ? 8u : (kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u));
+}
 inline size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
 int smCount();  // SMs of the current device, cached per device
 
@@ -216,6 +245,7 @@ int withKind(int kind, F&& f) {
     case kKindF16: return f(IntC<kKindF16>{});
     case kKindBF16: return f(IntC<kKindBF16>{});
     case kKindF32: return f(IntC<kKindF32>{});
+    case kKindF64: return f(IntC<kKindF64>{});
     default: return DGB_ERR_INVALID_ARG;
   }
 }
@@ -319,6 +349,12 @@ template <int OFF>
 __device__ __forceinline__ uint32_t ldsU16(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u16 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
+  return v;
+}
+template <int OFF>
+__device__ __forceinline__ uint32_t ldsU32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
   return v;
 }
 // block-wide exclusive scan of one value per thread for THREADS threads

@@ -1,5 +1,5 @@
 // decode.cu -- batched rANS decode (bytes) and fused float decompress
-// (fp16/bf16/fp32) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
+// (fp16/bf16/fp32/fp64) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
 // whose CTAs lease members (header checks and the 2^pb LUT from the archive's own pdf happen inside the
 // CTA) and whose warps claim 4 KiB blocks; lane states + compressed words of a block arrive by one TMA
 // bulk copy (cp.async.bulk + mbarrier), the 32-lane interleaved rANS decode of ans/GpuANSDecode.cuh:55-217
@@ -199,6 +199,67 @@ struct RowWriter16 {
 };
 template <> struct RowWriter<kKindF16> : RowWriter16<kKindF16> {};
 template <> struct RowWriter<kKindBF16> : RowWriter16<kKindBF16> {};
+
+template <>
+struct RowWriter<kKindF64> {
+  // per group: rows x 128 B of the u32 plane, rows x 64 B of the u16 plane, rows x 32 B of the u8 plane
+  static constexpr uint32_t kRingSlotBytes = kGroupRows * 224;
+  unsigned long long* out;
+  const uint32_t* non4;
+  const uint16_t* non2;
+  const uint8_t* non1;
+  const uint8_t* copy4;
+  const uint8_t* copy2;
+  const uint8_t* copy1;
+  uint32_t ring, lane;
+  struct Cursor { unsigned long long* o; uint32_t s4, s2, s1; };
+  __device__ __forceinline__ void setRing(uint32_t ringAddr, uint32_t l) { ring = ringAddr; lane = l; }
+  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
+    out = static_cast<unsigned long long*>(outBase) + (size_t)block * kBlockBytes + l;
+    const uint8_t* p4 = av.non + 4u * (size_t)block * kBlockBytes;
+    const uint8_t* p2 = av.non + floatU16PlaneOffset<uint32_t>(kKindF64, av.floatWords) + 2u * (size_t)block * kBlockBytes;
+    const uint8_t* p1 = av.non + floatU8PlaneOffset<uint32_t>(kKindF64, av.floatWords) + (size_t)block * kBlockBytes;
+    non4 = reinterpret_cast<const uint32_t*>(p4) + l;
+    non2 = reinterpret_cast<const uint16_t*>(p2) + l;
+    non1 = p1 + l;
+    copy4 = p4 + l * 16u;
+    copy2 = p2 + l * 16u;
+    copy1 = p1 + l * 16u;
+    __builtin_assume(__isGlobal(out));
+    __builtin_assume(__isGlobal(non4));
+    __builtin_assume(__isGlobal(non2));
+    __builtin_assume(__isGlobal(non1));
+    __builtin_assume(__isGlobal(copy4));
+    __builtin_assume(__isGlobal(copy2));
+    __builtin_assume(__isGlobal(copy1));
+  }
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    const uint32_t base = ring + slot * kRingSlotBytes;
+    return Cursor{out + row * 32u, base + lane * 4u, base + kGroupRows * 128 + lane * 2u, base + kGroupRows * 192 + lane};
+  }
+  __device__ __forceinline__ void issue(uint32_t row, uint32_t slot) const {
+    const uint32_t base = ring + slot * kRingSlotBytes;
+#pragma unroll
+    for (int h = 0; h < kGroupRows / 4; ++h)  // 32 lanes x 16 B = 4 rows x 128 B per copy
+      cpAsync16(base + h * 512 + lane * 16u, copy4 + row * 128u + h * 512);
+#pragma unroll
+    for (int h = 0; h < kGroupRows / 8; ++h)
+      cpAsync16(base + kGroupRows * 128 + h * 512 + lane * 16u, copy2 + row * 64u + h * 512);
+    if (lane < (uint32_t)(kGroupRows * 2)) cpAsync16(base + kGroupRows * 192 + lane * 16u, copy1 + row * 32u);
+  }
+  static __device__ __forceinline__ unsigned long long join(uint32_t entry, uint32_t lo, uint32_t mid, uint32_t hi) {
+    // (comp << 56 | stored 56 bits) rotated right by one; the high half is built as fp32's join builds its word
+    const uint32_t h = __byte_perm(mid, __byte_perm(hi, entry, 0x0040), 0x5410);
+    return ((unsigned long long)__funnelshift_r(h, lo, 1) << 32) | __funnelshift_r(lo, h, 1);
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = join(entry, ldsU32<J * 128>(c.s4), ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    out[row * 32u] = join(entry, __ldg(non4 + row * 32u), __ldg(non2 + row * 32u), __ldg(non1 + row * 32u));
+  }
+};
 
 template <>
 struct RowWriter<kKindF32> {
@@ -767,7 +828,9 @@ DecodePlan planDecodeScratch(uint32_t n) {
 // inside the kernel.
 template <int KIND, int PB>
 size_t decoderSmem(int warps, const Options& opt, uint32_t* slotWords) {
-  uint32_t slot = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words : (KIND == kKindBytes ? maxBlockWords(PB) : 1536u);
+  // fp64's stored-plane ring is 10.5 KiB per warp: with a 1024-word slot two 8-warp CTAs fit on an SM
+  uint32_t slot = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words
+                                            : (KIND == kKindBytes ? maxBlockWords(PB) : (KIND == kKindF64 ? 1024u : 1536u));
   slot = std::min(roundUp(slot, 8u), maxBlockWords(PB));
   *slotWords = slot;
   return (2 * kNumSymbols + 64) * 4 + ((warps + 1) & ~1) * 8 + (size_t)warps * kRingSlots * RowWriter<KIND>::kRingSlotBytes +
@@ -996,7 +1059,7 @@ __device__ __forceinline__ uint4 ldgNc(const uint4* p) {
 constexpr uint32_t kPullThreads = 512;
 constexpr uint32_t kPullChunkVecs = 4096;  // 64 KiB work units
 
-__device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {
+__device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {  // inlined: kind folds where it is constant
   uint32_t extra = 0;
   if (kind != kKindBytes) {
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(a));
@@ -1009,8 +1072,7 @@ __device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {
   return total > 0xfffffff0ull ? 32u : (uint32_t)total;
 }
 
-__global__ void __launch_bounds__(kPullThreads)
-pullArchivesKernel(const __grid_constant__ InlineMembers im, int kind, uint32_t* __restrict__ outBytes) {
+__device__ __forceinline__ void pullArchivesBody(const InlineMembers& im, int kind, uint32_t* __restrict__ outBytes) {
   __shared__ uint32_t sFirst[kInlineMembers + 1];  // first chunk of member i
   __shared__ uint32_t sBytes[kInlineMembers];
   const uint32_t t = threadIdx.x, n = im.count;
@@ -1044,6 +1106,18 @@ pullArchivesKernel(const __grid_constant__ InlineMembers im, int kind, uint32_t*
     for (; v < v1; v += kPullThreads) dst[v] = ldgNc(src + v);
   }
 }
+
+// byte, fp16, bf16 and fp32 archives (kind at run time)
+__global__ void __launch_bounds__(kPullThreads)
+pullArchivesKernel(const __grid_constant__ InlineMembers im, int kind, uint32_t* __restrict__ outBytes) {
+  __builtin_assume(kind != kKindF64);
+  pullArchivesBody(im, kind, outBytes);
+}
+// fp64 archives: their own instantiation, so the kernel above keeps its plane-size arithmetic
+__global__ void __launch_bounds__(kPullThreads)
+pullArchivesF64Kernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
+  pullArchivesBody(im, kKindF64, outBytes);
+}
 }  // namespace
 
 int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst, const uint32_t* capacity,
@@ -1065,7 +1139,11 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
       im.m[i].work0 = 0;
     }
     timerBegin(opt, kSlotPull, stream);
-    pullArchivesKernel<<<ctas, kPullThreads, 0, stream>>>(im, kind, outBytes_dev ? outBytes_dev + i0 : nullptr);
+    uint32_t* ob = outBytes_dev ? outBytes_dev + i0 : nullptr;
+    if (kind == kKindF64)
+      pullArchivesF64Kernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
+    else
+      pullArchivesKernel<<<ctas, kPullThreads, 0, stream>>>(im, kind, ob);
     DGB_CUDA_TRY(cudaGetLastError());
     timerEnd(opt, kSlotPull, stream);
   }

@@ -1,4 +1,4 @@
-// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32)
+// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64)
 // for sm_90a (H100).  Two launches per call, whatever the batch size:
 //
 //   K1  stats*Kernel     a pure read of the raw input: 256-bin histogram of the coded byte, taken out of
@@ -297,6 +297,8 @@ statsBytesKernel(EncodeScratch sc, const __grid_constant__ InlineMembers im, con
 //   bf16 : w' = rotl16(w, 1); comp = w' >> 8, non = w' & 0xff
 //   fp32 : w' = rotl32(w, 1); comp = w' >> 24, non = w' & 0xffffff
 //          stored as a u16 plane (low 16 bits) then a u8 plane (bits 16..23)
+//   fp64 : v = rotl64(w, 1); comp = v >> 56 (exponent bits 10..3), non = the low 56 bits, stored as a u32,
+//          a u16 and a u8 plane; comp is fp32's coded byte taken from the word's high 32-bit half
 // ---------------------------------------------------------------------------
 template <int FT>
 __device__ __forceinline__ uint32_t rot16x2(uint32_t w) {
@@ -327,8 +329,8 @@ __host__ __device__ inline uint32_t floatSlabs(const void* in, uint32_t size, ui
 // element in bits [LO, LO + 16) of a packed 16-bit pair, or of a 32-bit word: one shift, one mask.
 //   fp16 coded = w >> 8, bf16 coded = (w >> 7) & 0xff, fp32 coded = (w >> 23) & 0xff
 template <int FT>
-__device__ __forceinline__ uint32_t histOffLo(uint32_t w) {  // low half (or the whole fp32 word)
-  return FT == DGB_FLOAT32 ? (w >> 21) & 0x3fcu : (w >> (FT == DGB_BFLOAT16 ? 5 : 6)) & 0x3fcu;
+__device__ __forceinline__ uint32_t histOffLo(uint32_t w) {  // low half (or the whole fp32 word, or fp64's high half)
+  return FT == DGB_FLOAT32 || FT == DGB_FLOAT64 ? (w >> 21) & 0x3fcu : (w >> (FT == DGB_BFLOAT16 ? 5 : 6)) & 0x3fcu;
 }
 template <int FT>
 __device__ __forceinline__ uint32_t histOffHi(uint32_t w) {  // high half of a 16-bit pair
@@ -339,6 +341,7 @@ __device__ __forceinline__ void histAdd(uint32_t* wh, uint32_t byteOff) {
 }
 template <int FT>
 __device__ __forceinline__ uint32_t codedScalar(const uint8_t* in, uint32_t e) {
+  if (FT == DGB_FLOAT64) return (reinterpret_cast<const uint32_t*>(in)[2u * (size_t)e + 1u] >> 23) & 0xffu;
   if (FT == DGB_FLOAT32) return (reinterpret_cast<const uint32_t*>(in)[e] >> 23) & 0xffu;
   const uint32_t w = reinterpret_cast<const uint16_t*>(in)[e];
   return FT == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8;
@@ -360,6 +363,11 @@ __device__ __forceinline__ void histVectors(const uint4* __restrict__ vec, const
     for (int k = 0; k < kStatsUnroll; ++k) {
       const uint32_t i = i0 + k * kStatsThreads;
       if (i >= v1) break;
+      if (FT == DGB_FLOAT64) {  // two words per vector: the coded byte is in each odd 32-bit half
+        histAdd(wh, histOffLo<FT>(vv[k].y));
+        histAdd(wh, histOffLo<FT>(vv[k].w));
+        continue;
+      }
       const uint32_t w4[4] = {vv[k].x, vv[k].y, vv[k].z, vv[k].w};
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
@@ -377,8 +385,8 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
                                                uint32_t m, uint32_t y,
                                                uint32_t Y, uint32_t* __restrict__ outSize,
                                                const StatsStage& stage = StatsStage()) {
-  constexpr uint32_t EPV = (FT == DGB_FLOAT32) ? 4u : 8u;  // elements per 16 B vector
-  constexpr uint32_t WB = (FT == DGB_FLOAT32) ? 4u : 2u;   // word bytes
+  constexpr uint32_t EPV = (FT == DGB_FLOAT64) ? 2u : (FT == DGB_FLOAT32) ? 4u : 8u;  // elements per 16 B vector
+  constexpr uint32_t WB = 16u / EPV;                                                 // word bytes
   // shuffle => the histogram base is provably warp-uniform (ATOMS [R + UR], no per-symbol add)
   const uint32_t t = threadIdx.x, warp = __shfl_sync(0xffffffffu, t >> 5, 0);
   const uint8_t* in = static_cast<const uint8_t*>(md.in);
@@ -434,7 +442,12 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
         *reinterpret_cast<uint4*>(archive) =
             make_uint4(kFloatMagicVersion, size, (uint32_t)FT | ((useChecksum ? 1u : 0u) << 4), 0u);
       }
-      if (FT == DGB_FLOAT32) {
+      if (FT == DGB_FLOAT64) {
+        const uint32_t p16 = floatU16PlaneOffset<uint32_t>(FT, size), p8 = floatU8PlaneOffset<uint32_t>(FT, size);
+        for (uint32_t i = 4u * size + t; i < p16; i += kStatsThreads) non[i] = 0;
+        for (uint32_t i = p16 + 2u * size + t; i < p8; i += kStatsThreads) non[i] = 0;
+        for (uint32_t i = p8 + size + t; i < nonBytes; i += kStatsThreads) non[i] = 0;
+      } else if (FT == DGB_FLOAT32) {
         const uint32_t p16 = 2u * roundUp(size, 8u);
         for (uint32_t i = 2u * size + t; i < p16; i += kStatsThreads) non[i] = 0;
         for (uint32_t i = p16 + size + t; i < nonBytes; i += kStatsThreads) non[i] = 0;
@@ -443,7 +456,7 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
       }
     }
     if (useChecksum) {
-      // SURVEY A.6 / B6: the float checksum covers the first `size` BYTES only
+      // SURVEY A.6 / B6: the float checksum covers the first `size` BYTES only (fp64: the first size / 8 words)
       const uint32_t cbytes = size;  // bytes, not words
       for (uint32_t i = y * kStatsThreads + t; i < cbytes; i += participants * kStatsThreads)
         xorAcc ^= in[i];
@@ -529,10 +542,12 @@ constexpr int kEncGroupRows = DGB_ENC_GROUP_ROWS;  // rows per cp.async group
 //   fp16 : coded = w >> 8,        stored = w & 0xff                     (float/GpuFloatUtils.cuh:111-119)
 //   bf16 : coded = (w >> 7) & ff, stored = (w & 7f) << 1 | w >> 15      (:141-159)
 //   fp32 : coded = (w >> 23) & ff, stored = low 24 bits of rotl(w, 1): u16 plane then u8 plane (:181-203)
+//   fp64 : coded = (hi >> 23) & ff, stored = low 56 bits of rotl64(w, 1): u32, u16 then u8 plane
 // ---------------------------------------------------------------------------
 struct StoredPlanes {
-  uint8_t* non;   // fp16 / bf16: the stored byte plane; fp32: the u16 plane
-  uint8_t* non1;  // fp32: the u8 plane
+  uint8_t* non;   // fp16 / bf16: the stored byte plane; fp32: the u16 plane; fp64: the u32 plane
+  uint8_t* non1;  // fp32: the u8 plane; fp64: the u16 plane
+  uint8_t* non2;  // fp64: the u8 plane
 };
 
 template <int KIND>
@@ -647,9 +662,62 @@ struct EncIn<kKindF32> {
   }
 };
 
+#ifndef DGB_ENC_RING64
+#define DGB_ENC_RING64 3
+#endif
+// fp64: 16 rows x 32 lanes x 8 B = 4 KiB per group, so the ring bounds the coder CTAs per SM
+template <>
+struct EncIn<kKindF64> {
+  static constexpr uint32_t kWordBytes = 8, kRingSlots = DGB_ENC_RING64;
+  template <uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffsetOf(unsigned long long w) {
+    return EncIn<kKindF32>::tabOffsetOf<STRIDE>((uint32_t)(w >> 32));
+  }
+  template <int J, uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffset(uint32_t ringLane) {
+    // only the high half of the lane's word holds coded bits
+    uint32_t w;
+    asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(w) : "r"(ringLane), "n"(J * 256 + 4));
+    return EncIn<kKindF32>::tabOffsetOf<STRIDE>(w);
+  }
+  static __device__ __forceinline__ unsigned long long loadWord(const uint8_t* in, uint32_t e) {
+    return __ldg(reinterpret_cast<const unsigned long long*>(in) + e);
+  }
+  static __device__ __forceinline__ void storeScalar(const StoredPlanes& pl, uint32_t e, unsigned long long w) {
+    const unsigned long long v = (w << 1) | (w >> 63);
+    reinterpret_cast<uint32_t*>(pl.non)[e] = (uint32_t)v;
+    reinterpret_cast<uint16_t*>(pl.non1)[e] = (uint16_t)(v >> 32);
+    pl.non2[e] = (uint8_t)(v >> 48);
+  }
+  // one group of 16 rows = 512 words = 4 KiB in the ring slot: lane l handles words 4 (l + 32 h) .. +3, so
+  // every plane gets one vector store per lane and step (16 B, 8 B, 4 B)
+  static __device__ __forceinline__ void storeGroup(uint32_t slot, const StoredPlanes& pl, uint32_t elem0,
+                                                    uint32_t lane) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const uint32_t q = lane + 32u * h;
+      uint4 a, b;
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "r"(slot + q * 32u));
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "r"(slot + q * 32u + 16u));
+      // rotl64 by one of (hi:lo): lo' = lo << 1 | hi >> 31, hi' = hi << 1 | lo >> 31
+      const uint4 lo = make_uint4(__funnelshift_l(a.y, a.x, 1), __funnelshift_l(a.w, a.z, 1), __funnelshift_l(b.y, b.x, 1),
+                                  __funnelshift_l(b.w, b.z, 1));
+      const uint32_t h0 = __funnelshift_l(a.x, a.y, 1), h1 = __funnelshift_l(a.z, a.w, 1);
+      const uint32_t h2 = __funnelshift_l(b.x, b.y, 1), h3 = __funnelshift_l(b.z, b.w, 1);
+      const uint32_t e = elem0 + q * 4u;
+      *reinterpret_cast<uint4*>(pl.non + 4u * (size_t)e) = lo;
+      *reinterpret_cast<uint2*>(pl.non1 + 2u * (size_t)e) = make_uint2(__byte_perm(h0, h1, 0x5410), __byte_perm(h2, h3, 0x5410));
+      *reinterpret_cast<uint32_t*>(pl.non2 + e) =
+          __byte_perm(__byte_perm(h0, h1, 0x0062), __byte_perm(h2, h3, 0x0062), 0x5410);
+    }
+  }
+};
+
 __host__ __device__ constexpr uint32_t encRingBytes(int kind) {
-  return kind == kKindBytes ? 4u * kEncGroupRows * 32u
-                            : (kind == kKindF32 ? 3u * kEncGroupRows * 128u : (uint32_t)DGB_ENC_RING16 * kEncGroupRows * 64u);
+  return kind == kKindF64 ? (uint32_t)DGB_ENC_RING64 * kEncGroupRows * 256u
+         : kind == kKindBytes
+             ? 4u * kEncGroupRows * 32u
+             : (kind == kKindF32 ? 3u * kEncGroupRows * 128u : (uint32_t)DGB_ENC_RING16 * kEncGroupRows * 64u);
 }
 
 // One rANS step for a full row (ans/GpuANSEncode.cuh:49-90 restated).  The
@@ -871,6 +939,9 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   constexpr uint32_t kGroupBytes = U * 32 * WB;     // 512 B, 1 KiB or 2 KiB
   constexpr uint32_t kChunks = kGroupBytes / 512u;  // 16 B copies per lane and group
   constexpr uint32_t kStride = EncSym<WIDE>::kStride;
+  // groups in flight ahead of the one being coded: two, or one in a two-slot ring
+  constexpr uint32_t kAhead = In::kRingSlots > 2 ? 2u : 1u;
+  static_assert(In::kRingSlots >= 2 && (!TMA || kAhead == 2), "");
   uint32_t state = kStateMin;
   uint32_t wa = stageAddr;
   const EncRegs rc = makeEncRegs(tabAddr, pb);
@@ -916,16 +987,18 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
       };
       if (groups > 0) issue(0, 0);
       cpAsyncCommit();
-      if (groups > 1) issue(1, 1);
-      cpAsyncCommit();
-      uint32_t slot = 0, slotNext = 2 % In::kRingSlots;
+      if (kAhead > 1) {
+        if (groups > 1) issue(1, 1);
+        cpAsyncCommit();
+      }
+      uint32_t slot = 0, slotNext = kAhead % In::kRingSlots;
       for (uint32_t k = 0; k < groups; ++k) {
         if (sp.area && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
-        cpAsyncWait<1>();  // group k has landed (group k + 1 may still be in flight)
+        cpAsyncWait<kAhead - 1>();  // group k has landed (group k + 1 may still be in flight)
         // one warp barrier does both jobs: every lane sees group k, and every lane is done reading group
-        // k - 1, whose ring slot (three-slot ring) the request below overwrites
+        // k - 1, whose ring slot the request below overwrites
         __syncwarp();
-        if (k + 2 < groups) issue(k + 2, slotNext);
+        if (k + kAhead < groups) issue(k + kAhead, slotNext);
         cpAsyncCommit();
         const uint32_t slotAddr = ringAddr + slot * kGroupBytes;
         if (KIND != kKindBytes) In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
@@ -941,7 +1014,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   uint32_t e = r * 32u + lane;
   for (uint32_t j = 0; r < fullRows; ++r, ++j, e += 32) {
     if (sp.area && (j % U) == 0 && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
-    const uint32_t w = In::loadWord(in, e);
+    const auto w = In::loadWord(in, e);
     In::storeScalar(planes, elem0 + e, w);
     encodeStep<WIDE>(state, In::template tabOffsetOf<kStride>(w), rc, wa);
   }
@@ -949,7 +1022,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   if (rem) {
     if (sp.area && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
     const bool valid = lane < rem;
-    const uint32_t w = valid ? In::loadWord(in, e) : 0u;
+    const auto w = valid ? In::loadWord(in, e) : 0u;
     if (valid) In::storeScalar(planes, elem0 + e, w);
     encodeStepPartial<WIDE>(valid, state, In::template tabOffsetOf<kStride>(w), rc, wa);
   }
@@ -1045,7 +1118,7 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
     const uint8_t* ansIn;
     uint8_t* ansOut;
     uint32_t extraBytes = 0;
-    StoredPlanes planes{nullptr, nullptr};
+    StoredPlanes planes{nullptr, nullptr, nullptr};
     ansIn = static_cast<const uint8_t*>(md.in);
     if (kind == kKindBytes) {
       ansOut = static_cast<uint8_t*>(md.out);
@@ -1053,7 +1126,13 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
       extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
       ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
       planes.non = static_cast<uint8_t*>(md.out) + kFloatHeaderBytes;
-      planes.non1 = planes.non + 2u * roundUp(size, 8u);
+      if (kind == kKindF64) {
+        planes.non1 = planes.non + floatU16PlaneOffset<uint32_t>(kind, size);
+        planes.non2 = planes.non + floatU8PlaneOffset<uint32_t>(kind, size);
+        __builtin_assume(__isGlobal(planes.non2));
+      } else {
+        planes.non1 = planes.non + 2u * roundUp(size, 8u);
+      }
       __builtin_assume(__isGlobal(planes.non));
       __builtin_assume(__isGlobal(planes.non1));
     }
@@ -1188,7 +1267,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
   const uint8_t* ansIn;
   uint8_t* ansOut;
   uint32_t extraBytes = 0;
-  StoredPlanes planes{nullptr, nullptr};
+  StoredPlanes planes{nullptr, nullptr, nullptr};
   ansIn = static_cast<const uint8_t*>(md.in);
   if (kind == kKindBytes) {
     ansOut = static_cast<uint8_t*>(md.out);
@@ -1196,7 +1275,13 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
     extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
     ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
     planes.non = static_cast<uint8_t*>(md.out) + kFloatHeaderBytes;
-    planes.non1 = planes.non + 2u * roundUp(size, 8u);
+    if (kind == kKindF64) {
+      planes.non1 = planes.non + floatU16PlaneOffset<uint32_t>(kind, size);
+      planes.non2 = planes.non + floatU8PlaneOffset<uint32_t>(kind, size);
+      __builtin_assume(__isGlobal(planes.non2));
+    } else {
+      planes.non1 = planes.non + 2u * roundUp(size, 8u);
+    }
     __builtin_assume(__isGlobal(planes.non));
     __builtin_assume(__isGlobal(planes.non1));
   }
@@ -1469,6 +1554,11 @@ ScratchPlan planScratch(int kind, uint32_t n, uint32_t maxSize, uint32_t totalTi
 
 uint32_t ticketsFor(uint32_t size) { return divUp(size, kBlockBytes); }
 
+// fp64 staging slot of the fast coder: the smallest the coder allows.  The fp64 ring is 12 KiB per warp, and a
+// smaller slot is what lets a second 8-warp CTA fit on an SM; fp64's coded byte (the high exponent byte)
+// compresses so well that a block rarely emits more than the slot holds (those that do spill, see Spill).
+constexpr uint32_t kEncSlotWordsF64 = kEncGroupRows * 32u + 264u;
+
 }  // namespace
 
 size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize) {
@@ -1491,7 +1581,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const bool fused = !canonical && opt.encode_fused != 0;
   // staging slot of the fast / fused encoder (spills to global scratch when a block needs more)
   uint32_t slotWords = opt.encode_slot_words > 0 ? (uint32_t)opt.encode_slot_words
-                                                 : (kind == kKindBytes ? 2304u : 1536u);
+                                                 : (kind == kKindBytes ? 2304u : (kind == kKindF64 ? kEncSlotWordsF64 : 1536u));
   slotWords = std::max<uint32_t>(roundUp(slotWords, 8u), kEncGroupRows * 32u + 264u);
   slotWords = std::min(slotWords, maxBlockWords(pb));
   // statistics slab: the two-kernel path streams it through registers; the fused launch lands it in
@@ -1573,7 +1663,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const int sms = smCount();
   // encoder table format (see EncSym in this file): wide entries for exponent-byte planes
   const bool wideTable = !canonical && opt.encode_wide_table != 0 &&
-                         (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32);
+                         (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32 || kind == DGB_FLOAT64);
   sc.wideTable = wideTable;
 
   if (fused) {

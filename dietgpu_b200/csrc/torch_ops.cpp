@@ -35,6 +35,7 @@ FloatType floatTypeOf(const Tensor& t) {
     case at::ScalarType::Half: return FloatType::kFloat16;
     case at::ScalarType::BFloat16: return FloatType::kBFloat16;
     case at::ScalarType::Float: return FloatType::kFloat32;
+    case at::ScalarType::Double: return FloatType::kFloat64;
     default: TORCH_CHECK(false, "dietgpu: unsupported float dtype ", t.scalar_type());
   }
   return FloatType::kUndefined;
@@ -44,6 +45,7 @@ at::ScalarType dtypeOf(FloatType ft) {
     case FloatType::kFloat16: return at::ScalarType::Half;
     case FloatType::kBFloat16: return at::ScalarType::BFloat16;
     case FloatType::kFloat32: return at::ScalarType::Float;
+    case FloatType::kFloat64: return at::ScalarType::Double;
     default: TORCH_CHECK(false, "dietgpu: invalid float type in archive");
   }
   return at::ScalarType::Half;

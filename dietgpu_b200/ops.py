@@ -29,7 +29,8 @@ from . import capi
 
 K_DEFAULT_PRECISION = 10  # DietGpu.cpp:114
 
-_FLOAT_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32}
+_FLOAT_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32,
+                torch.float64: capi.FLOAT64}
 _DTYPE_OF = {v: k for k, v in _FLOAT_TYPES.items()}
 
 

@@ -50,10 +50,13 @@ extern "C" {
 #define DGB_ERR_TOO_LARGE 5       /* a size exceeds the format's 32-bit limits */
 #define DGB_ERR_CAPTURING 6       /* decode with checksum verification on a stream that is being captured */
 
-/* float/GpuFloatCodec.h:18-23 FloatType */
+/* float/GpuFloatCodec.h:18-23 FloatType; DGB_FLOAT64 is this library's extension: its archives (float type 4)
+ * carry the high exponent byte of each double in the ANS part and the other 56 bits in a u32, a u16 and a
+ * u8 plane (DESIGN.md section 0).  The reference cannot read them. */
 #define DGB_FLOAT16 1
 #define DGB_BFLOAT16 2
 #define DGB_FLOAT32 3
+#define DGB_FLOAT64 4
 
 /* ans/GpuANSCodec.h:16,20 */
 #define DGB_ANS_REQUIRED_ALIGNMENT 4
@@ -68,7 +71,8 @@ int dgb_last_cuda_error(void);
 
 /* ans/GpuANSEncode.cu:13-25 getMaxCompressedSize (same value, same quirk). */
 uint32_t dgb_ans_max_compressed_size(uint32_t uncompressed_bytes);
-/* float/GpuFloatCompress.cu:23-45 getMaxFloatCompressedSize. */
+/* float/GpuFloatCompress.cu:23-45 getMaxFloatCompressedSize; for DGB_FLOAT64, 16 + the ANS bound + the three
+ * planes.  0 when the bound does not fit 32 bits (encode then returns DGB_ERR_TOO_LARGE). */
 uint32_t dgb_float_max_compressed_size(int float_type, uint32_t num_floats);
 
 /* ---- scratch sizing (new; the reference sizes scratch implicitly through
@@ -145,11 +149,12 @@ int dgb_ans_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* c
                                 int in_is_device_array, uint32_t num_in_batch,
                                 uint32_t* out_sizes_dev, uint32_t* out_checksum_dev, void* stream);
 
-/* ---- float codec (fp16 / bf16 / fp32) ------------------------------------ */
+/* ---- float codec (fp16 / bf16 / fp32 / fp64) ------------------------------ */
 
 /* float/GpuFloatCodec.h:103-139 / float/GpuFloatCompress.cu:47-101 floatCompress.
  * in_size counts float WORDS.  out[i] must hold
- * dgb_float_max_compressed_size(float_type, in_size[i]) bytes. */
+ * dgb_float_max_compressed_size(float_type, in_size[i]) bytes.  The checksum covers the first in_size[i]
+ * BYTES of the input, the reference's float rule (for DGB_FLOAT64, the first in_size[i] / 8 words). */
 int dgb_float_compress_pointer(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
                                int use_checksum, uint32_t num_in_batch, const void* const* in,
                                const uint32_t* in_size, void* const* out, uint32_t* out_size_dev,
@@ -197,7 +202,7 @@ int dgb_copy_rows_async(void* dst, size_t dst_pitch, const void* src, size_t src
 /* ---- archive mover (new; for the compressed collectives) -------------------- */
 /* Copies num_in_batch archives from src[i] to dst[i] (host arrays of device pointers, 16 B aligned), each
  * exactly as long as its own header says and at most dst_capacity[i] bytes: float_type 0 = ANS archives
- * (ans/GpuANSUtils.cuh:67-227 header), DGB_FLOAT16/BFLOAT16/FLOAT32 = float archives
+ * (ans/GpuANSUtils.cuh:67-227 header), DGB_FLOAT16/BFLOAT16/FLOAT32/FLOAT64 = float archives
  * (float/GpuFloatUtils.cuh:26-74).  src may be memory of a peer GPU mapped into this process (NVLink):
  * sizes are read on the device, nothing travels to the host; out_bytes_dev (optional, device, [n]) receives
  * the archive sizes.  An archive with a bad header is copied as its first 32 bytes so that the decoder

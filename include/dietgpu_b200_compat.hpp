@@ -274,7 +274,8 @@ struct ANSDecodeStatus {
 };
 
 // ---- float/GpuFloatCodec.h:18-97 ----
-enum class FloatType : uint32_t { kUndefined = 0, kFloat16 = 1, kBFloat16 = 2, kFloat32 = 3 };
+// kFloat64: this library's extension (archives of float type 4, which the reference cannot read)
+enum class FloatType : uint32_t { kUndefined = 0, kFloat16 = 1, kBFloat16 = 2, kFloat32 = 3, kFloat64 = 4 };
 
 inline uint32_t getMaxFloatCompressedSize(FloatType ft, uint32_t size) {
   return dgb_float_max_compressed_size((int)ft, size);
