@@ -293,7 +293,9 @@ void timerEnd(const Options& opt, int slot, cudaStream_t stream) {
 
 namespace {
 
-bool validFloatType(int ft) { return ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32 || ft == DGB_FLOAT64; }
+bool validFloatType(int ft) {
+  return ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32 || ft == DGB_FLOAT64 || isSparseKind(ft);
+}
 
 // the calling thread's member list, sized for n members
 HostMember* stageMembers(uint32_t n) {
@@ -348,7 +350,8 @@ uint32_t dgb_float_max_compressed_size(int ft, uint32_t n) {
   if (!validFloatType(ft)) return 0;
   const uint32_t ans = dgb_ans_max_compressed_size(n);
   if (ans == 0u) return 0u;  // too large (see above)
-  const uint64_t total = (uint64_t)kFloatHeaderBytes + ans + floatPlanesBytes<uint64_t>(ft, n);
+  const uint64_t total = isSparseKind(ft) ? sparseExtraBytes<uint64_t>(n, n) + ans
+                                          : (uint64_t)kFloatHeaderBytes + ans + floatPlanesBytes<uint64_t>(ft, n);
   return total <= 0xffffffffull ? (uint32_t)total : 0u;
 }
 

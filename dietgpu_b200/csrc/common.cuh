@@ -62,6 +62,27 @@ __host__ __device__ constexpr T floatPlanesBytes(int ft, T n) {
 }
 __host__ __device__ constexpr uint32_t floatNonCompBytes(int ft, uint32_t n) { return floatPlanesBytes<uint32_t>(ft, n); }
 
+// Sparse fp16 / bf16 archives (types 5 and 6, an extension the reference does not have): the dense type's coded
+// symbol and stored byte, but +0 and -0 words are coded as two symbols no other word uses (E+, E-) and store
+// nothing.  After the 32 B header (the dense 16 B, then S = words that store a byte, esc = E+ | E- << 8 | 1 << 16
+// or 0 when nothing is elided, 0, 0) come a u32 per 4 KiB block (stored bytes of all earlier blocks), the S
+// stored bytes in element order, and the ANS archive; every section starts 16 B aligned and is zero padded.
+constexpr uint32_t kSparseHeaderBytes = 32;
+__host__ __device__ constexpr bool isSparseKind(int ft) { return ft == DGB_FLOAT16_SPARSE || ft == DGB_BFLOAT16_SPARSE; }
+__host__ __device__ constexpr int denseKind(int ft) {  // the dense type whose symbol and stored byte a kind uses
+  return ft == DGB_FLOAT16_SPARSE ? DGB_FLOAT16 : ft == DGB_BFLOAT16_SPARSE ? DGB_BFLOAT16 : ft;
+}
+template <class T>
+__host__ __device__ constexpr T sparseTableBytes(T n) { return T(4) * roundUpT<T>((n + 4095) / 4096, 4); }
+// header + block table + stored bytes in front of the ANS archive (S = stored bytes)
+template <class T>
+__host__ __device__ constexpr T sparseExtraBytes(T n, T S) {
+  return T(kSparseHeaderBytes) + sparseTableBytes<T>(n) + roundUpT<T>(S, 16);
+}
+__host__ __device__ constexpr bool sparseEscValid(uint32_t esc) {
+  return esc == 0u || ((esc >> 16) == 1u && (esc & 0xffu) < ((esc >> 8) & 0xffu));
+}
+
 // Worst-case u16 words one 4 KiB block can emit: every symbol costs at most
 // probBits bits (a symbol of pdf 1), so 4096*pb/16 words; +8 for 16 B padding.
 __host__ __device__ constexpr uint32_t maxBlockWords(int pb) { return 256u * (uint32_t)pb + 8u; }
@@ -72,7 +93,9 @@ enum CodecKind : int {
   kKindF16 = DGB_FLOAT16,
   kKindBF16 = DGB_BFLOAT16,
   kKindF32 = DGB_FLOAT32,
-  kKindF64 = DGB_FLOAT64
+  kKindF64 = DGB_FLOAT64,
+  kKindF16S = DGB_FLOAT16_SPARSE,
+  kKindBF16S = DGB_BFLOAT16_SPARSE
 };
 
 struct MemberDesc {
@@ -246,6 +269,8 @@ int withKind(int kind, F&& f) {
     case kKindBF16: return f(IntC<kKindBF16>{});
     case kKindF32: return f(IntC<kKindF32>{});
     case kKindF64: return f(IntC<kKindF64>{});
+    case kKindF16S: return f(IntC<kKindF16S>{});
+    case kKindBF16S: return f(IntC<kKindBF16S>{});
     default: return DGB_ERR_INVALID_ARG;
   }
 }

@@ -1,5 +1,5 @@
 // decode.cu -- batched rANS decode (bytes) and fused float decompress
-// (fp16/bf16/fp32/fp64) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
+// (fp16/bf16/fp32/fp64, sparse fp16/bf16) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
 // whose CTAs lease members (header checks and the 2^pb LUT from the archive's own pdf happen inside the
 // CTA) and whose warps claim 4 KiB blocks; lane states + compressed words of a block arrive by one TMA
 // bulk copy (cp.async.bulk + mbarrier), the 32-lane interleaved rANS decode of ans/GpuANSDecode.cuh:55-217
@@ -44,6 +44,10 @@ struct ArchiveView {
   const uint8_t* non;      // float kinds: stored (non-compressed) plane(s)
   uint32_t floatWords;     // float kinds: size field of the float header
   bool ok;
+  // sparse kinds: block table, stored bytes (`non`), escape word
+  const uint32_t* table;
+  uint32_t storedBytes;
+  uint32_t esc;
 };
 
 template <int KIND>
@@ -54,6 +58,17 @@ __device__ __forceinline__ ArchiveView openArchive(const uint8_t* in) {
     v.non = nullptr;
     v.floatWords = 0;
     v.ok = true;
+  } else if constexpr (isSparseKind(KIND)) {
+    // the 32 B header: the dense 16 B, then S and esc (DESIGN.md section 0)
+    const uint4 fh = __ldg(reinterpret_cast<const uint4*>(in));
+    const uint4 sh = __ldg(reinterpret_cast<const uint4*>(in) + 1);
+    v.ok = fh.x == kFloatMagicVersion && (int)(fh.z & 0xfu) == KIND && sh.x <= fh.y && sparseEscValid(sh.y);
+    v.floatWords = fh.y;
+    v.storedBytes = sh.x;
+    v.esc = sh.y;
+    v.table = reinterpret_cast<const uint32_t*>(in + kSparseHeaderBytes);
+    v.non = in + kSparseHeaderBytes + sparseTableBytes<uint32_t>(fh.y);
+    v.ans = in + sparseExtraBytes<uint32_t>(fh.y, sh.x);
   } else {
     // float/GpuFloatUtils.cuh:26-74 GpuFloatHeader
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(in));
@@ -199,6 +214,84 @@ struct RowWriter16 {
 };
 template <> struct RowWriter<kKindF16> : RowWriter16<kKindF16> {};
 template <> struct RowWriter<kKindBF16> : RowWriter16<kKindBF16> {};
+
+// Sparse fp16 / bf16: the block's segment of stored bytes, [table[k], table[k + 1] or S), sits in the warp's ring
+// (one copy per block, widened to 16 B bounds: at most 4112 bytes).  Rows are walked backwards, so the cursor
+// starts one past the segment's last byte; per row it moves back by the number of kept lanes (symbol neither E+ nor
+// E-), and a kept lane reads its byte at the cursor plus its rank among the kept lanes.  E+ / E- lanes write +0 / -0.
+template <int KIND>
+struct RowWriterSparse {
+  static constexpr int BT = denseKind(KIND);
+  static constexpr uint32_t kRingSlotBytes = 1376;  // 3 slots = 4128 bytes >= the widest segment
+  uint16_t* out;
+  const uint8_t* src;    // 16 B aligned start of the segment's copy
+  uint32_t copyBytes;    // bytes to copy (multiple of 16)
+  uint32_t ring, lane, ltMask;
+  uint32_t ep, em;       // escape symbols; 0x100 / 0x101 (no symbol) when nothing is elided
+  mutable uint32_t cur;  // shared address one past the next row's kept bytes
+  struct Cursor { uint16_t* o; };
+  __device__ __forceinline__ void setRing(uint32_t ringAddr, uint32_t l) {
+    ring = ringAddr;
+    lane = l;
+    ltMask = laneMaskLt();
+  }
+  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
+    out = static_cast<uint16_t*>(outBase) + (size_t)block * kBlockBytes + l;
+    const uint32_t nb = divUp(av.floatWords, kBlockBytes);
+    const uint32_t begin = __ldg(av.table + block);
+    const uint32_t end = block + 1 < nb ? __ldg(av.table + block + 1) : av.storedBytes;
+    const uint32_t a0 = begin & ~15u;
+    src = av.non + a0;
+    copyBytes = roundUp(end, 16u) - a0;
+    cur = ring + (end - a0);
+    const bool elide = av.esc != 0u;
+    ep = elide ? (av.esc & 0xffu) : 0x100u;
+    em = elide ? ((av.esc >> 8) & 0xffu) : 0x101u;
+    __builtin_assume(__isGlobal(out));
+    __builtin_assume(__isGlobal(src));
+  }
+  // the segment arrives by a bulk copy on the block's mbarrier (lane 0; bytes counted by the caller's expect_tx)
+  __device__ __forceinline__ uint32_t bulkBytes() const { return copyBytes; }
+  __device__ __forceinline__ void bulkIssue(uint32_t bar) const {
+    if (copyBytes) {
+      fenceProxyAsync();  // the ring may have been written through the generic proxy (copySync)
+      bulkLoad(ring, src, copyBytes, bar);
+    }
+  }
+  // ... or, when the block's stream is read from global memory, by the warp itself
+  __device__ __forceinline__ void copySync() const {
+    __syncwarp();
+    for (uint32_t i = lane * 16u; i < copyBytes; i += 512u) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(src + i));
+      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(ring + i), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+                   : "memory");
+    }
+    __syncwarp();
+  }
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t) const { return Cursor{out + row * 32u}; }
+  __device__ __forceinline__ void issue(uint32_t, uint32_t) const {}
+  // the word of this lane's element in the current row (whole warp; lanes with valid = false hold none)
+  __device__ __forceinline__ uint32_t word(uint32_t entry, bool valid) const {
+    const uint32_t s = entry & 0xffu;
+    const bool keep = valid && s != ep && s != em;
+    const uint32_t b = __ballot_sync(0xffffffffu, keep);
+    cur -= __popc(b);
+    uint32_t nc = 0;
+    if (keep) asm volatile("ld.shared.u8 %0, [%1];" : "=r"(nc) : "r"(cur + __popc(b & ltMask)));
+    return keep ? RowWriter16<BT>::join(entry, nc) : (s == ep ? 0u : 0x8000u);
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)word(entry, true);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { out[row * 32u] = (uint16_t)word(entry, true); }
+  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
+    const uint32_t w = word(entry, valid);
+    if (valid) out[row * 32u] = (uint16_t)w;
+  }
+};
+template <> struct RowWriter<kKindF16S> : RowWriterSparse<kKindF16S> {};
+template <> struct RowWriter<kKindBF16S> : RowWriterSparse<kKindBF16S> {};
 
 template <>
 struct RowWriter<kKindF64> {
@@ -471,7 +564,10 @@ __device__ __forceinline__ void decodeBlockWarp(uint32_t state, Stream st, uint3
   if (rem) {
     const bool valid = lane < rem;
     const uint32_t e = decodeStepPartial<PB, LUT64>(valid, state, lut, st, geMask);
-    if (valid) wr.writeSlow(row, e);
+    if constexpr (isSparseKind(KIND))
+      wr.writePartial(row, e, valid);  // its ballot needs every lane
+    else if (valid)
+      wr.writeSlow(row, e);
   }
   uint32_t slot = 0, slotNext = 2;  // ring slots of group k and of group k + 2
   for (uint32_t k = 0; k < groups; ++k) {
@@ -769,7 +865,13 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
           const uint32_t streamBytes = roundUp(words, 8u) * 2u;
           __syncwarp();
           if (lane == 0) {
-            mbarExpectTx(myBar, 128u + streamBytes);
+            if constexpr (isSparseKind(KIND)) {
+              // the block's stored bytes ride on the same mbarrier
+              mbarExpectTx(myBar, 128u + streamBytes + wr.bulkBytes());
+              wr.bulkIssue(myBar);
+            } else {
+              mbarExpectTx(myBar, 128u + streamBytes);
+            }
             bulkLoad(smemAddr(mySlot), pStates + 128u * (size_t)block, 128u, myBar);
             if (streamBytes) bulkLoad(smemAddr(mySlot + 128), stream, streamBytes, myBar);
           }
@@ -779,6 +881,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
           SmemStream st{smemAddr(mySlot + 128) + 2u * words};
           decodeBlockWarp<KIND, PB, false>(state, st, blockLen, lut, wr, lane);
         } else {
+          if constexpr (isSparseKind(KIND)) wr.copySync();
           const uint32_t state = __ldg(reinterpret_cast<const uint32_t*>(pStates) + block * 32u + lane);
           GmemStream st{stream + words};
           decodeBlockWarp<KIND, PB, false>(state, st, blockLen, lut, wr, lane);
@@ -905,7 +1008,8 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   }
 
   const Options opt = options();  // one snapshot per call
-  const bool fused = opt.decode_fused != 0;
+  // the sparse kinds have only the single-launch decoder: decode_fused=0 runs it for them (INTEGRATION.md section 4)
+  const bool fused = opt.decode_fused != 0 || isSparseKind(kind);
   HostStage& hs = hostStage();
   hs.decodeTable.resize(n);
   MemberDesc* desc = hs.decodeTable.data();
@@ -973,19 +1077,23 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     SubBatches parts(kind, desc, n, opt, true, stream);
     if (const int rc = parts.fork(); rc != DGB_OK) return rc;
     const int rc = withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
-      for (int part = 0; part < parts.count(); ++part) {
-        const uint32_t m0 = parts.begin(part), m1 = parts.end(part);
-        if (m1 == m0) continue;
-        cudaStream_t ps;
-        int prc = parts.stream(part, &ps);
-        if (prc != DGB_OK) return prc;
-        uint64_t partBound = 0;
-        for (uint32_t i = m0; i < m1; ++i) partBound += divUp(desc[i].size, kBlockBytes);
-        prc = launchPlanDecode<decltype(K)::value, decltype(P)::value>(opt, sc, checksum, m0, m1, part, partBound,
-                                                                      outSuccess_dev, outSize_dev, ps);
-        if (prc != DGB_OK) return prc;
+      if constexpr (isSparseKind(decltype(K)::value)) {
+        return (int)DGB_ERR_INVALID_ARG;  // not reached (`fused` above)
+      } else {
+        for (int part = 0; part < parts.count(); ++part) {
+          const uint32_t m0 = parts.begin(part), m1 = parts.end(part);
+          if (m1 == m0) continue;
+          cudaStream_t ps;
+          int prc = parts.stream(part, &ps);
+          if (prc != DGB_OK) return prc;
+          uint64_t partBound = 0;
+          for (uint32_t i = m0; i < m1; ++i) partBound += divUp(desc[i].size, kBlockBytes);
+          prc = launchPlanDecode<decltype(K)::value, decltype(P)::value>(opt, sc, checksum, m0, m1, part, partBound,
+                                                                        outSuccess_dev, outSize_dev, ps);
+          if (prc != DGB_OK) return prc;
+        }
+        return (int)DGB_OK;
       }
-      return DGB_OK;
     }); });
     if (rc != DGB_OK) return rc;
   }  // ~SubBatches orders the helper streams before the caller's stream
@@ -1059,9 +1167,15 @@ __device__ __forceinline__ uint4 ldgNc(const uint4* p) {
 constexpr uint32_t kPullThreads = 512;
 constexpr uint32_t kPullChunkVecs = 4096;  // 64 KiB work units
 
+template <bool SPARSE>
 __device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {  // inlined: kind folds where it is constant
   uint32_t extra = 0;
-  if (kind != kKindBytes) {
+  if constexpr (SPARSE) {  // fp16 and bf16 lay out their sections alike
+    const uint4 fh = __ldg(reinterpret_cast<const uint4*>(a));
+    const uint4 sh = __ldg(reinterpret_cast<const uint4*>(a) + 1);
+    if (fh.x != kFloatMagicVersion || sh.x > fh.y) return 32u;
+    extra = sparseExtraBytes<uint32_t>(fh.y, sh.x);
+  } else if (kind != kKindBytes) {
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(a));
     if (fh.x != kFloatMagicVersion) return 32u;
     extra = kFloatHeaderBytes + floatNonCompBytes(kind, fh.y);
@@ -1072,12 +1186,13 @@ __device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {  
   return total > 0xfffffff0ull ? 32u : (uint32_t)total;
 }
 
+template <bool SPARSE>
 __device__ __forceinline__ void pullArchivesBody(const InlineMembers& im, int kind, uint32_t* __restrict__ outBytes) {
   __shared__ uint32_t sFirst[kInlineMembers + 1];  // first chunk of member i
   __shared__ uint32_t sBytes[kInlineMembers];
   const uint32_t t = threadIdx.x, n = im.count;
   if (t < n) {
-    const uint32_t want = archiveBytes(kind, static_cast<const uint8_t*>(im.m[t].in));
+    const uint32_t want = archiveBytes<SPARSE>(kind, static_cast<const uint8_t*>(im.m[t].in));
     const uint32_t b = min(want, im.m[t].size & ~15u);
     sBytes[t] = b;
     if (outBytes && blockIdx.x == 0) outBytes[t] = want;
@@ -1111,12 +1226,17 @@ __device__ __forceinline__ void pullArchivesBody(const InlineMembers& im, int ki
 __global__ void __launch_bounds__(kPullThreads)
 pullArchivesKernel(const __grid_constant__ InlineMembers im, int kind, uint32_t* __restrict__ outBytes) {
   __builtin_assume(kind != kKindF64);
-  pullArchivesBody(im, kind, outBytes);
+  pullArchivesBody<false>(im, kind, outBytes);
 }
 // fp64 archives: their own instantiation, so the kernel above keeps its plane-size arithmetic
 __global__ void __launch_bounds__(kPullThreads)
 pullArchivesF64Kernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
-  pullArchivesBody(im, kKindF64, outBytes);
+  pullArchivesBody<false>(im, kKindF64, outBytes);
+}
+// sparse fp16 / bf16 archives: sizes from the 32 B header
+__global__ void __launch_bounds__(kPullThreads)
+pullArchivesSparseKernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
+  pullArchivesBody<true>(im, kKindF16S, outBytes);
 }
 }  // namespace
 
@@ -1142,6 +1262,8 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
     uint32_t* ob = outBytes_dev ? outBytes_dev + i0 : nullptr;
     if (kind == kKindF64)
       pullArchivesF64Kernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
+    else if (isSparseKind(kind))
+      pullArchivesSparseKernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
     else
       pullArchivesKernel<<<ctas, kPullThreads, 0, stream>>>(im, kind, ob);
     DGB_CUDA_TRY(cudaGetLastError());

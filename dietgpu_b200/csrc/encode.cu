@@ -1,4 +1,4 @@
-// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64)
+// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16)
 // for sm_90a (H100).  Two launches per call, whatever the batch size:
 //
 //   K1  stats*Kernel     a pure read of the raw input: 256-bin histogram of the coded byte, taken out of
@@ -72,12 +72,22 @@ struct EncodeScratch {
   unsigned long long* lookback;   // [totalTickets](zeroed)   canonical (ordered) layout only
   unsigned long long* allocDone;  // [n]           (zeroed)   low: words handed out, high: blocks placed
   uint8_t* spill;                 // [resident warps][maxBlockWords] u16: overflow of small staging slots
-  uint4* table;                   // [n][256] slots of 16 B (packed entries use the first half)
+  uint4* table;                   // [n][tableSlots(kind)] slots of 16 B (packed entries use the first half)
   bool wideTable;                 // entry format: EncEntryWide (16 B) or EncEntry (8 B)
+  uint32_t blockZerosOff;         // sparse kinds: see blockZeros() (in the padding after wideTable: the kernel
+                                  // parameters of the other kinds keep their layout)
   // fused single-launch encoder only
   const uint2* workIdx;           // [n + 1] {first stats item, first encode chunk} of member i
   uint32_t* ready;                // [n]  (zeroed) 1 once the member's table is published
 };
+static_assert(sizeof(EncodeScratch) == 96, "");
+
+// The sparse kinds never run the fused launch, so they keep their counters in its (zeroed) `ready` array:
+// +0 and -0 words of member m, and the +-0 words of the 4 KiB block with ticket work0 + k.
+__device__ __forceinline__ uint32_t* zeroCounts(const EncodeScratch& sc, uint32_t m) { return sc.ready + 2u * m; }
+__device__ __forceinline__ uint32_t* blockZeros(const EncodeScratch& sc, uint32_t work0) {
+  return sc.ready + sc.blockZerosOff + work0;
+}
 
 // ---------------------------------------------------------------------------
 // Normalisation epilogue: 256 threads, thread t owns symbol t.
@@ -137,6 +147,15 @@ __device__ void publishEmptyMember(uint8_t* ansArchive, int pb, bool useChecksum
     if (outSize) outSize[m] = ansOverhead(0) + extraBytes;
   }
 }
+
+// Encoder table of a member: 16 B slots in scratch, entries in shared memory.  The sparse kinds have two more
+// entries: 256 for +0 and 257 for -0 words (copies of the entries of E+ and E-, or of the natural symbols when
+// nothing is elided), so the coder turns a word into its table entry without any per-member escape state.
+__host__ __device__ constexpr uint32_t tableSlots(int kind) { return isSparseKind(kind) ? 260u : kNumSymbols; }
+__host__ __device__ constexpr uint32_t encTabVecs(bool wide, int kind) {
+  return isSparseKind(kind) ? (wide ? 258u : 130u) : (wide ? kNumSymbols : kNumSymbols / 2);
+}
+__host__ __device__ constexpr uint32_t encTabBytes(int kind) { return isSparseKind(kind) ? 2080u : kNumSymbols * 8u; }
 
 __device__ __forceinline__ uint32_t foldXor(uint32_t v) {
   return (v ^ (v >> 8) ^ (v >> 16) ^ (v >> 24)) & 0xffu;
@@ -378,6 +397,149 @@ __device__ __forceinline__ void histVectors(const uint4* __restrict__ vec, const
   }
 }
 
+// ---- sparse kinds: the +0 / -0 counts of the statistics pass ----------------------------------------------
+// Bit j = element j of a 16 B vector of 16-bit words is +0 or -0; pz / nz count the +0 / -0 words.
+__device__ __forceinline__ uint32_t zeroMask8(const uint4& v, uint32_t& pz, uint32_t& nz) {
+  const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+  uint32_t m = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const uint32_t lo = w4[q] & 0xffffu, hi = w4[q] >> 16;
+    m |= (uint32_t)((lo & 0x7fffu) == 0u) << (2 * q);
+    m |= (uint32_t)((hi & 0x7fffu) == 0u) << (2 * q + 1);
+    pz += (uint32_t)(lo == 0u) + (uint32_t)(hi == 0u);
+    nz += (uint32_t)(lo == 0x8000u) + (uint32_t)(hi == 0x8000u);
+  }
+  return m;
+}
+
+// The vector body for the sparse kinds: the natural symbols' histogram as for the dense type BT, plus the +-0
+// words per member (registers) and per 4 KiB block (`bz`, global).  The 32 vectors a warp reads at once
+// are 256 consecutive elements, so they touch at most two blocks: one warp reduction per block, one atomic each.
+// `head` = elements before the first vector; when it is not 0 every block boundary falls inside a vector.
+template <int BT>
+__device__ __forceinline__ void histZeroVectors(const uint4* __restrict__ vec, uint32_t v0, uint32_t v1, uint32_t t,
+                                                uint32_t* wh, uint32_t head, uint32_t* __restrict__ bz,
+                                                uint32_t& pz, uint32_t& nz) {
+  const uint32_t lane = t & 31u;
+  for (uint32_t w0 = v0 + (t & ~31u); w0 < v1; w0 += kStatsUnroll * kStatsThreads) {  // warp-uniform
+    uint4 vv[kStatsUnroll];
+#pragma unroll
+    for (int k = 0; k < kStatsUnroll; ++k) {
+      const uint32_t i = w0 + lane + k * kStatsThreads;
+      vv[k] = i < v1 ? ldStream16(vec + i) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int k = 0; k < kStatsUnroll; ++k) {
+      const uint32_t wi = w0 + k * kStatsThreads;  // the warp's first vector
+      if (wi >= v1) break;
+      const uint32_t i = wi + lane;
+      const uint32_t wb = (head + 8u * wi) >> 12;  // block of the warp's first element
+      uint32_t c0 = 0, c1 = 0;                     // +-0 words in blocks wb and wb + 1
+      if (i < v1) {
+        const uint32_t w4[4] = {vv[k].x, vv[k].y, vv[k].z, vv[k].w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          histAdd(wh, histOffLo<BT>(w4[q]));
+          histAdd(wh, histOffHi<BT>(w4[q]));
+        }
+        const uint32_t zm = zeroMask8(vv[k], pz, nz);
+        const uint32_t e0 = head + 8u * i, bA = e0 >> 12;
+        uint32_t cA = __popc(zm), cB = 0;
+        if (((e0 + 7u) >> 12) != bA) {  // straddles a boundary: elements j < 8 - head are in block bA
+          const uint32_t j = 8u - head;
+          cA = __popc(zm & ((1u << j) - 1u));
+          cB = __popc(zm >> j);
+        }
+        c0 = bA == wb ? cA : 0u;
+        c1 = bA == wb ? cB : cA;
+      }
+      const uint32_t s0 = __reduce_add_sync(0xffffffffu, c0), s1 = __reduce_add_sync(0xffffffffu, c1);
+      if (lane == 0) {
+        if (s0) atomicAdd(bz + wb, s0);
+        if (s1) atomicAdd(bz + wb + 1, s1);
+      }
+    }
+  }
+}
+
+// Last CTA of a sparse member (256 threads, thread t = symbol t): picks E+ and E-, moves the +0 / -0 counts from
+// their natural symbols (+0: 0; -0: 0x80 for fp16, 0 for bf16) to them, normalises, and writes the block table,
+// the 32 B header, the zero padding of the table and the stored bytes, the pdf and the encoder table.
+template <int FT>
+__device__ void finishSparseMember(const EncodeScratch& sc, int pb, bool useChecksum, const MemberDesc& md, uint32_t m,
+                                   uint32_t* __restrict__ outSize) {
+  constexpr uint32_t kNegSym = FT == kKindF16S ? 0x80u : 0u;
+  __shared__ uint32_t sFree[kStatsWarps];
+  __shared__ uint32_t sScan[kStatsWarps];
+  const uint32_t t = threadIdx.x;
+  const uint32_t size = md.size;
+  uint8_t* archive = static_cast<uint8_t*>(md.out);
+  const uint32_t pz = __ldcg(zeroCounts(sc, m)), nz = __ldcg(zeroCounts(sc, m) + 1);
+  uint32_t* hist = sc.hist + m * kNumSymbols;
+  const uint32_t other = __ldcg(hist + t) - (t == 0u ? pz : 0u) - (t == kNegSym ? nz : 0u);  // words neither +0 nor -0
+  const uint32_t freeMask = __ballot_sync(0xffffffffu, other == 0u);
+  if ((t & 31u) == 0u) sFree[t >> 5] = freeMask;
+  __syncthreads();
+  // E+ / E-: the two smallest symbols no other word uses (both or neither, see DESIGN.md section 0)
+  uint32_t ep = 0, em = 0, found = 0;
+  for (uint32_t w = 0; w < (uint32_t)kStatsWarps && found < 2u; ++w) {
+    for (uint32_t f = sFree[w]; f != 0u && found < 2u; f &= f - 1u, ++found) {
+      const uint32_t s = 32u * w + (uint32_t)__ffs((int)f) - 1u;
+      if (found == 0u) ep = s; else em = s;
+    }
+  }
+  const bool elide = found == 2u;
+  const uint32_t esc = elide ? (ep | (em << 8) | (1u << 16)) : 0u;
+  if (elide) hist[t] = other + (t == ep ? pz : 0u) + (t == em ? nz : 0u);  // read back by this thread below
+
+  // block table: exclusive prefix of the stored bytes per block; each thread takes a contiguous run of blocks
+  const uint32_t nb = divUp(size, kBlockBytes);
+  uint32_t* table = reinterpret_cast<uint32_t*>(archive + kSparseHeaderBytes);
+  const uint32_t* bz = blockZeros(sc, md.work0);
+  const uint32_t per = divUp(nb, (uint32_t)kStatsThreads);
+  const uint32_t b0 = min(nb, t * per), b1 = min(nb, b0 + per);
+  auto kept = [&](uint32_t b) { return min(kBlockBytes, size - b * kBlockBytes) - (elide ? __ldcg(bz + b) : 0u); };
+  uint32_t sum = 0;
+  for (uint32_t b = b0; b < b1; ++b) sum += kept(b);
+  uint32_t S;
+  uint32_t run = blockExclusiveScan<kStatsThreads>(sum, sScan, &S);
+  for (uint32_t b = b0; b < b1; ++b) {
+    table[b] = run;
+    run += kept(b);
+  }
+  for (uint32_t b = nb + t; b < roundUp(nb, 4u); b += kStatsThreads) table[b] = 0;
+  uint8_t* plane = archive + kSparseHeaderBytes + sparseTableBytes<uint32_t>(size);
+  for (uint32_t i = S + t; i < roundUp(S, 16u); i += kStatsThreads) plane[i] = 0;
+  if (t == 0) {
+    uint4* h = reinterpret_cast<uint4*>(archive);
+    h[0] = make_uint4(kFloatMagicVersion, size, (uint32_t)FT | ((useChecksum ? 1u : 0u) << 4),
+                      useChecksum ? __ldcg(sc.checksum + m) : 0u);
+    h[1] = make_uint4(S, esc, 0u, 0u);
+  }
+  uint8_t* ansArchive = archive + sparseExtraBytes<uint32_t>(size, S);
+  if (size == 0) {
+    publishEmptyMember(ansArchive, pb, false, outSize, m, kSparseHeaderBytes);
+    return;
+  }
+  uint4* tab = sc.table + (size_t)m * tableSlots(FT);
+  normalizeAndPublish(hist, size, pb, sc.wideTable, tab, ansArchive);
+  // entries 256 (+0) and 257 (-0); thread t reads back the entry it has just written
+  const uint32_t srcP = elide ? ep : 0u, srcN = elide ? em : kNegSym;
+  if (t == srcP || t == srcN) {
+    if (sc.wideTable) {
+      const uint4 e = tab[t];
+      if (t == srcP) tab[256] = e;
+      if (t == srcN) tab[257] = e;
+    } else {
+      uint2* p = reinterpret_cast<uint2*>(tab);
+      const uint2 e = p[t];
+      if (t == srcP) p[256] = e;
+      if (t == srcN) p[257] = e;
+    }
+  }
+}
+
 // Work of CTA y of Y on member m; returns true in the CTA that finished the member.
 template <int FT, bool STAGED>
 __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t (*sHist)[kNumSymbols], int pb,
@@ -385,7 +547,9 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
                                                uint32_t m, uint32_t y,
                                                uint32_t Y, uint32_t* __restrict__ outSize,
                                                const StatsStage& stage = StatsStage()) {
-  constexpr uint32_t EPV = (FT == DGB_FLOAT64) ? 2u : (FT == DGB_FLOAT32) ? 4u : 8u;  // elements per 16 B vector
+  constexpr bool SPARSE = isSparseKind(FT);
+  constexpr int BT = denseKind(FT);  // the dense type whose natural symbols the histogram counts
+  constexpr uint32_t EPV = (BT == DGB_FLOAT64) ? 2u : (BT == DGB_FLOAT32) ? 4u : 8u;  // elements per 16 B vector
   constexpr uint32_t WB = 16u / EPV;                                                 // word bytes
   // shuffle => the histogram base is provably warp-uniform (ATOMS [R + UR], no per-symbol add)
   const uint32_t t = threadIdx.x, warp = __shfl_sync(0xffffffffu, t >> 5, 0);
@@ -419,6 +583,7 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
     __syncthreads();
     uint32_t* wh = sHist[warp];
     uint32_t xorAcc = 0;
+    uint32_t pz = 0, nz = 0;  // sparse kinds: +0 / -0 words seen by this thread
 
     // ---- vector body ----
     for (uint32_t slab = y; slab < nSlabs; slab += Y) {
@@ -429,9 +594,35 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
       }
       // four independent 16 B loads per thread are issued before any of them is consumed: the
       // kernel is a pure stream and was latency-bound with one load in flight
-      histVectors<FT, STAGED>(vec, stage, v0, v1, t, wh);
+      if constexpr (SPARSE)
+        histZeroVectors<BT>(vec, v0, v1, t, wh, head, blockZeros(sc, md.work0), pz, nz);
+      else
+        histVectors<FT, STAGED>(vec, stage, v0, v1, t, wh);
     }
-    if (y == 0) {
+    if constexpr (SPARSE) {
+      if (y == 0) {
+        // scalar head and tail; the 32 B header, the table and the padding are written by the last CTA
+        const uint32_t tailStart = head + nVec * EPV;
+        uint32_t* bz = blockZeros(sc, md.work0);
+        const uint16_t* in16 = reinterpret_cast<const uint16_t*>(in);
+        auto scalar = [&](uint32_t e) {
+          const uint32_t w = in16[e];
+          atomicAdd(&wh[BT == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8], 1u);
+          if ((w & 0x7fffu) == 0u) {
+            pz += w == 0u;
+            nz += w != 0u;
+            atomicAdd(bz + (e >> 12), 1u);
+          }
+        };
+        if (t < head) scalar(t);
+        if (t < size - tailStart) scalar(tailStart + t);
+      }
+      const uint32_t p = __reduce_add_sync(0xffffffffu, pz), q = __reduce_add_sync(0xffffffffu, nz);
+      if ((t & 31u) == 0u) {
+        if (p) atomicAdd(zeroCounts(sc, m), p);
+        if (q) atomicAdd(zeroCounts(sc, m) + 1, q);
+      }
+    } else if (y == 0) {
       // ---- scalar head and tail (fewer than one vector each) ----
       const uint32_t tailStart = head + nVec * EPV;
       if (t < head) atomicAdd(&wh[codedScalar<FT>(in, t)], 1u);
@@ -467,6 +658,10 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
   }
 
   // ---- last CTA of the member ----
+  if constexpr (SPARSE) {
+    finishSparseMember<FT>(sc, pb, useChecksum, md, m, outSize);
+    return true;
+  }
   if (size == 0) {
     if (t == 0) {
       *reinterpret_cast<uint4*>(archive) =
@@ -548,6 +743,9 @@ struct StoredPlanes {
   uint8_t* non;   // fp16 / bf16: the stored byte plane; fp32: the u16 plane; fp64: the u32 plane
   uint8_t* non1;  // fp32: the u8 plane; fp64: the u16 plane
   uint8_t* non2;  // fp64: the u8 plane
+  // sparse kinds: `non` holds the kept words' bytes, block k's from table[k] on
+  const uint32_t* table;
+  uint32_t keepAll;  // 1: nothing is elided (esc == 0), every word stores its byte
 };
 
 template <int KIND>
@@ -619,6 +817,74 @@ struct EncIn16 {
 };
 template <> struct EncIn<kKindF16> : EncIn16<kKindF16> {};
 template <> struct EncIn<kKindBF16> : EncIn16<kKindBF16> {};
+
+// Sparse fp16 / bf16: a +0 / -0 word looks up table entry 256 / 257 (see tableSlots), every other word its
+// natural symbol's.  The stored bytes of the kept words are compacted in element order: per group by a warp scan
+// of the lanes' kept counts, per scalar row by a ballot; `cur` is the plane offset of the next kept byte.
+template <int KIND>
+struct EncInSparse {
+  static constexpr int BT = denseKind(KIND);
+  static constexpr uint32_t kWordBytes = 2, kRingSlots = DGB_ENC_RING16;
+  template <uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffsetOf(uint32_t w) {
+    const uint32_t nat = BT == kKindBF16 ? (w >> 7) & 0xffu : w >> 8;
+    return STRIDE * ((w & 0x7fffu) == 0u ? 256u + (w >> 15) : nat);
+  }
+  template <int J, uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffset(uint32_t ringLane) {
+    uint32_t w;
+    asm volatile("ld.shared.u16 %0, [%1+%2];" : "=r"(w) : "r"(ringLane), "n"(J * 64));
+    return tabOffsetOf<STRIDE>(w);
+  }
+  static __device__ __forceinline__ uint32_t loadWord(const uint8_t* in, uint32_t e) {
+    return __ldg(reinterpret_cast<const uint16_t*>(in) + e);
+  }
+  // one row of words, whole warp (lanes without a word pass valid = false)
+  static __device__ __forceinline__ void storeRow(const StoredPlanes& pl, uint32_t& cur, uint32_t w, bool valid,
+                                                  uint32_t ltMask) {
+    const bool keep = valid && (pl.keepAll != 0u || (w & 0x7fffu) != 0u);
+    const uint32_t b = __ballot_sync(0xffffffffu, keep);
+    if (keep) pl.non[cur + __popc(b & ltMask)] = (uint8_t)EncIn16<BT>::storedOf(w);
+    cur += __popc(b);
+  }
+  // one group of 16 rows (512 elements in the ring slot): lane l takes vectors l and l + 32, 8 elements each
+  static __device__ __forceinline__ void storeGroup(uint32_t slot, const StoredPlanes& pl, uint32_t& cur,
+                                                    uint32_t lane) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t v = lane + 32u * h;
+      uint4 x;
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w) : "r"(slot + v * 16u));
+      const uint32_t w4[4] = {x.x, x.y, x.z, x.w};
+      uint32_t keep = 0xffu;
+      if (!pl.keepAll) {
+        keep = 0;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          keep |= (uint32_t)((w4[q] & 0x7fffu) != 0u) << (2 * q);
+          keep |= (uint32_t)((w4[q] & 0x7fff0000u) != 0u) << (2 * q + 1);
+        }
+      }
+      const uint32_t lo = __byte_perm(rot16x2<BT>(x.x), rot16x2<BT>(x.y), 0x6420);
+      const uint32_t hi = __byte_perm(rot16x2<BT>(x.z), rot16x2<BT>(x.w), 0x6420);
+      const uint32_t c = __popc(keep);
+      uint32_t incl = c;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t s = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= (uint32_t)d) incl += s;
+      }
+      uint8_t* p = pl.non + cur + (incl - c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        if ((keep >> j) & 1u) *p++ = (uint8_t)((j < 4 ? lo : hi) >> (8 * (j & 3)));
+      }
+      cur += __shfl_sync(0xffffffffu, incl, 31);
+    }
+  }
+};
+template <> struct EncIn<kKindF16S> : EncInSparse<kKindF16S> {};
+template <> struct EncIn<kKindBF16S> : EncInSparse<kKindBF16S> {};
 
 template <>
 struct EncIn<kKindF32> {
@@ -942,12 +1208,15 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   // groups in flight ahead of the one being coded: two, or one in a two-slot ring
   constexpr uint32_t kAhead = In::kRingSlots > 2 ? 2u : 1u;
   static_assert(In::kRingSlots >= 2 && (!TMA || kAhead == 2), "");
+  constexpr bool kSparse = isSparseKind(KIND);
   uint32_t state = kStateMin;
   uint32_t wa = stageAddr;
   const EncRegs rc = makeEncRegs(tabAddr, pb);
   const uint32_t fullRows = n >> 5;
   uint32_t r = 0;
   sp.spilled = 0;
+  uint32_t pcur = 0;  // sparse kinds: plane offset of the block's next kept byte
+  if constexpr (kSparse) pcur = __ldcg(planes.table + (elem0 >> 12));
   if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
     const uint32_t groups = fullRows / U;
     if (TMA) {
@@ -970,7 +1239,10 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
         mbarWait(ringBar + 8u * slot, (phases >> slot) & 1u);
         phases ^= 1u << slot;
         const uint32_t slotAddr = ringAddr + slot * kGroupBytes;
-        if (KIND != kKindBytes) In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
+        if constexpr (kSparse)
+          In::storeGroup(slotAddr, planes, pcur, lane);
+        else if (KIND != kKindBytes)
+          In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
         encodeGroup<WIDE, KIND>(state, slotAddr + lane * WB, rc, wa);
         slot = slot + 1 == In::kRingSlots ? 0u : slot + 1;
         slotNext = slotNext + 1 == In::kRingSlots ? 0u : slotNext + 1;
@@ -1001,7 +1273,10 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
         if (k + kAhead < groups) issue(k + kAhead, slotNext);
         cpAsyncCommit();
         const uint32_t slotAddr = ringAddr + slot * kGroupBytes;
-        if (KIND != kKindBytes) In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
+        if constexpr (kSparse)
+          In::storeGroup(slotAddr, planes, pcur, lane);
+        else if (KIND != kKindBytes)
+          In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
         encodeGroup<WIDE, KIND>(state, slotAddr + lane * WB, rc, wa);
         slot = slot + 1 == In::kRingSlots ? 0u : slot + 1;
         slotNext = slotNext + 1 == In::kRingSlots ? 0u : slotNext + 1;
@@ -1015,7 +1290,10 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   for (uint32_t j = 0; r < fullRows; ++r, ++j, e += 32) {
     if (sp.area && (j % U) == 0 && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
     const auto w = In::loadWord(in, e);
-    In::storeScalar(planes, elem0 + e, w);
+    if constexpr (kSparse)
+      In::storeRow(planes, pcur, w, true, rc.ltMask);
+    else
+      In::storeScalar(planes, elem0 + e, w);
     encodeStep<WIDE>(state, In::template tabOffsetOf<kStride>(w), rc, wa);
   }
   const uint32_t rem = n & 31u;
@@ -1023,7 +1301,10 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
     if (sp.area && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
     const bool valid = lane < rem;
     const auto w = valid ? In::loadWord(in, e) : 0u;
-    if (valid) In::storeScalar(planes, elem0 + e, w);
+    if constexpr (kSparse)
+      In::storeRow(planes, pcur, w, valid, rc.ltMask);
+    else if (valid)
+      In::storeScalar(planes, elem0 + e, w);
     encodeStepPartial<WIDE>(valid, state, In::template tabOffsetOf<kStride>(w), rc, wa);
   }
   stateOut = state;
@@ -1077,7 +1358,20 @@ __device__ __forceinline__ uint32_t lookbackWarp(volatile unsigned long long* de
 
 // dynamic shared memory per warp: [table 2 KiB][input ring 2 KiB][staging slot]
 __host__ __device__ constexpr uint32_t encWarpSmem(int pb, int kind) {
-  return kNumSymbols * 8u + encRingBytes(kind) + maxBlockWords(pb) * 2u;
+  return encTabBytes(kind) + encRingBytes(kind) + maxBlockWords(pb) * 2u;
+}
+
+// Sparse kinds: plane, table and keep flag of a member's archive from the header line the statistics pass
+// wrote; returns the bytes in front of the ANS archive.
+__device__ __forceinline__ uint32_t sparsePlanes(void* out, uint32_t size, StoredPlanes& pl) {
+  uint8_t* a = static_cast<uint8_t*>(out);
+  const uint4 h1 = __ldcg(reinterpret_cast<const uint4*>(a) + 1);  // S, esc
+  pl.table = reinterpret_cast<const uint32_t*>(a + kSparseHeaderBytes);
+  pl.non = a + kSparseHeaderBytes + sparseTableBytes<uint32_t>(size);
+  pl.keepAll = (h1.y >> 16) == 0u ? 1u : 0u;
+  __builtin_assume(__isGlobal(pl.non));
+  __builtin_assume(__isGlobal(pl.table));
+  return sparseExtraBytes<uint32_t>(size, h1.x);
 }
 
 template <int KIND>
@@ -1092,8 +1386,8 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
   uint8_t* mine = smem + (size_t)warp * encWarpSmem(pb, kind);
   uint4* myTab = reinterpret_cast<uint4*>(mine);
   const uint32_t tabAddr = smemAddr(mine);
-  const uint32_t ringAddr = tabAddr + kNumSymbols * 8u;
-  uint16_t* myStage = reinterpret_cast<uint16_t*>(mine + kNumSymbols * 8u + encRingBytes(kind));
+  const uint32_t ringAddr = tabAddr + encTabBytes(kind);
+  uint16_t* myStage = reinterpret_cast<uint16_t*>(mine + encTabBytes(kind) + encRingBytes(kind));
   const uint32_t stageAddr = smemAddr(myStage);
   volatile unsigned long long* desc = sc.lookback;
   uint32_t curMember = 0xffffffffu;
@@ -1122,6 +1416,9 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
     ansIn = static_cast<const uint8_t*>(md.in);
     if (kind == kKindBytes) {
       ansOut = static_cast<uint8_t*>(md.out);
+    } else if constexpr (isSparseKind(KIND)) {
+      extraBytes = sparsePlanes(md.out, size, planes);
+      ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
     } else {
       extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
       ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
@@ -1141,9 +1438,13 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
 
     if (m != curMember) {
       // this member's encoder table -> my private copy (written by K1's epilogue)
-      const uint4* src = sc.table + (size_t)m * kNumSymbols;
+      const uint4* src = sc.table + (size_t)m * tableSlots(KIND);
+      if constexpr (isSparseKind(KIND)) {
+        for (uint32_t i = lane; i < encTabVecs(false, KIND); i += 32u) myTab[i] = __ldcg(src + i);
+      } else {
 #pragma unroll
-      for (uint32_t i = 0; i < kNumSymbols / 64; ++i) myTab[i * 32 + lane] = __ldcg(src + i * 32 + lane);
+        for (uint32_t i = 0; i < kNumSymbols / 64; ++i) myTab[i * 32 + lane] = __ldcg(src + i * 32 + lane);
+      }
       curMember = m;
       __syncwarp();
     }
@@ -1246,10 +1547,10 @@ __device__ __forceinline__ WarpSmem warpSmem(const EncodeScratch& sc, uint8_t* s
 }
 
 // Loads member m's encoder table (written by the statistics epilogue) into the CTA's table slot.
-template <bool WIDE>
+template <bool WIDE, int KIND>
 __device__ __forceinline__ void loadTable(const EncodeScratch& sc, uint4* sTab, uint32_t m) {
-  const uint4* src = sc.table + (size_t)m * kNumSymbols;
-  for (uint32_t i = threadIdx.x; i < (WIDE ? kNumSymbols : kNumSymbols / 2); i += blockDim.x) sTab[i] = __ldcg(src + i);
+  const uint4* src = sc.table + (size_t)m * tableSlots(KIND);
+  for (uint32_t i = threadIdx.x; i < encTabVecs(WIDE, KIND); i += blockDim.x) sTab[i] = __ldcg(src + i);
 }
 
 // Warps of the CTA encode blocks [first, last) of member m (block k by warp (k - first) % W): the
@@ -1271,6 +1572,9 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
   ansIn = static_cast<const uint8_t*>(md.in);
   if (kind == kKindBytes) {
     ansOut = static_cast<uint8_t*>(md.out);
+  } else if constexpr (isSparseKind(KIND)) {
+    extraBytes = sparsePlanes(md.out, size, planes);
+    ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
   } else {
     extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
     ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
@@ -1331,7 +1635,7 @@ encodeKernelFast(EncodeScratch sc, const __grid_constant__ InlineMembers im, int
                                  uint32_t slotWords, uint32_t spillWarpBase,
                                  uint32_t* __restrict__ outSize) {
   extern __shared__ __align__(16) uint8_t smem[];
-  __shared__ __align__(16) uint4 sTab[WIDE ? kNumSymbols : kNumSymbols / 2];  // static: constant base for the hot LDS
+  __shared__ __align__(16) uint4 sTab[encTabVecs(WIDE, KIND)];  // static: constant base for the hot LDS
   __shared__ uint32_t sMember;
   const uint32_t t = threadIdx.x, lane = t & 31u;
   const uint32_t warp = __shfl_sync(0xffffffffu, t >> 5, 0);
@@ -1362,7 +1666,7 @@ encodeKernelFast(EncodeScratch sc, const __grid_constant__ InlineMembers im, int
     const MemberDesc md = memberAt(im, sc.members, m);
     const uint32_t nb = divUp(md.size, kBlockBytes);
     const uint32_t memberEnd = min(end, md.work0 + nb);
-    loadTable<WIDE>(sc, sTab, m);
+    loadTable<WIDE, KIND>(sc, sTab, m);
     __syncthreads();
     encodeMemberBlocks<WIDE, KIND>(sc, md, m, cur - md.work0, memberEnd - md.work0, pb, useChecksum, tabAddr, ws,
                                    warp, W, lane, outSize);
@@ -1495,7 +1799,7 @@ encodeFusedKernel(EncodeScratch sc, const uint32_t* __restrict__ histogramGiven,
     } else if (act == kActEncode) {
       const MemberDesc md = sc.members[m];
       if (tabMember != m) {
-        loadTable<WIDE>(sc, sTab, m);
+        loadTable<WIDE, KIND>(sc, sTab, m);
         tabMember = m;
         __syncthreads();
       }
@@ -1511,9 +1815,10 @@ encodeFusedKernel(EncodeScratch sc, const uint32_t* __restrict__ histogramGiven,
 }
 
 struct ScratchPlan {
-  size_t members, workIdx, uploadEnd, zeroBegin, hist, histDone, checksum, ticket, allocDone, ready, zeroEnd, lookback,
-      lookbackEnd, table, spill, total;
+  size_t members, workIdx, uploadEnd, zeroBegin, hist, histDone, checksum, ticket, allocDone, ready, zeroEnd,
+      lookback, lookbackEnd, table, spill, total;
   uint32_t spillWarps;
+  uint32_t blockZerosOff;
 };
 
 // Encoder warps that may need a spill slot (one slot = the worst-case stream of one block): never
@@ -1540,12 +1845,14 @@ ScratchPlan planScratch(int kind, uint32_t n, uint32_t maxSize, uint32_t totalTi
   p.checksum = o; o = alignUp256(o + sizeof(uint32_t) * (size_t)n);
   p.ticket = o; o = alignUp256(o + 16);
   p.allocDone = o; o = alignUp256(o + sizeof(unsigned long long) * (size_t)n);
-  p.ready = o; o = alignUp256(o + sizeof(uint32_t) * (size_t)n);
+  // sparse kinds: [2n] +0 / -0 words per member, then [totalTickets] +-0 words per block (zeroCounts, blockZeros)
+  p.blockZerosOff = isSparseKind(kind) ? roundUp(2u * n, 64u) : 0u;
+  p.ready = o; o = alignUp256(o + sizeof(uint32_t) * (isSparseKind(kind) ? (size_t)p.blockZerosOff + totalTickets : (size_t)n));
   p.zeroEnd = o;
   // look-back descriptors: canonical (ordered) layout only; cleared only then
   p.lookback = o; o = alignUp256(o + sizeof(unsigned long long) * (size_t)totalTickets);
   p.lookbackEnd = o;
-  p.table = o; o = alignUp256(o + sizeof(uint4) * kNumSymbols * (size_t)n);
+  p.table = o; o = alignUp256(o + sizeof(uint4) * tableSlots(kind) * (size_t)n);
   p.spillWarps = spillWarps;
   p.spill = o; o = alignUp256(o + (size_t)spillWarps * maxBlockWords(11) * 2u);
   p.total = o;
@@ -1578,7 +1885,10 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const uint32_t W = (uint32_t)std::max(1, std::min(opt.encode_warps, 8));  // warps per CTA (two-kernel path)
   const uint32_t elemBytes = wordBytes(kind);
   const bool canonical = opt.encode_canonical != 0;
-  const bool fused = !canonical && opt.encode_fused != 0;
+  // the sparse kinds have neither the fused launch nor the staged statistics kernel: those options run the
+  // default kernels for them (INTEGRATION.md section 4)
+  const bool sparse = isSparseKind(kind);
+  const bool fused = !canonical && opt.encode_fused != 0 && !sparse;
   // staging slot of the fast / fused encoder (spills to global scratch when a block needs more)
   uint32_t slotWords = opt.encode_slot_words > 0 ? (uint32_t)opt.encode_slot_words
                                                  : (kind == kKindBytes ? 2304u : (kind == kKindF64 ? kEncSlotWordsF64 : 1536u));
@@ -1646,11 +1956,12 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   sc.ready = reinterpret_cast<uint32_t*>(base + sp.ready);
   sc.spill = base + sp.spill;
   sc.table = reinterpret_cast<uint4*>(base + sp.table);
+  sc.blockZerosOff = sp.blockZerosOff;
+  const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0 && !sparse;
 
   // member table: inside the kernel parameters when it fits and the default kernels run, else uploaded to scratch
   static thread_local InlineMembers im;
-  const bool inlined = opt.inline_members != 0 && n <= kInlineMembers && !fused && !canonical &&
-                       !(kind != kKindBytes && opt.stats_stage != 0);
+  const bool inlined = opt.inline_members != 0 && n <= kInlineMembers && !fused && !canonical && !stagedK1;
   im.count = inlined ? n : 0u;
   if (inlined) {
     std::memcpy(im.m, desc, descBytes);
@@ -1663,13 +1974,17 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const int sms = smCount();
   // encoder table format (see EncSym in this file): wide entries for exponent-byte planes
   const bool wideTable = !canonical && opt.encode_wide_table != 0 &&
-                         (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32 || kind == DGB_FLOAT64);
+                         (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32 || kind == DGB_FLOAT64 ||
+                          kind == DGB_BFLOAT16_SPARSE);
   sc.wideTable = wideTable;
 
   if (fused) {
     // ---- one persistent launch: statistics items and encode chunks from two counters ----
     const uint32_t statsEvery = (uint32_t)std::max(0, opt.fused_stats_every);
     return withKind(kind, [&](auto K) { return withBool(wideTable, [&](auto WD) { return withBool(staged, [&](auto ST) {
+      if constexpr (isSparseKind(decltype(K)::value)) {
+        return (int)DGB_ERR_INVALID_ARG;  // not reached: `fused` is false for the sparse kinds
+      } else {
       auto kern = encodeFusedKernel<decltype(K)::value, decltype(WD)::value, decltype(ST)::value>;
       constexpr uint32_t W = kStatsThreads / 32;
       const size_t smemBytes = (size_t)W * encFastWarpSmem(slotWords, kind);
@@ -1687,6 +2002,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
       DGB_CUDA_TRY(cudaGetLastError());
       timerEnd(opt, kSlotFused, stream);
       return DGB_OK;
+      }
     }); }); });
   }
 
@@ -1695,7 +2011,6 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   SubBatches parts(kind, desc, n, opt, !canonical, stream);
   if (const int rc = parts.fork(); rc != DGB_OK) return rc;
   const uint32_t spillWarpsPerPart = sp.spillWarps / (uint32_t)parts.count();
-  const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0;
   const uint32_t slabVecsK1 = stagedK1 ? std::min<uint32_t>(slabVecs, (uint32_t)std::max(1, opt.stats_stage_kb) * 64u) : slabVecs;
   // K2 launch configuration (same for every part)
   const size_t smemBytes = (size_t)W * (canonical ? encWarpSmem(pb, kind) : encFastWarpSmem(slotWords, kind));
@@ -1734,6 +2049,8 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
       timerBegin(opt, kSlotStats, ps);
       if constexpr (KIND == kKindBytes) {
         statsBytesKernel<<<grid1, kStatsThreads, 0, ps>>>(sc, im, histogram_dev, pb, checksum, slabVecs, m0, outSize_dev);
+      } else if constexpr (isSparseKind(KIND)) {
+        statsFloatKernel<KIND><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
       } else if (stagedK1 && gridY * (uint64_t)slabVecsK1 >= maxVecs) {
         rc = residentCtasPerSm((const void*)statsFloatStagedKernel<KIND>, kStatsThreads, 0, 128 * 1024, nullptr);
         if (rc != DGB_OK) return rc;

@@ -32,6 +32,9 @@ K_DEFAULT_PRECISION = 10  # DietGpu.cpp:114
 _FLOAT_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32,
                 torch.float64: capi.FLOAT64}
 _DTYPE_OF = {v: k for k, v in _FLOAT_TYPES.items()}
+# sparse=True: fp16 / bf16 archives that code +0 and -0 words as two spare symbols and store no byte for them
+_SPARSE_TYPES = {torch.float16: capi.FLOAT16_SPARSE, torch.bfloat16: capi.BFLOAT16_SPARSE}
+_SPARSE_DTYPE_OF = {v: k for k, v in _SPARSE_TYPES.items()}
 
 
 def _check(cond: bool, msg: str = "") -> None:
@@ -39,9 +42,18 @@ def _check(cond: bool, msg: str = "") -> None:
         raise RuntimeError("dietgpu_b200 check failed" + (": " + msg if msg else ""))
 
 
-def _float_type(t: torch.Tensor) -> int:
+def _float_type(t: torch.Tensor, sparse: bool = False) -> int:
+    if sparse:
+        if t.dtype not in _SPARSE_TYPES:
+            raise ValueError(f"sparse=True needs float16 or bfloat16 tensors, not {t.dtype}")
+        return _SPARSE_TYPES[t.dtype]
     _check(t.dtype in _FLOAT_TYPES, f"unsupported float dtype {t.dtype}")
     return _FLOAT_TYPES[t.dtype]
+
+
+def _check_sparse(compress_as_float: bool, sparse: bool) -> None:
+    if sparse and not compress_as_float:
+        raise ValueError("sparse=True needs compress_as_float=True")
 
 
 def _stream() -> int:
@@ -98,13 +110,13 @@ def _bound(v: int, size: int) -> int:
     return v
 
 
-def max_float_compressed_output_size(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
+def max_float_compressed_output_size(ts: Sequence[torch.Tensor], *, sparse: bool = False) -> Tuple[int, int]:
     mx, _ = _max_numel_and_bytes(ts)
-    return len(ts), _bound(capi.lib().dgb_float_max_compressed_size(_float_type(ts[0]), mx), mx)
+    return len(ts), _bound(capi.lib().dgb_float_max_compressed_size(_float_type(ts[0], sparse), mx), mx)
 
 
-def max_float_compressed_size(dtype: torch.Tensor, size: int) -> int:
-    return _bound(capi.lib().dgb_float_max_compressed_size(_float_type(dtype), size), size)
+def max_float_compressed_size(dtype: torch.Tensor, size: int, *, sparse: bool = False) -> int:
+    return _bound(capi.lib().dgb_float_max_compressed_size(_float_type(dtype, sparse), size), size)
 
 
 def max_any_compressed_output_size(ts: Sequence[torch.Tensor]) -> Tuple[int, int]:
@@ -143,16 +155,17 @@ def _validate_out(out_compressed, out_sizes, n: int, cols: int, dev):
 def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checksum: bool = False,
                   temp_mem: Optional[torch.Tensor] = None, out_compressed: Optional[torch.Tensor] = None,
                   out_compressed_bytes: Optional[torch.Tensor] = None, *,
-                  prob_bits: int = K_DEFAULT_PRECISION):
+                  prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False):
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0, "empty batch")
     dev = ts_in[0].device
     for t in ts_in:
         _check(t.is_cuda and t.is_contiguous() and t.device == dev)
         if compress_as_float:
             _check(t.dtype == ts_in[0].dtype)
-            _float_type(t)
+            _float_type(t, sparse)
     n = len(ts_in)
-    _, cols = (max_float_compressed_output_size(ts_in) if compress_as_float
+    _, cols = (max_float_compressed_output_size(ts_in, sparse=sparse) if compress_as_float
                else max_any_compressed_output_size(ts_in))
     comp, sizes = _validate_out(out_compressed, out_compressed_bytes, n, cols, dev)
     row = comp.size(1)
@@ -161,7 +174,7 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
     L = capi.lib()
     with torch.cuda.device(dev):
         if compress_as_float:
-            ft = _float_type(ts_in[0])
+            ft = _float_type(ts_in[0], sparse)
             in_sizes = capi.u32_array([t.numel() for t in ts_in])
             need = L.dgb_float_compress_temp_bytes(ft, n, max(t.numel() for t in ts_in))
             tmp = _Temp(temp_mem, need, dev)
@@ -188,10 +201,11 @@ def compress_data_split_size(compress_as_float: bool, t_in: torch.Tensor, t_in_s
                              checksum: bool = False, temp_mem: Optional[torch.Tensor] = None,
                              out_compressed: Optional[torch.Tensor] = None,
                              out_compressed_bytes: Optional[torch.Tensor] = None, *,
-                             prob_bits: int = K_DEFAULT_PRECISION):
+                             prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False):
+    _check_sparse(compress_as_float, sparse)
     dev = t_in.device
     _check(t_in.is_cuda and t_in.is_contiguous())
-    ft = _float_type(t_in) if compress_as_float else 0
+    ft = _float_type(t_in, sparse) if compress_as_float else 0
     if not compress_as_float:
         _check(t_in.data_ptr() % 4 == 0, "start pointer is not aligned")
     _check(t_in_split_sizes.is_contiguous() and t_in_split_sizes.device.type == "cpu"
@@ -227,27 +241,31 @@ def compress_data_split_size(compress_as_float: bool, t_in: torch.Tensor, t_in_s
 
 
 def compress_data_simple(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checksum: bool = False,
-                         temp_mem: Optional[int] = 64 * 1024 * 1024) -> List[torch.Tensor]:
+                         temp_mem: Optional[int] = 64 * 1024 * 1024, *, sparse: bool = False) -> List[torch.Tensor]:
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0)
     scratch = None
     if temp_mem and temp_mem > 0:
         scratch = torch.empty(temp_mem, dtype=torch.uint8, device=ts_in[0].device)
-    comp, sizes, _ = compress_data(compress_as_float, ts_in, checksum, scratch, None, None)
+    comp, sizes, _ = compress_data(compress_as_float, ts_in, checksum, scratch, None, None, sparse=sparse)
     host = sizes.cpu().tolist()
     return [comp[i, :host[i]].clone() for i in range(len(ts_in))]
 
 
 def pull_archives(compress_as_float: bool, ts_src: Sequence[torch.Tensor], ts_dst: Sequence[torch.Tensor],
-                  float_dtype: Optional[torch.dtype] = None, out_bytes: Optional[torch.Tensor] = None) -> None:
+                  float_dtype: Optional[torch.dtype] = None, out_bytes: Optional[torch.Tensor] = None, *,
+                  sparse: bool = False) -> None:
     """Copies each archive of ts_src (uint8 rows, e.g. views of a peer GPU's memory) into the matching row of
     ts_dst, exactly as long as its header says (dgb_archives_pull): the transfer step of the compressed
-    collectives.  `float_dtype` names the float kind of the archives when compress_as_float."""
+    collectives.  `float_dtype` names the float kind of the archives when compress_as_float (`sparse`: archives
+    made with sparse=True)."""
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_src) > 0 and len(ts_src) == len(ts_dst))
     dev = ts_dst[0].device
     for a, b in zip(ts_src, ts_dst):
         _check(a.is_cuda and b.is_cuda and b.device == dev and a.dtype == torch.uint8 and b.dtype == torch.uint8)
         _check(a.is_contiguous() and b.is_contiguous())
-    ft = _float_type(torch.empty(0, dtype=float_dtype)) if compress_as_float else 0
+    ft = _float_type(torch.empty(0, dtype=float_dtype), sparse) if compress_as_float else 0
     if out_bytes is not None:
         _check(out_bytes.is_cuda and out_bytes.dtype == torch.int32 and out_bytes.numel() >= len(ts_src))
     with torch.cuda.device(dev):
@@ -282,7 +300,8 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
                     checksum: bool = False, temp_mem: Optional[torch.Tensor] = None,
                     out_status: Optional[torch.Tensor] = None,
                     out_decompressed_words: Optional[torch.Tensor] = None, *,
-                    prob_bits: int = K_DEFAULT_PRECISION) -> int:
+                    prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False) -> int:
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out))
     dev = ts_in[0].device
     n = len(ts_in)
@@ -292,7 +311,7 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
         _check_archive_aligned(ti)
         _check(to.is_cuda and to.device == dev and to.is_contiguous())
         if compress_as_float:
-            _float_type(to)
+            _float_type(to, sparse)
             # capacities are counted in words of one float type
             _check(to.dtype == ts_out[0].dtype, "float outputs must all have the same dtype")
         cap = to.numel() if compress_as_float else to.numel() * to.element_size()
@@ -305,7 +324,7 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
     cap_arr = capi.u32_array(caps)
     with torch.cuda.device(dev):
         if compress_as_float:
-            ft = _float_type(ts_out[0])
+            ft = _float_type(ts_out[0], sparse)
             need = L.dgb_float_decompress_temp_bytes(ft, n, max(caps))
             tmp = _Temp(temp_mem, need, dev)
             rc = L.dgb_float_decompress_pointer(tmp.ptr, tmp.bytes, ft, prob_bits, int(checksum), n, in_ptrs,
@@ -324,7 +343,8 @@ def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Te
                                temp_mem: Optional[torch.Tensor] = None,
                                out_status: Optional[torch.Tensor] = None,
                                out_decompressed_words: Optional[torch.Tensor] = None, *,
-                               prob_bits: int = K_DEFAULT_PRECISION) -> int:
+                               prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False) -> int:
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0)
     dev = ts_in[0].device
     n = t_out_split_sizes.numel()
@@ -338,7 +358,7 @@ def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Te
         _check(s > 0)
     _check(t_out.is_cuda and t_out.is_contiguous())
     _check(t_out.device == dev, "t_out is not on the device of the compressed inputs")
-    ft = _float_type(t_out) if compress_as_float else 0
+    ft = _float_type(t_out, sparse) if compress_as_float else 0
     _split_total(splits, t_out.numel() if compress_as_float else t_out.numel() * t_out.element_size(), "t_out")
     st_ptr, sz_ptr = _validate_status(out_status, out_decompressed_words, n, dev)
     L = capi.lib()
@@ -360,7 +380,8 @@ def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Te
 
 
 def decompress_data_simple(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checksum: bool = False,
-                           temp_mem: Optional[int] = 64 * 1024 * 1024) -> List[torch.Tensor]:
+                           temp_mem: Optional[int] = 64 * 1024 * 1024, *, sparse: bool = False) -> List[torch.Tensor]:
+    _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0)
     dev = ts_in[0].device
     n = len(ts_in)
@@ -381,15 +402,16 @@ def decompress_data_simple(compress_as_float: bool, ts_in: Sequence[torch.Tensor
                                                _stream())
     capi.check(rc, "get_compressed_info")
     hs, ht = sizes.cpu().tolist(), types.cpu().tolist()
+    dtype_of = _SPARSE_DTYPE_OF if sparse else _DTYPE_OF
     outs = []
     for i in range(n):
         if compress_as_float:
-            _check(ht[i] == ht[0] and ht[i] in _DTYPE_OF, "inconsistent / invalid float type in archives")
-            outs.append(torch.empty(hs[i], dtype=_DTYPE_OF[ht[i]], device=dev))
+            _check(ht[i] == ht[0] and ht[i] in dtype_of, "inconsistent / invalid float type in archives")
+            outs.append(torch.empty(hs[i], dtype=dtype_of[ht[i]], device=dev))
         else:
             outs.append(torch.empty(hs[i], dtype=torch.uint8, device=dev))
     scratch = None
     if temp_mem and temp_mem >= 256:
         scratch = torch.empty(temp_mem, dtype=torch.uint8, device=dev)
-    decompress_data(compress_as_float, ts_in, outs, checksum, scratch, None, None)
+    decompress_data(compress_as_float, ts_in, outs, checksum, scratch, None, None, sparse=sparse)
     return outs

@@ -57,6 +57,13 @@ extern "C" {
 #define DGB_BFLOAT16 2
 #define DGB_FLOAT32 3
 #define DGB_FLOAT64 4
+/* Sparse fp16 / bf16 (also this library's extension; the reference cannot read these archives either): the
+ * dense type's archive, except that +0 and -0 words are coded as two otherwise unused symbols and store no
+ * byte, so zero-heavy data (ReLU activations, masked or pruned tensors) compresses further.  The header is
+ * 32 B (the dense 16 B, then the stored-byte count and the two escape symbols), followed by a u32 per 4 KiB
+ * block, the stored bytes and the ANS archive (DESIGN.md section 0). */
+#define DGB_FLOAT16_SPARSE 5
+#define DGB_BFLOAT16_SPARSE 6
 
 /* ans/GpuANSCodec.h:16,20 */
 #define DGB_ANS_REQUIRED_ALIGNMENT 4
@@ -72,7 +79,8 @@ int dgb_last_cuda_error(void);
 /* ans/GpuANSEncode.cu:13-25 getMaxCompressedSize (same value, same quirk). */
 uint32_t dgb_ans_max_compressed_size(uint32_t uncompressed_bytes);
 /* float/GpuFloatCompress.cu:23-45 getMaxFloatCompressedSize; for DGB_FLOAT64, 16 + the ANS bound + the three
- * planes.  0 when the bound does not fit 32 bits (encode then returns DGB_ERR_TOO_LARGE). */
+ * planes; for the sparse types, 32 + 4 * roundUp(ceil(n / 4096), 4) + roundUp(n, 16) + the ANS bound.  0 when
+ * the bound does not fit 32 bits (encode then returns DGB_ERR_TOO_LARGE). */
 uint32_t dgb_float_max_compressed_size(int float_type, uint32_t num_floats);
 
 /* ---- scratch sizing (new; the reference sizes scratch implicitly through
@@ -202,7 +210,7 @@ int dgb_copy_rows_async(void* dst, size_t dst_pitch, const void* src, size_t src
 /* ---- archive mover (new; for the compressed collectives) -------------------- */
 /* Copies num_in_batch archives from src[i] to dst[i] (host arrays of device pointers, 16 B aligned), each
  * exactly as long as its own header says and at most dst_capacity[i] bytes: float_type 0 = ANS archives
- * (ans/GpuANSUtils.cuh:67-227 header), DGB_FLOAT16/BFLOAT16/FLOAT32/FLOAT64 = float archives
+ * (ans/GpuANSUtils.cuh:67-227 header), DGB_FLOAT16/BFLOAT16/FLOAT32/FLOAT64 and the sparse types = float archives
  * (float/GpuFloatUtils.cuh:26-74).  src may be memory of a peer GPU mapped into this process (NVLink):
  * sizes are read on the device, nothing travels to the host; out_bytes_dev (optional, device, [n]) receives
  * the archive sizes.  An archive with a bad header is copied as its first 32 bytes so that the decoder

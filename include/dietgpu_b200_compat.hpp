@@ -274,8 +274,17 @@ struct ANSDecodeStatus {
 };
 
 // ---- float/GpuFloatCodec.h:18-97 ----
-// kFloat64: this library's extension (archives of float type 4, which the reference cannot read)
-enum class FloatType : uint32_t { kUndefined = 0, kFloat16 = 1, kBFloat16 = 2, kFloat32 = 3, kFloat64 = 4 };
+// kFloat64, kFloat16Sparse, kBFloat16Sparse: this library's extensions (archives of float types 4, 5 and 6,
+// which the reference cannot read)
+enum class FloatType : uint32_t {
+  kUndefined = 0,
+  kFloat16 = 1,
+  kBFloat16 = 2,
+  kFloat32 = 3,
+  kFloat64 = 4,
+  kFloat16Sparse = 5,
+  kBFloat16Sparse = 6
+};
 
 inline uint32_t getMaxFloatCompressedSize(FloatType ft, uint32_t size) {
   return dgb_float_max_compressed_size((int)ft, size);
