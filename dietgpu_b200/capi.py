@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("DIETGPU_B200_LIB") or os.path.join(_HERE, "libdietgpu
 OK, ERR_INVALID_ARG, ERR_TEMP_TOO_SMALL, ERR_CUDA, ERR_CHECKSUM, ERR_TOO_LARGE, ERR_CAPTURING = range(7)
 FLOAT16, BFLOAT16, FLOAT32, FLOAT64 = 1, 2, 3, 4  # FLOAT64: archives the reference cannot read
 FLOAT16_SPARSE, BFLOAT16_SPARSE = 5, 6  # +-0 words coded as two spare symbols; the reference cannot read these either
+FLOAT32_SPARSE = 8  # the same for float32 words (7 is unassigned)
 
 # every symbol include/dietgpu_b200.h declares (tests check the .so exports all of them)
 SYMBOLS = [

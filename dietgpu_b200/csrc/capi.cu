@@ -350,7 +350,7 @@ uint32_t dgb_float_max_compressed_size(int ft, uint32_t n) {
   if (!validFloatType(ft)) return 0;
   const uint32_t ans = dgb_ans_max_compressed_size(n);
   if (ans == 0u) return 0u;  // too large (see above)
-  const uint64_t total = isSparseKind(ft) ? sparseExtraBytes<uint64_t>(n, n) + ans
+  const uint64_t total = isSparseKind(ft) ? sparseExtraBytes<uint64_t>(ft, n, n) + ans
                                           : (uint64_t)kFloatHeaderBytes + ans + floatPlanesBytes<uint64_t>(ft, n);
   return total <= 0xffffffffull ? (uint32_t)total : 0u;
 }

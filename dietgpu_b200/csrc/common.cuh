@@ -67,17 +67,34 @@ __host__ __device__ constexpr uint32_t floatNonCompBytes(int ft, uint32_t n) { r
 // nothing.  After the 32 B header (the dense 16 B, then S = words that store a byte, esc = E+ | E- << 8 | 1 << 16
 // or 0 when nothing is elided, 0, 0) come a u32 per 4 KiB block (stored bytes of all earlier blocks), the S
 // stored bytes in element order, and the ANS archive; every section starts 16 B aligned and is zero padded.
+// Sparse fp32 (type 8) is the same layout with the dense fp32 symbol (r >> 24, r = rotl32(w, 1)) and stored bits:
+// S counts the kept words, and the stored section is a u16 plane (2 roundUp(S, 8) B, r & 0xffff) followed by a u8
+// plane (roundUp(S, 16) B, bits 16..23 of r), both compacted in element order; the table counts kept words.
 constexpr uint32_t kSparseHeaderBytes = 32;
-__host__ __device__ constexpr bool isSparseKind(int ft) { return ft == DGB_FLOAT16_SPARSE || ft == DGB_BFLOAT16_SPARSE; }
-__host__ __device__ constexpr int denseKind(int ft) {  // the dense type whose symbol and stored byte a kind uses
-  return ft == DGB_FLOAT16_SPARSE ? DGB_FLOAT16 : ft == DGB_BFLOAT16_SPARSE ? DGB_BFLOAT16 : ft;
+__host__ __device__ constexpr bool isSparseKind(int ft) {
+  return ft == DGB_FLOAT16_SPARSE || ft == DGB_BFLOAT16_SPARSE || ft == DGB_FLOAT32_SPARSE;
+}
+__host__ __device__ constexpr int denseKind(int ft) {  // the dense type whose symbol and stored byte(s) a kind uses
+  return ft == DGB_FLOAT16_SPARSE    ? DGB_FLOAT16
+         : ft == DGB_BFLOAT16_SPARSE ? DGB_BFLOAT16
+         : ft == DGB_FLOAT32_SPARSE  ? DGB_FLOAT32
+                                     : ft;
 }
 template <class T>
 __host__ __device__ constexpr T sparseTableBytes(T n) { return T(4) * roundUpT<T>((n + 4095) / 4096, 4); }
-// header + block table + stored bytes in front of the ANS archive (S = stored bytes)
+// header + block table + stored bytes in front of the ANS archive of a sparse fp16 / bf16 archive (S = stored bytes)
 template <class T>
 __host__ __device__ constexpr T sparseExtraBytes(T n, T S) {
   return T(kSparseHeaderBytes) + sparseTableBytes<T>(n) + roundUpT<T>(S, 16);
+}
+// the same for any sparse kind ft (S = kept words): the stored section depends on the stored width
+template <class T>
+__host__ __device__ constexpr T sparseStoredBytes(int ft, T S) {
+  return ft == DGB_FLOAT32_SPARSE ? T(2) * roundUpT<T>(S, 8) + roundUpT<T>(S, 16) : roundUpT<T>(S, 16);
+}
+template <class T>
+__host__ __device__ constexpr T sparseExtraBytes(int ft, T n, T S) {
+  return T(kSparseHeaderBytes) + sparseTableBytes<T>(n) + sparseStoredBytes<T>(ft, S);
 }
 __host__ __device__ constexpr bool sparseEscValid(uint32_t esc) {
   return esc == 0u || ((esc >> 16) == 1u && (esc & 0xffu) < ((esc >> 8) & 0xffu));
@@ -95,7 +112,8 @@ enum CodecKind : int {
   kKindF32 = DGB_FLOAT32,
   kKindF64 = DGB_FLOAT64,
   kKindF16S = DGB_FLOAT16_SPARSE,
-  kKindBF16S = DGB_BFLOAT16_SPARSE
+  kKindBF16S = DGB_BFLOAT16_SPARSE,
+  kKindF32S = DGB_FLOAT32_SPARSE
 };
 
 struct MemberDesc {
@@ -190,7 +208,7 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
 void setLastCudaError(cudaError_t e);
 
 inline uint32_t wordBytes(int kind) {
-  return kind == kKindF64 ? 8u : (kind == kKindF32 ? 4u : (kind == kKindBytes ? 1u : 2u));
+  return kind == kKindF64 ? 8u : (kind == kKindF32 || kind == kKindF32S ? 4u : (kind == kKindBytes ? 1u : 2u));
 }
 inline size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
 int smCount();  // SMs of the current device, cached per device
@@ -271,6 +289,7 @@ int withKind(int kind, F&& f) {
     case kKindF64: return f(IntC<kKindF64>{});
     case kKindF16S: return f(IntC<kKindF16S>{});
     case kKindBF16S: return f(IntC<kKindBF16S>{});
+    case kKindF32S: return f(IntC<kKindF32S>{});
     default: return DGB_ERR_INVALID_ARG;
   }
 }

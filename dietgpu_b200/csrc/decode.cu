@@ -1,5 +1,5 @@
 // decode.cu -- batched rANS decode (bytes) and fused float decompress
-// (fp16/bf16/fp32/fp64, sparse fp16/bf16) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
+// (fp16/bf16/fp32/fp64, sparse fp16/bf16/fp32) for sm_90a (H100).  One launch per call (decodeFusedKernel, further down): a persistent grid
 // whose CTAs lease members (header checks and the 2^pb LUT from the archive's own pdf happen inside the
 // CTA) and whose warps claim 4 KiB blocks; lane states + compressed words of a block arrive by one TMA
 // bulk copy (cp.async.bulk + mbarrier), the 32-lane interleaved rANS decode of ans/GpuANSDecode.cuh:55-217
@@ -68,7 +68,10 @@ __device__ __forceinline__ ArchiveView openArchive(const uint8_t* in) {
     v.esc = sh.y;
     v.table = reinterpret_cast<const uint32_t*>(in + kSparseHeaderBytes);
     v.non = in + kSparseHeaderBytes + sparseTableBytes<uint32_t>(fh.y);
-    v.ans = in + sparseExtraBytes<uint32_t>(fh.y, sh.x);
+    if constexpr (KIND == kKindF32S)
+      v.ans = in + sparseExtraBytes<uint32_t>(KIND, fh.y, sh.x);
+    else
+      v.ans = in + sparseExtraBytes<uint32_t>(fh.y, sh.x);
   } else {
     // float/GpuFloatUtils.cuh:26-74 GpuFloatHeader
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(in));
@@ -292,6 +295,9 @@ struct RowWriterSparse {
 };
 template <> struct RowWriter<kKindF16S> : RowWriterSparse<kKindF16S> {};
 template <> struct RowWriter<kKindBF16S> : RowWriterSparse<kKindBF16S> {};
+// the kinds whose writer loads a block's whole stored segment (bulkIssue / copySync)
+__host__ __device__ constexpr bool copiesSegment(int kind) { return kind == kKindF16S || kind == kKindBF16S; }
+
 
 template <>
 struct RowWriter<kKindF64> {
@@ -402,6 +408,150 @@ struct RowWriter<kKindF32> {
   }
   __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
     out[row * 32u] = join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u));
+  }
+};
+
+// Sparse fp32: a block's kept words [begin, end) store 3 bytes each, up to 12 KiB per block, so the segment is
+// streamed instead of copied whole: windows of 512 kept words anchored at the segment's end (window w holds kept
+// words [max(begin, end - 512 (w + 1)), end - 512 w)), each as its u16 bytes and its u8 bytes widened to 16 B bounds
+// (<= 1040 + 528 B), in a ring of three slots.  Rows are walked backwards with a kept-word cursor as in
+// RowWriterSparse.  A row takes at most 32 kept words, so while the cursor is in window c the row reads windows c and
+// c + 1 only; when it crosses into c + 1, window c's slot takes window c + 3 (cp.async, 16 B per lane) and window
+// c + 2 must have landed.  The block starts with windows 0, 1 and 2 in flight (issued by setBlock, overlapping the
+// stream's own load).  Whether a window has landed is tracked here alone (cp.async.wait_group 0 covers any group),
+// so the generic loop's waits are only ever extra.
+template <>
+struct RowWriter<kKindF32S> {
+  static constexpr uint32_t kWinWords = 512, kWin8 = 1040;  // u8 bytes start at slot + kWin8
+  static constexpr uint32_t kRingSlotBytes = kWin8 + 528;    // 3 slots = 4704 bytes per warp
+  uint32_t* out;
+  const uint8_t* non16;  // u16 plane
+  const uint8_t* non8;   // u8 plane
+  uint32_t ring, lane, ltMask;
+  uint32_t ep, em;  // escape symbols; 0x100 / 0x101 (no symbol) when nothing is elided
+  uint32_t begin, end, numWin;
+  mutable uint32_t cur;            // kept index one past the next row's kept words
+  mutable uint32_t win, winLo;     // current window and its lowest kept index
+  mutable uint32_t trig;           // the next row needs slowPath() when cur < trig
+  mutable uint32_t issued, landed; // windows [0, issued) requested, [0, landed) known to be in shared memory
+  mutable uint32_t b16c, b8c, b16n, b8n;  // shared address of kept index 0 (u16 / u8) in windows win and win + 1
+  struct Cursor { uint32_t* o; };
+  __device__ __forceinline__ void setRing(uint32_t ringAddr, uint32_t l) {
+    ring = ringAddr;
+    lane = l;
+    ltMask = laneMaskLt();
+  }
+  __device__ __forceinline__ uint32_t winHi(uint32_t w) const { return end - kWinWords * w; }
+  __device__ __forceinline__ uint32_t winLow(uint32_t w) const {
+    const uint32_t hi = winHi(w);
+    return hi - begin > kWinWords ? hi - kWinWords : begin;
+  }
+  __device__ __forceinline__ uint32_t slotOf(uint32_t w) const { return ring + (w % 3u) * kRingSlotBytes; }
+  __device__ __forceinline__ void bases(uint32_t w, uint32_t& b16, uint32_t& b8) const {
+    const uint32_t lo = winLow(w);
+    b16 = slotOf(w) - ((2u * lo) & ~15u);
+    b8 = slotOf(w) + kWin8 - (lo & ~15u);
+  }
+  // requests window w into its slot (whole warp; the slot's previous window is no longer read)
+  __device__ __forceinline__ void issueWin(uint32_t w) const {
+    const uint32_t lo = winLow(w), hi = winHi(w);
+    const uint32_t a16 = (2u * lo) & ~15u, a8 = lo & ~15u;
+    const uint32_t c16 = (roundUp(2u * hi, 16u) - a16) >> 4, c8 = (roundUp(hi, 16u) - a8) >> 4;
+    const uint32_t slot = slotOf(w);
+    for (uint32_t i = lane; i < c16 + c8; i += 32u) {
+      if (i < c16)
+        cpAsync16(slot + 16u * i, non16 + a16 + 16u * i);
+      else
+        cpAsync16(slot + kWin8 + 16u * (i - c16), non8 + a8 + 16u * (i - c16));
+    }
+  }
+  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
+    out = static_cast<uint32_t*>(outBase) + (size_t)block * kBlockBytes + l;
+    const uint32_t nb = divUp(av.floatWords, kBlockBytes);
+    begin = __ldg(av.table + block);
+    end = block + 1 < nb ? __ldg(av.table + block + 1) : av.storedBytes;
+    non16 = av.non;
+    non8 = av.non + 2u * (size_t)roundUp(av.storedBytes, 8u);
+    __builtin_assume(__isGlobal(out));
+    __builtin_assume(__isGlobal(non16));
+    __builtin_assume(__isGlobal(non8));
+    const bool elide = av.esc != 0u;
+    ep = elide ? (av.esc & 0xffu) : 0x100u;
+    em = elide ? ((av.esc >> 8) & 0xffu) : 0x101u;
+    // a malformed table (end < begin, or a segment longer than a block) must not send the copies past the ring
+    if (end < begin || end - begin > kBlockBytes) end = begin;
+    numWin = divUp(end - begin, kWinWords);
+    cur = end;
+    win = 0;
+    winLo = winLow(0);
+    trig = 0xffffffffu;  // the first row waits for windows 0 and 1
+    // every window of the previous block has landed (its rows read them all); every lane is done reading the ring
+    __syncwarp();
+    issued = min(numWin, 3u);
+    if (issued > 0u) issueWin(0);
+    if (issued > 1u) issueWin(1);
+    cpAsyncCommit();
+    if (issued > 2u) issueWin(2);
+    cpAsyncCommit();
+    landed = 0;
+    bases(0, b16c, b8c);
+    bases(1, b16n, b8n);
+  }
+  __device__ __forceinline__ void slowPath() const {
+    if (landed == 0u) {
+      // windows 0 and 1 were committed before window 2's group and the decode loop's two (empty) groups
+      cpAsyncWait<3>();
+      __syncwarp();
+      landed = min(issued, 2u);
+    }
+    if (cur <= winLo && win + 1u < numWin) {  // the next row starts in window win + 1
+      ++win;
+      winLo = winLow(win);
+      b16c = b16n;
+      b8c = b8n;
+      if (win + 1u < numWin) {
+        bases(win + 1u, b16n, b8n);
+        if (landed <= win + 1u) {
+          cpAsyncWait<0>();
+          __syncwarp();
+          landed = issued;
+        }
+      }
+      if (issued < numWin && issued == win + 2u) {  // window win + 2 goes where window win - 1 was
+        __syncwarp();
+        issueWin(issued);
+        cpAsyncCommit();
+        ++issued;
+      }
+    }
+    trig = win + 1u < numWin ? winLo + 1u : 0u;
+  }
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t) const { return Cursor{out + row * 32u}; }
+  __device__ __forceinline__ void issue(uint32_t, uint32_t) const {}
+  // the word of this lane's element in the current row (whole warp; lanes with valid = false hold none)
+  __device__ __forceinline__ uint32_t word(uint32_t entry, bool valid) const {
+    if (cur < trig) slowPath();
+    const uint32_t s = entry & 0xffu;
+    const bool keep = valid && s != ep && s != em;
+    const uint32_t b = __ballot_sync(0xffffffffu, keep);
+    cur -= __popc(b);
+    const uint32_t idx = cur + __popc(b & ltMask);
+    const bool inCur = idx >= winLo;
+    uint32_t lo = 0, hi = 0;
+    if (keep) {
+      asm volatile("ld.shared.u16 %0, [%1];" : "=r"(lo) : "r"((inCur ? b16c : b16n) + 2u * idx));
+      asm volatile("ld.shared.u8 %0, [%1];" : "=r"(hi) : "r"((inCur ? b8c : b8n) + idx));
+    }
+    return keep ? RowWriter<kKindF32>::join(entry, lo, hi) : (s == ep ? 0u : 0x80000000u);
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = word(entry, true);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { out[row * 32u] = word(entry, true); }
+  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
+    const uint32_t w = word(entry, valid);
+    if (valid) out[row * 32u] = w;
   }
 };
 
@@ -865,7 +1015,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
           const uint32_t streamBytes = roundUp(words, 8u) * 2u;
           __syncwarp();
           if (lane == 0) {
-            if constexpr (isSparseKind(KIND)) {
+            if constexpr (copiesSegment(KIND)) {
               // the block's stored bytes ride on the same mbarrier
               mbarExpectTx(myBar, 128u + streamBytes + wr.bulkBytes());
               wr.bulkIssue(myBar);
@@ -881,7 +1031,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
           SmemStream st{smemAddr(mySlot + 128) + 2u * words};
           decodeBlockWarp<KIND, PB, false>(state, st, blockLen, lut, wr, lane);
         } else {
-          if constexpr (isSparseKind(KIND)) wr.copySync();
+          if constexpr (copiesSegment(KIND)) wr.copySync();
           const uint32_t state = __ldg(reinterpret_cast<const uint32_t*>(pStates) + block * 32u + lane);
           GmemStream st{stream + words};
           decodeBlockWarp<KIND, PB, false>(state, st, blockLen, lut, wr, lane);
@@ -1167,10 +1317,16 @@ __device__ __forceinline__ uint4 ldgNc(const uint4* p) {
 constexpr uint32_t kPullThreads = 512;
 constexpr uint32_t kPullChunkVecs = 4096;  // 64 KiB work units
 
-template <bool SPARSE>
+// SPARSE: 0 for the dense kinds, else the sparse kind (fp16 and bf16 lay out their sections alike)
+template <int SPARSE>
 __device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {  // inlined: kind folds where it is constant
   uint32_t extra = 0;
-  if constexpr (SPARSE) {  // fp16 and bf16 lay out their sections alike
+  if constexpr (SPARSE == kKindF32S) {
+    const uint4 fh = __ldg(reinterpret_cast<const uint4*>(a));
+    const uint4 sh = __ldg(reinterpret_cast<const uint4*>(a) + 1);
+    if (fh.x != kFloatMagicVersion || sh.x > fh.y) return 32u;
+    extra = sparseExtraBytes<uint32_t>(SPARSE, fh.y, sh.x);
+  } else if constexpr (SPARSE != 0) {
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(a));
     const uint4 sh = __ldg(reinterpret_cast<const uint4*>(a) + 1);
     if (fh.x != kFloatMagicVersion || sh.x > fh.y) return 32u;
@@ -1186,7 +1342,7 @@ __device__ __forceinline__ uint32_t archiveBytes(int kind, const uint8_t* a) {  
   return total > 0xfffffff0ull ? 32u : (uint32_t)total;
 }
 
-template <bool SPARSE>
+template <int SPARSE>
 __device__ __forceinline__ void pullArchivesBody(const InlineMembers& im, int kind, uint32_t* __restrict__ outBytes) {
   __shared__ uint32_t sFirst[kInlineMembers + 1];  // first chunk of member i
   __shared__ uint32_t sBytes[kInlineMembers];
@@ -1226,17 +1382,22 @@ __device__ __forceinline__ void pullArchivesBody(const InlineMembers& im, int ki
 __global__ void __launch_bounds__(kPullThreads)
 pullArchivesKernel(const __grid_constant__ InlineMembers im, int kind, uint32_t* __restrict__ outBytes) {
   __builtin_assume(kind != kKindF64);
-  pullArchivesBody<false>(im, kind, outBytes);
+  pullArchivesBody<0>(im, kind, outBytes);
 }
 // fp64 archives: their own instantiation, so the kernel above keeps its plane-size arithmetic
 __global__ void __launch_bounds__(kPullThreads)
 pullArchivesF64Kernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
-  pullArchivesBody<false>(im, kKindF64, outBytes);
+  pullArchivesBody<0>(im, kKindF64, outBytes);
 }
 // sparse fp16 / bf16 archives: sizes from the 32 B header
 __global__ void __launch_bounds__(kPullThreads)
 pullArchivesSparseKernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
-  pullArchivesBody<true>(im, kKindF16S, outBytes);
+  pullArchivesBody<kKindF16S>(im, kKindF16S, outBytes);
+}
+// sparse fp32 archives: the same header, two stored planes
+__global__ void __launch_bounds__(kPullThreads)
+pullArchivesSparse32Kernel(const __grid_constant__ InlineMembers im, uint32_t* __restrict__ outBytes) {
+  pullArchivesBody<kKindF32S>(im, kKindF32S, outBytes);
 }
 }  // namespace
 
@@ -1262,6 +1423,8 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
     uint32_t* ob = outBytes_dev ? outBytes_dev + i0 : nullptr;
     if (kind == kKindF64)
       pullArchivesF64Kernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
+    else if (kind == kKindF32S)
+      pullArchivesSparse32Kernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
     else if (isSparseKind(kind))
       pullArchivesSparseKernel<<<ctas, kPullThreads, 0, stream>>>(im, ob);
     else

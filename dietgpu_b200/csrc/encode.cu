@@ -1,4 +1,4 @@
-// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16)
+// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16/fp32)
 // for sm_90a (H100).  Two launches per call, whatever the batch size:
 //
 //   K1  stats*Kernel     a pure read of the raw input: 256-bin histogram of the coded byte, taken out of
@@ -463,9 +463,65 @@ __device__ __forceinline__ void histZeroVectors(const uint4* __restrict__ vec, u
   }
 }
 
+// Sparse fp32: the same counts over 16 B vectors of four 32-bit words (a warp's 32 vectors are 128 consecutive
+// elements, so they too touch at most two blocks).  `head` = elements before the first vector (0..3).
+__device__ __forceinline__ uint32_t zeroMask4(const uint4& v, uint32_t& pz, uint32_t& nz) {
+  const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+  uint32_t m = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    m |= (uint32_t)((w4[q] & 0x7fffffffu) == 0u) << q;
+    pz += (uint32_t)(w4[q] == 0u);
+    nz += (uint32_t)(w4[q] == 0x80000000u);
+  }
+  return m;
+}
+__device__ __forceinline__ void histZeroVectors32(const uint4* __restrict__ vec, uint32_t v0, uint32_t v1, uint32_t t,
+                                                  uint32_t* wh, uint32_t head, uint32_t* __restrict__ bz,
+                                                  uint32_t& pz, uint32_t& nz) {
+  const uint32_t lane = t & 31u;
+  for (uint32_t w0 = v0 + (t & ~31u); w0 < v1; w0 += kStatsUnroll * kStatsThreads) {  // warp-uniform
+    uint4 vv[kStatsUnroll];
+#pragma unroll
+    for (int k = 0; k < kStatsUnroll; ++k) {
+      const uint32_t i = w0 + lane + k * kStatsThreads;
+      vv[k] = i < v1 ? ldStream16(vec + i) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int k = 0; k < kStatsUnroll; ++k) {
+      const uint32_t wi = w0 + k * kStatsThreads;  // the warp's first vector
+      if (wi >= v1) break;
+      const uint32_t i = wi + lane;
+      const uint32_t wb = (head + 4u * wi) >> 12;  // block of the warp's first element
+      uint32_t c0 = 0, c1 = 0;                     // +-0 words in blocks wb and wb + 1
+      if (i < v1) {
+        histAdd(wh, histOffLo<DGB_FLOAT32>(vv[k].x));
+        histAdd(wh, histOffLo<DGB_FLOAT32>(vv[k].y));
+        histAdd(wh, histOffLo<DGB_FLOAT32>(vv[k].z));
+        histAdd(wh, histOffLo<DGB_FLOAT32>(vv[k].w));
+        const uint32_t zm = zeroMask4(vv[k], pz, nz);
+        const uint32_t e0 = head + 4u * i, bA = e0 >> 12;
+        uint32_t cA = __popc(zm), cB = 0;
+        if (((e0 + 3u) >> 12) != bA) {  // straddles a boundary: elements j < 4 - head are in block bA
+          const uint32_t j = 4u - head;
+          cA = __popc(zm & ((1u << j) - 1u));
+          cB = __popc(zm >> j);
+        }
+        c0 = bA == wb ? cA : 0u;
+        c1 = bA == wb ? cB : cA;
+      }
+      const uint32_t s0 = __reduce_add_sync(0xffffffffu, c0), s1 = __reduce_add_sync(0xffffffffu, c1);
+      if (lane == 0) {
+        if (s0) atomicAdd(bz + wb, s0);
+        if (s1) atomicAdd(bz + wb + 1, s1);
+      }
+    }
+  }
+}
+
 // Last CTA of a sparse member (256 threads, thread t = symbol t): picks E+ and E-, moves the +0 / -0 counts from
-// their natural symbols (+0: 0; -0: 0x80 for fp16, 0 for bf16) to them, normalises, and writes the block table,
-// the 32 B header, the zero padding of the table and the stored bytes, the pdf and the encoder table.
+// their natural symbols (+0: 0; -0: 0x80 for fp16, 0 for bf16 and fp32) to them, normalises, and writes the block
+// table, the 32 B header, the zero padding of the table and the stored plane(s), the pdf and the encoder table.
 template <int FT>
 __device__ void finishSparseMember(const EncodeScratch& sc, int pb, bool useChecksum, const MemberDesc& md, uint32_t m,
                                    uint32_t* __restrict__ outSize) {
@@ -510,14 +566,24 @@ __device__ void finishSparseMember(const EncodeScratch& sc, int pb, bool useChec
   }
   for (uint32_t b = nb + t; b < roundUp(nb, 4u); b += kStatsThreads) table[b] = 0;
   uint8_t* plane = archive + kSparseHeaderBytes + sparseTableBytes<uint32_t>(size);
-  for (uint32_t i = S + t; i < roundUp(S, 16u); i += kStatsThreads) plane[i] = 0;
+  if constexpr (FT == kKindF32S) {  // u16 plane, then u8 plane
+    const uint32_t p8 = 2u * roundUp(S, 8u);
+    for (uint32_t i = 2u * S + t; i < p8; i += kStatsThreads) plane[i] = 0;
+    for (uint32_t i = S + t; i < roundUp(S, 16u); i += kStatsThreads) plane[p8 + i] = 0;
+  } else {
+    for (uint32_t i = S + t; i < roundUp(S, 16u); i += kStatsThreads) plane[i] = 0;
+  }
   if (t == 0) {
     uint4* h = reinterpret_cast<uint4*>(archive);
     h[0] = make_uint4(kFloatMagicVersion, size, (uint32_t)FT | ((useChecksum ? 1u : 0u) << 4),
                       useChecksum ? __ldcg(sc.checksum + m) : 0u);
     h[1] = make_uint4(S, esc, 0u, 0u);
   }
-  uint8_t* ansArchive = archive + sparseExtraBytes<uint32_t>(size, S);
+  uint8_t* ansArchive;
+  if constexpr (FT == kKindF32S)
+    ansArchive = archive + sparseExtraBytes<uint32_t>(FT, size, S);
+  else
+    ansArchive = archive + sparseExtraBytes<uint32_t>(size, S);
   if (size == 0) {
     publishEmptyMember(ansArchive, pb, false, outSize, m, kSparseHeaderBytes);
     return;
@@ -594,7 +660,9 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
       }
       // four independent 16 B loads per thread are issued before any of them is consumed: the
       // kernel is a pure stream and was latency-bound with one load in flight
-      if constexpr (SPARSE)
+      if constexpr (FT == kKindF32S)
+        histZeroVectors32(vec, v0, v1, t, wh, head, blockZeros(sc, md.work0), pz, nz);
+      else if constexpr (SPARSE)
         histZeroVectors<BT>(vec, v0, v1, t, wh, head, blockZeros(sc, md.work0), pz, nz);
       else
         histVectors<FT, STAGED>(vec, stage, v0, v1, t, wh);
@@ -604,18 +672,33 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
         // scalar head and tail; the 32 B header, the table and the padding are written by the last CTA
         const uint32_t tailStart = head + nVec * EPV;
         uint32_t* bz = blockZeros(sc, md.work0);
-        const uint16_t* in16 = reinterpret_cast<const uint16_t*>(in);
-        auto scalar = [&](uint32_t e) {
-          const uint32_t w = in16[e];
-          atomicAdd(&wh[BT == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8], 1u);
-          if ((w & 0x7fffu) == 0u) {
-            pz += w == 0u;
-            nz += w != 0u;
-            atomicAdd(bz + (e >> 12), 1u);
-          }
-        };
-        if (t < head) scalar(t);
-        if (t < size - tailStart) scalar(tailStart + t);
+        if constexpr (FT == kKindF32S) {
+          const uint32_t* in32 = reinterpret_cast<const uint32_t*>(in);
+          auto scalar = [&](uint32_t e) {
+            const uint32_t w = in32[e];
+            atomicAdd(&wh[(w >> 23) & 0xffu], 1u);
+            if ((w & 0x7fffffffu) == 0u) {
+              pz += w == 0u;
+              nz += w != 0u;
+              atomicAdd(bz + (e >> 12), 1u);
+            }
+          };
+          if (t < head) scalar(t);
+          if (t < size - tailStart) scalar(tailStart + t);
+        } else {
+          const uint16_t* in16 = reinterpret_cast<const uint16_t*>(in);
+          auto scalar = [&](uint32_t e) {
+            const uint32_t w = in16[e];
+            atomicAdd(&wh[BT == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8], 1u);
+            if ((w & 0x7fffu) == 0u) {
+              pz += w == 0u;
+              nz += w != 0u;
+              atomicAdd(bz + (e >> 12), 1u);
+            }
+          };
+          if (t < head) scalar(t);
+          if (t < size - tailStart) scalar(tailStart + t);
+        }
       }
       const uint32_t p = __reduce_add_sync(0xffffffffu, pz), q = __reduce_add_sync(0xffffffffu, nz);
       if ((t & 31u) == 0u) {
@@ -928,6 +1011,129 @@ struct EncIn<kKindF32> {
   }
 };
 
+// Sparse fp32: a +0 / -0 word looks up table entry 256 / 257, every other word its exponent symbol.  The kept words'
+// 16 + 8 stored bits are compacted into the u16 and u8 planes in element order.  A group of 16 rows (512 words in the
+// ring slot) goes in two steps: lane l takes words 16 l .. 16 l + 15 and one warp scan of the lanes' kept counts
+// places its kept words in the warp's run (shared memory after the ring: a u16 half and a u8 half); then every
+// complete unit of 16 kept words in the run goes to the planes as aligned 16 B vector stores (one u8 vector, two u16
+// vectors), and the last partial unit moves to the run's start, carried over to the next group.  Run position p holds
+// the kept word with plane index (cur & ~15) + p, so units are 16-word aligned in both planes.  A warp stores only the
+// bytes its block owns, kept words [lo, segment end) with lo = table[block]: segments are not 16-word aligned, so the
+// unit that starts below lo is stored word by word, and so is the partial unit left after the last group (flushTail).
+// The scalar paths (unaligned input, the remaining rows, the partial row) store word by word too.
+template <>
+struct EncIn<kKindF32S> {
+  static constexpr uint32_t kWordBytes = 4, kRingSlots = 3;
+  static constexpr uint32_t kRingGroupBytes = kRingSlots * kEncGroupRows * 128u;  // the run starts here
+  static constexpr uint32_t kRun8 = 1056u;                                        // u8 half (u16 half: 528 x 2 B)
+  static constexpr uint32_t kRunBytes = kRun8 + 528u;                             // a run holds < 16 + 512 words
+  template <uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffsetOf(uint32_t w) {
+    return STRIDE * ((w & 0x7fffffffu) == 0u ? 256u + (w >> 31) : (w >> 23) & 0xffu);
+  }
+  template <int J, uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffset(uint32_t ringLane) {
+    uint32_t w;
+    asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(w) : "r"(ringLane), "n"(J * 128));
+    return tabOffsetOf<STRIDE>(w);
+  }
+  static __device__ __forceinline__ uint32_t loadWord(const uint8_t* in, uint32_t e) {
+    return __ldg(reinterpret_cast<const uint32_t*>(in) + e);
+  }
+  // kept word idx of the planes <- r's low 24 bits
+  static __device__ __forceinline__ void storeWord(const StoredPlanes& pl, uint32_t idx, uint32_t r) {
+    reinterpret_cast<uint16_t*>(pl.non)[idx] = (uint16_t)r;
+    pl.non1[idx] = (uint8_t)(r >> 16);
+  }
+  // run position p as r's low 24 bits
+  static __device__ __forceinline__ uint32_t runWord(uint32_t run, uint32_t p) {
+    uint32_t lo16, hi8;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(lo16) : "r"(run + 2u * p));
+    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(hi8) : "r"(run + kRun8 + p));
+    return lo16 | (hi8 << 16);
+  }
+  static __device__ __forceinline__ void setRunWord(uint32_t run, uint32_t p, uint32_t r) {
+    asm volatile("st.shared.u16 [%0], %1;" ::"r"(run + 2u * p), "h"((unsigned short)r) : "memory");
+    asm volatile("st.shared.u8 [%0], %1;" ::"r"(run + kRun8 + p), "r"(r >> 16) : "memory");
+  }
+  // one row of words, whole warp (lanes without a word pass valid = false)
+  static __device__ __forceinline__ void storeRow(const StoredPlanes& pl, uint32_t& cur, uint32_t w, bool valid,
+                                                  uint32_t ltMask) {
+    const bool keep = valid && (pl.keepAll != 0u || (w & 0x7fffffffu) != 0u);
+    const uint32_t b = __ballot_sync(0xffffffffu, keep);
+    if (keep) storeWord(pl, cur + __popc(b & ltMask), __funnelshift_l(w, w, 1));
+    cur += __popc(b);
+  }
+  // one group of 16 rows in the ring slot at `slot`; `run` = shared address of the warp's run
+  static __device__ __forceinline__ void storeGroup(uint32_t slot, const StoredPlanes& pl, uint32_t& cur, uint32_t lo,
+                                                    uint32_t run, uint32_t lane) {
+    uint32_t w[16];
+#pragma unroll
+    for (int h = 0; h < 4; ++h)
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                   : "=r"(w[4 * h]), "=r"(w[4 * h + 1]), "=r"(w[4 * h + 2]), "=r"(w[4 * h + 3])
+                   : "r"(slot + lane * 64u + h * 16u));
+    uint32_t keep = 0xffffu;
+    if (!pl.keepAll) {
+      keep = 0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) keep |= (uint32_t)((w[j] & 0x7fffffffu) != 0u) << j;
+    }
+    const uint32_t c = __popc(keep);
+    uint32_t incl = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t x = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= (uint32_t)d) incl += x;
+    }
+    const uint32_t k = __shfl_sync(0xffffffffu, incl, 31);
+    // 1. compaction into the run
+    const uint32_t p = (cur & 15u) + incl - c;
+    uint32_t a16 = run + 2u * p, a8 = run + kRun8 + p;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      if ((keep >> j) & 1u) {
+        const uint32_t r = __funnelshift_l(w[j], w[j], 1);
+        asm volatile("st.shared.u16 [%0], %1;" ::"r"(a16), "h"((unsigned short)r) : "memory");
+        asm volatile("st.shared.u8 [%0], %1;" ::"r"(a8), "r"(r >> 16) : "memory");
+        a16 += 2u;
+        a8 += 1u;
+      }
+    }
+    __syncwarp();
+    // 2. complete units to the planes (lane u takes unit u); the partial unit's words into registers
+    const uint32_t A = cur & ~15u, total = (cur & 15u) + k, units = total >> 4, tail = total & 15u;
+    if (lane < units) {
+      const uint32_t v = A + 16u * lane;
+      if (v >= lo) {
+        uint4 x, y, z;
+        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w) : "r"(run + 32u * lane));
+        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(y.x), "=r"(y.y), "=r"(y.z), "=r"(y.w) : "r"(run + 32u * lane + 16u));
+        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(z.x), "=r"(z.y), "=r"(z.z), "=r"(z.w) : "r"(run + kRun8 + 16u * lane));
+        uint4* d16 = reinterpret_cast<uint4*>(pl.non + 2u * (size_t)v);
+        d16[0] = x;
+        d16[1] = y;
+        *reinterpret_cast<uint4*>(pl.non1 + v) = z;
+      } else {  // the block's first unit starts inside the previous block's segment
+        for (uint32_t i = lo - v; i < 16u; ++i) storeWord(pl, v + i, runWord(run, 16u * lane + i));
+      }
+    }
+    const bool move = units != 0u && lane < tail;
+    const uint32_t carry = move ? runWord(run, 16u * units + lane) : 0u;
+    __syncwarp();
+    if (move) setRunWord(run, lane, carry);
+    __syncwarp();
+    cur += k;
+  }
+  // the partial unit left in the run after the last group: kept words [max(cur & ~15, lo), cur)
+  static __device__ __forceinline__ void flushTail(const StoredPlanes& pl, uint32_t cur, uint32_t lo, uint32_t run,
+                                                   uint32_t lane) {
+    const uint32_t idx = (cur & ~15u) + lane;
+    if (lane < (cur & 15u) && idx >= lo) storeWord(pl, idx, runWord(run, lane));
+    __syncwarp();
+  }
+};
+
 #ifndef DGB_ENC_RING64
 #define DGB_ENC_RING64 3
 #endif
@@ -979,8 +1185,9 @@ struct EncIn<kKindF64> {
   }
 };
 
-__host__ __device__ constexpr uint32_t encRingBytes(int kind) {
-  return kind == kKindF64 ? (uint32_t)DGB_ENC_RING64 * kEncGroupRows * 256u
+__host__ __device__ constexpr uint32_t encRingBytes(int kind) {  // sparse fp32: the ring, then the warp's run
+  return kind == kKindF32S ? EncIn<kKindF32S>::kRingGroupBytes + EncIn<kKindF32S>::kRunBytes
+         : kind == kKindF64 ? (uint32_t)DGB_ENC_RING64 * kEncGroupRows * 256u
          : kind == kKindBytes
              ? 4u * kEncGroupRows * 32u
              : (kind == kKindF32 ? 3u * kEncGroupRows * 128u : (uint32_t)DGB_ENC_RING16 * kEncGroupRows * 64u);
@@ -1217,6 +1424,8 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   sp.spilled = 0;
   uint32_t pcur = 0;  // sparse kinds: plane offset of the block's next kept byte
   if constexpr (kSparse) pcur = __ldcg(planes.table + (elem0 >> 12));
+  [[maybe_unused]] const uint32_t plo = pcur;  // sparse fp32: the block's first kept word, and the warp's run
+  [[maybe_unused]] const uint32_t run = ringAddr + EncIn<kKindF32S>::kRingGroupBytes;
   if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
     const uint32_t groups = fullRows / U;
     if (TMA) {
@@ -1239,7 +1448,9 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
         mbarWait(ringBar + 8u * slot, (phases >> slot) & 1u);
         phases ^= 1u << slot;
         const uint32_t slotAddr = ringAddr + slot * kGroupBytes;
-        if constexpr (kSparse)
+        if constexpr (KIND == kKindF32S)
+          In::storeGroup(slotAddr, planes, pcur, plo, run, lane);
+        else if constexpr (kSparse)
           In::storeGroup(slotAddr, planes, pcur, lane);
         else if (KIND != kKindBytes)
           In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
@@ -1273,7 +1484,9 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
         if (k + kAhead < groups) issue(k + kAhead, slotNext);
         cpAsyncCommit();
         const uint32_t slotAddr = ringAddr + slot * kGroupBytes;
-        if constexpr (kSparse)
+        if constexpr (KIND == kKindF32S)
+          In::storeGroup(slotAddr, planes, pcur, plo, run, lane);
+        else if constexpr (kSparse)
           In::storeGroup(slotAddr, planes, pcur, lane);
         else if (KIND != kKindBytes)
           In::storeGroup(slotAddr, planes, elem0 + k * (U * 32), lane);
@@ -1282,6 +1495,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
         slotNext = slotNext + 1 == In::kRingSlots ? 0u : slotNext + 1;
       }
     }
+    if constexpr (KIND == kKindF32S) In::flushTail(planes, pcur, plo, run, lane);
     r = groups * U;
   }
   // remaining rows (fewer than U, or all of them when the input is not 16 B aligned): every U rows
@@ -1363,6 +1577,8 @@ __host__ __device__ constexpr uint32_t encWarpSmem(int pb, int kind) {
 
 // Sparse kinds: plane, table and keep flag of a member's archive from the header line the statistics pass
 // wrote; returns the bytes in front of the ANS archive.
+// (sparse fp32: `non` is the u16 plane and `non1` the u8 plane)
+template <int KIND>
 __device__ __forceinline__ uint32_t sparsePlanes(void* out, uint32_t size, StoredPlanes& pl) {
   uint8_t* a = static_cast<uint8_t*>(out);
   const uint4 h1 = __ldcg(reinterpret_cast<const uint4*>(a) + 1);  // S, esc
@@ -1371,7 +1587,13 @@ __device__ __forceinline__ uint32_t sparsePlanes(void* out, uint32_t size, Store
   pl.keepAll = (h1.y >> 16) == 0u ? 1u : 0u;
   __builtin_assume(__isGlobal(pl.non));
   __builtin_assume(__isGlobal(pl.table));
-  return sparseExtraBytes<uint32_t>(size, h1.x);
+  if constexpr (KIND == kKindF32S) {
+    pl.non1 = pl.non + 2u * roundUp(h1.x, 8u);
+    __builtin_assume(__isGlobal(pl.non1));
+    return sparseExtraBytes<uint32_t>(KIND, size, h1.x);
+  } else {
+    return sparseExtraBytes<uint32_t>(size, h1.x);
+  }
 }
 
 template <int KIND>
@@ -1417,7 +1639,7 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
     if (kind == kKindBytes) {
       ansOut = static_cast<uint8_t*>(md.out);
     } else if constexpr (isSparseKind(KIND)) {
-      extraBytes = sparsePlanes(md.out, size, planes);
+      extraBytes = sparsePlanes<KIND>(md.out, size, planes);
       ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
     } else {
       extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
@@ -1573,7 +1795,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
   if (kind == kKindBytes) {
     ansOut = static_cast<uint8_t*>(md.out);
   } else if constexpr (isSparseKind(KIND)) {
-    extraBytes = sparsePlanes(md.out, size, planes);
+    extraBytes = sparsePlanes<KIND>(md.out, size, planes);
     ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
   } else {
     extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
@@ -1975,7 +2197,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   // encoder table format (see EncSym in this file): wide entries for exponent-byte planes
   const bool wideTable = !canonical && opt.encode_wide_table != 0 &&
                          (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32 || kind == DGB_FLOAT64 ||
-                          kind == DGB_BFLOAT16_SPARSE);
+                          kind == DGB_BFLOAT16_SPARSE || kind == DGB_FLOAT32_SPARSE);
   sc.wideTable = wideTable;
 
   if (fused) {

@@ -32,8 +32,9 @@ K_DEFAULT_PRECISION = 10  # DietGpu.cpp:114
 _FLOAT_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32,
                 torch.float64: capi.FLOAT64}
 _DTYPE_OF = {v: k for k, v in _FLOAT_TYPES.items()}
-# sparse=True: fp16 / bf16 archives that code +0 and -0 words as two spare symbols and store no byte for them
-_SPARSE_TYPES = {torch.float16: capi.FLOAT16_SPARSE, torch.bfloat16: capi.BFLOAT16_SPARSE}
+# sparse=True: fp16 / bf16 / fp32 archives that code +0 and -0 words as two spare symbols and store no bits for them
+_SPARSE16_TYPES = {torch.float16: capi.FLOAT16_SPARSE, torch.bfloat16: capi.BFLOAT16_SPARSE}
+_SPARSE_TYPES = {**_SPARSE16_TYPES, torch.float32: capi.FLOAT32_SPARSE}
 _SPARSE_DTYPE_OF = {v: k for k, v in _SPARSE_TYPES.items()}
 
 
@@ -45,7 +46,7 @@ def _check(cond: bool, msg: str = "") -> None:
 def _float_type(t: torch.Tensor, sparse: bool = False) -> int:
     if sparse:
         if t.dtype not in _SPARSE_TYPES:
-            raise ValueError(f"sparse=True needs float16 or bfloat16 tensors, not {t.dtype}")
+            raise ValueError(f"sparse=True needs float16, bfloat16 or float32 tensors, not {t.dtype}")
         return _SPARSE_TYPES[t.dtype]
     _check(t.dtype in _FLOAT_TYPES, f"unsupported float dtype {t.dtype}")
     return _FLOAT_TYPES[t.dtype]
@@ -116,6 +117,12 @@ def max_float_compressed_output_size(ts: Sequence[torch.Tensor], *, sparse: bool
 
 
 def max_float_compressed_size(dtype: torch.Tensor, size: int, *, sparse: bool = False) -> int:
+    """The single-size bound keeps its original `sparse=True` contract, float16 / bfloat16 only; the bound of a
+    sparse float32 archive comes from max_float_compressed_output_size(ts, sparse=True) (or, for a size alone, from
+    capi.lib().dgb_float_max_compressed_size(capi.FLOAT32_SPARSE, size))."""
+    if sparse and dtype.dtype not in _SPARSE16_TYPES:
+        raise ValueError(f"max_float_compressed_size(sparse=True) takes float16 or bfloat16, not {dtype.dtype}; "
+                         "size sparse float32 archives with max_float_compressed_output_size(ts, sparse=True)")
     return _bound(capi.lib().dgb_float_max_compressed_size(_float_type(dtype, sparse), size), size)
 
 

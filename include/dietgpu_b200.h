@@ -64,6 +64,11 @@ extern "C" {
  * block, the stored bytes and the ANS archive (DESIGN.md section 0). */
 #define DGB_FLOAT16_SPARSE 5
 #define DGB_BFLOAT16_SPARSE 6
+/* Sparse fp32 (the same extension for float32 words): +0 and -0 words are coded as two otherwise unused exponent
+ * symbols and store none of their 24 low bits; every other word stores them as in DGB_FLOAT32, in a compacted u16
+ * plane and a compacted u8 plane.  Same 32 B header and block table as the 16-bit sparse types (DESIGN.md
+ * section 0).  7 stays unassigned. */
+#define DGB_FLOAT32_SPARSE 8
 
 /* ans/GpuANSCodec.h:16,20 */
 #define DGB_ANS_REQUIRED_ALIGNMENT 4
@@ -79,8 +84,9 @@ int dgb_last_cuda_error(void);
 /* ans/GpuANSEncode.cu:13-25 getMaxCompressedSize (same value, same quirk). */
 uint32_t dgb_ans_max_compressed_size(uint32_t uncompressed_bytes);
 /* float/GpuFloatCompress.cu:23-45 getMaxFloatCompressedSize; for DGB_FLOAT64, 16 + the ANS bound + the three
- * planes; for the sparse types, 32 + 4 * roundUp(ceil(n / 4096), 4) + roundUp(n, 16) + the ANS bound.  0 when
- * the bound does not fit 32 bits (encode then returns DGB_ERR_TOO_LARGE). */
+ * planes; for the sparse fp16 / bf16 types, 32 + 4 * roundUp(ceil(n / 4096), 4) + roundUp(n, 16) + the ANS bound;
+ * for DGB_FLOAT32_SPARSE, 32 + 4 * roundUp(ceil(n / 4096), 4) + 2 * roundUp(n, 8) + roundUp(n, 16) + the ANS
+ * bound.  0 when the bound does not fit 32 bits (encode then returns DGB_ERR_TOO_LARGE). */
 uint32_t dgb_float_max_compressed_size(int float_type, uint32_t num_floats);
 
 /* ---- scratch sizing (new; the reference sizes scratch implicitly through

@@ -274,8 +274,8 @@ struct ANSDecodeStatus {
 };
 
 // ---- float/GpuFloatCodec.h:18-97 ----
-// kFloat64, kFloat16Sparse, kBFloat16Sparse: this library's extensions (archives of float types 4, 5 and 6,
-// which the reference cannot read)
+// kFloat64, kFloat16Sparse, kBFloat16Sparse, kFloat32Sparse: this library's extensions (archives of float types
+// 4, 5, 6 and 8, which the reference cannot read)
 enum class FloatType : uint32_t {
   kUndefined = 0,
   kFloat16 = 1,
@@ -283,7 +283,8 @@ enum class FloatType : uint32_t {
   kFloat32 = 3,
   kFloat64 = 4,
   kFloat16Sparse = 5,
-  kBFloat16Sparse = 6
+  kBFloat16Sparse = 6,
+  kFloat32Sparse = 8
 };
 
 inline uint32_t getMaxFloatCompressedSize(FloatType ft, uint32_t size) {

@@ -1,9 +1,10 @@
-"""Sparse fp16 / bf16 archives (float types 5 and 6) against the dense float codec on the same ReLU(N(0,1)) data,
-on one GPU.
+"""Sparse fp16 / bf16 / fp32 archives (float types 5, 6 and 8) against the dense float codec on the same data, on one
+GPU.
 
-    python tools/sparse_bench.py [--iters 30]
+    python tools/sparse_bench.py [--iters 30] [--dtype float32]
 
-Shapes: the c4 shape (256 x 512 Ki fp16) and 64 x 2 Mi bf16.  For each shape, dense and sparse alternate within
+Shapes: the c4 shape (256 x 512 Ki fp16) and 64 x 2 Mi bf16, both ReLU(N(0,1)); with --dtype float32, 64 x 1 Mi and
+256 x 256 Ki fp32 ReLU(N(0,1)) and 64 x 1 Mi fp32 N(0,1) with the 90 % smallest magnitudes of each member set to +0.  For each shape, dense and sparse alternate within
 the run:
   - event-timed encode and decode calls (inputs, archives and scratch preallocated), as time and as uncompressed
     GB/s;
@@ -67,7 +68,8 @@ class Codec:
     def check(self):
         self.decode()
         torch.cuda.synchronize()
-        return all(torch.equal(a.view(torch.int16), b.view(torch.int16)) for a, b in zip(self.ins, self.outs))
+        iv = torch.int32 if self.ins[0].element_size() == 4 else torch.int16
+        return all(torch.equal(a.view(iv), b.view(iv)) for a, b in zip(self.ins, self.outs))
 
 
 def timed(fn, iters):
@@ -104,25 +106,45 @@ def kernel_fractions(c, U, table_bytes):
     return out
 
 
+def workloads(dtype, g):
+    """(label, n x k tensor) pairs"""
+    if dtype == "float32":
+        for n, k in ((64, 1 << 20), (256, 256 * 1024)):
+            yield "relu", torch.randn((n, k), generator=g, device="cuda").relu_()
+        x = torch.randn((64, 1 << 20), generator=g, device="cuda")
+        kth = x.abs().kthvalue(int(0.9 * x.size(1)), dim=1, keepdim=True).values
+        yield "pruned90", x.masked_fill(x.abs() <= kth, 0.0)
+        return
+    yield "relu", torch.randn((256, 512 * 1024), generator=g, device="cuda").relu_().to(torch.float16)
+    yield "relu", torch.randn((64, 2 * 1024 * 1024), generator=g, device="cuda").relu_().to(torch.bfloat16)
+
+
 def main():
+    import sparse32_oracle as S32
     import sparse_oracle as S
 
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
+    ap.add_argument("--dtype", choices=["float16/bfloat16", "float32"], default="float16/bfloat16")
     a = ap.parse_args()
     print("card:", card(), "| library:", capi.LIB_PATH, flush=True)
     g = torch.Generator(device="cuda").manual_seed(1234)
-    for (n, k), dtype in (((256, 512 * 1024), torch.float16), ((64, 2 * 1024 * 1024), torch.bfloat16)):
-        x = torch.randn((n, k), generator=g, device="cuda").relu_().to(dtype)
+    for label, x in workloads(a.dtype, g):
+        n, k = x.shape
+        dtype = x.dtype
         ts = [x[i] for i in range(n)]
-        U = x.numel() * 2
-        ft = S.F16S if dtype == torch.float16 else S.BF16S
+        U = x.numel() * x.element_size()
         table_bytes = n * S.table_bytes(k)
         codecs = {"dense": Codec(False, ts), "sparse": Codec(True, ts)}
         for name, c in codecs.items():
             assert c.check(), f"{name} round trip"
-        host = x.view(torch.int16).cpu().numpy().view(np.uint16)
-        cpu = [S.compress(host[i], ft, 10).size for i in range(n)]
+        if dtype == torch.float32:
+            host = x.view(torch.int32).cpu().numpy().view(np.uint32)
+            cpu = [S32.compress(host[i], 10).size for i in range(n)]
+        else:
+            host = x.view(torch.int16).cpu().numpy().view(np.uint16)
+            ft = S.F16S if dtype == torch.float16 else S.BF16S
+            cpu = [S.compress(host[i], ft, 10).size for i in range(n)]
         assert codecs["sparse"].hs == cpu, "sparse archive sizes differ from the CPU restatement's"
         res = {name: [[], []] for name in codecs}
         for _ in range(3):  # alternate the two codecs
@@ -133,7 +155,8 @@ def main():
             te, td = min(res[name][0]), min(res[name][1])
             kf = " ".join(f"{kk} {us:.1f}us {fr:.2f}" for kk, (us, fr) in kernel_fractions(c, U, table_bytes).items())
             extra = f" (CPU restatement {sum(cpu) / U:.4f})" if name == "sparse" else ""
-            print(f"{n}x{k} {str(dtype).split('.')[1]} {name:6s} ratio {c.archive_bytes / U:.4f}{extra} | "
+            tag = f" {label}" if dtype == torch.float32 else ""  # the fp16 / bf16 lines keep their format
+            print(f"{n}x{k} {str(dtype).split('.')[1]}{tag} {name:6s} ratio {c.archive_bytes / U:.4f}{extra} | "
                   f"enc {te:.1f}us {U / te / 1e3:.0f} GB/s (runs {' '.join(f'{t:.1f}' for t in res[name][0])}) | "
                   f"dec {td:.1f}us {U / td / 1e3:.0f} GB/s (runs {' '.join(f'{t:.1f}' for t in res[name][1])}) | "
                   f"kernels (us, share of 3.35 TB/s): {kf}", flush=True)
