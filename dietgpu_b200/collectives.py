@@ -3,6 +3,8 @@ README.md:72, 103-104; SURVEY.md section 8f rank 3) and ships no code for.
 
     all_gather_compressed(t)       every rank contributes t, every rank receives the concatenation
     all_to_all_compressed(chunks)  rank r sends chunks[d] to rank d and receives one chunk from every rank
+    reduce_scatter_compressed(t)   rank r receives the elementwise sum over ranks of chunk r of t
+    all_reduce_compressed(t)       every rank receives the elementwise sum over ranks of t
 
 Each rank compresses what it sends, the ranks exchange the variable-size archives, every rank
 decompresses what it received.  The wire carries about `ratio` x the raw bytes (0.67 for bf16
@@ -417,6 +419,19 @@ def _all_to_all_peer(flats: List[torch.Tensor], as_float: bool, ws: PeerWorkspac
     return outs
 
 
+def _all_to_all_bytes(send: torch.Tensor, send_sizes: List[int], recv_sizes: List[int], group,
+                      on_device: bool) -> torch.Tensor:
+    """all_to_all_single of a packed uint8 buffer on send's device; staged through host memory where the
+    backend has no device collectives."""
+    if on_device:
+        recv = torch.empty(sum(recv_sizes), dtype=torch.uint8, device=send.device)
+        dist.all_to_all_single(recv, send, recv_sizes, send_sizes, group=group)
+        return recv
+    host = torch.empty(sum(recv_sizes), dtype=torch.uint8)
+    dist.all_to_all_single(host, send.cpu(), recv_sizes, send_sizes, group=group)
+    return host.to(send.device)
+
+
 def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, peer: Optional[PeerWorkspace] = None,
                           check: bool = True, peer_mode: str = "pull") -> List[torch.Tensor]:
@@ -456,13 +471,7 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
         k = int(meta_out[d, 0])
         send[o:o + k].copy_(comp[d, :k])
         o += send_sizes[d]
-    if on_device:
-        recv = torch.empty(sum(recv_sizes), dtype=torch.uint8, device=dev)
-        dist.all_to_all_single(recv, send, recv_sizes, send_sizes, group=group)
-    else:
-        host = torch.empty(sum(recv_sizes), dtype=torch.uint8)
-        dist.all_to_all_single(host, send.cpu(), recv_sizes, send_sizes, group=group)
-        recv = host.to(dev)
+    recv = _all_to_all_bytes(send, send_sizes, recv_sizes, group, on_device)
     ins, outs, o = [], [], 0
     for s in range(world):
         k, elems = int(recv_meta[s][0]), int(recv_meta[s][1])
@@ -474,3 +483,106 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
     if not bool(status.all()):
         raise RuntimeError("all_to_all_compressed: a received archive failed to decode")
     return [x if as_float else x.view(dt) for x in outs]
+
+
+_REDUCE_DTYPES = (torch.float16, torch.bfloat16, torch.float32)
+
+
+def _check_reducible(t: torch.Tensor, what: str) -> None:
+    if not t.is_cuda or not t.is_contiguous():
+        raise ValueError(f"{what}: contiguous CUDA tensor expected (no CPU fallback)")
+    if t.dtype not in _REDUCE_DTYPES:
+        raise ValueError(f"{what}: float16, bfloat16 or float32 tensor expected, not {t.dtype}")
+
+
+def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
+                              temp_mem: Optional[torch.Tensor] = None, check: bool = True) -> torch.Tensor:
+    """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
+    world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
+    ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
+    rank), so the wire carries compressed bytes; the receiver decodes and sums them in one kernel
+    (ops.decompress_data_reduce) without a decoded temporary per source.  The sum is the left fold over ranks in
+    rank order, with torch's adds in t's dtype, for every element on every rank: the result is bit-identical to
+    ((t_0 + t_1) + t_2) + ... whatever `members` and the backend.  `check` raises RuntimeError when a received
+    archive fails to decode."""
+    _check_reducible(t, "reduce_scatter_compressed")
+    world = _world(group)
+    flat = t.reshape(-1)
+    n = flat.numel()
+    if n % world:
+        raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
+    if world == 1 or n == 0:
+        return flat[: n // world].clone()
+    rank, dev = dist.get_rank(group), t.device
+    shard = n // world
+    bounds = _split(shard, max(1, int(members)), 8)
+    m = len(bounds) - 1
+    dests = [d for d in range(world) if d != rank]
+    comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
+                                              for d in dests for i in range(m)], False, temp_mem)
+    on_device = _device_collectives(group)
+    cdev = dev if on_device else torch.device("cpu")
+    hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
+    meta_out = torch.zeros(world, m, dtype=torch.int64)
+    for k, d in enumerate(dests):
+        meta_out[d] = torch.tensor(hs[k * m:(k + 1) * m], dtype=torch.int64)
+    meta_in = torch.empty_like(meta_out, device=cdev)
+    dist.all_to_all_single(meta_in, meta_out.to(cdev), group=group)
+    recv_meta = meta_in.cpu().tolist()
+    send_sizes = [sum(_round_up(int(v), _ALIGN) for v in row) for row in meta_out.tolist()]
+    recv_sizes = [sum(_round_up(int(v), _ALIGN) for v in row) for row in recv_meta]
+    send = torch.zeros(sum(send_sizes), dtype=torch.uint8, device=dev)
+    o = 0
+    for k, d in enumerate(dests):
+        for i in range(m):
+            a = hs[k * m + i]
+            send[o:o + a].copy_(comp[k * m + i, :a])
+            o += _round_up(a, _ALIGN)
+    recv = _all_to_all_bytes(send, send_sizes, recv_sizes, group, on_device)
+    archives = []  # archives[s][i]: member i of the chunk source s sent here
+    o = 0
+    for s in range(world):
+        row = []
+        for a in recv_meta[s]:
+            row.append(recv[o:o + int(a)])
+            o += _round_up(int(a), _ALIGN)
+        archives.append(row)
+    out = torch.empty(shard, dtype=t.dtype, device=dev)
+    outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
+    own = flat[rank * shard:(rank + 1) * shard]
+    statuses = []
+    # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add), + r+1..world-1
+    if rank == 0:
+        out.copy_(own)
+    else:
+        st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st)
+        statuses.append(st)
+        out.add_(own)
+    if rank + 1 < world:
+        st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
+                                   temp_mem, st)
+        statuses.append(st)
+    if check and not all(bool(st.all()) for st in statuses):
+        raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
+    return out
+
+
+def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
+                          check: bool = True) -> torch.Tensor:
+    """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
+    returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
+    t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
+    for the exchange.  Bit-identical on every rank to the rank-order left fold with torch's adds."""
+    _check_reducible(t, "all_reduce_compressed")
+    world = _world(group)
+    flat = t.reshape(-1)
+    n = flat.numel()
+    if world == 1 or n == 0:
+        return t.clone()
+    per = _round_up(-(-n // world), 8)
+    src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
+    shard = reduce_scatter_compressed(src, group, members, temp_mem, check)
+    full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check)
+    return full[:n].view(t.shape)

@@ -513,6 +513,13 @@ int dgb_float_decompress_split_size(void* temp, size_t tempBytes, int ft, int pb
                            outSuccess_dev, outSize_dev, mismatchHost, stream);
 }
 
+int dgb_float_decompress_reduce(void* temp, size_t tempBytes, int ft, int pb, uint32_t numGroups,
+                                uint32_t archivesPerGroup, const void* const* in, void* const* out,
+                                const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
+  return decodeReduce(ft, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
+                      outSuccess_dev, (cudaStream_t)stream);
+}
+
 // ---- info ------------------------------------------------------------------
 
 int dgb_ans_get_compressed_info(void* temp, size_t tempBytes, const void* const* in,

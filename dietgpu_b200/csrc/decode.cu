@@ -1140,6 +1140,292 @@ int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineM
   return DGB_OK;
 }
 
+// ---------------------------------------------------------------------------
+// Decode-and-sum (dgb_float_decompress_reduce, no reference counterpart).  G groups of W archives of one dense
+// fp16 / bf16 / fp32 kind; out[g] = (accumulate ? out[g] : x(g,0)) + x(g,1) + ... + x(g,W-1), left to right, each
+// add one IEEE round-to-nearest-even add in the element type with subnormals kept.  A CTA leases a GROUP (the
+// single-launch decoder's lease / claim / seen pattern over groups), checks the headers of all W archives, builds
+// one LUT per archive of the current pass, and each warp claims a 4 KiB block index k and decodes block k of
+// every archive of the pass in archive order.  Lane l owns the same elements of block k in every archive, so
+// its running sums are its own earlier stores (program order, no atomics, no cross-lane traffic), and the sum
+// order per element is fixed whatever the grid, the claims or the passes: the result is bit-reproducible.
+// The first archive of an accumulate=0 call is stored verbatim (the ordinary writer); every later one goes
+// through an add writer that loads the 16 running sums of a row group when the group starts (once per group
+// instead of once per row on the decode loop), adds, and stores.
+// LUTs cost shared memory, so at most kReducePass archives are decoded per launch; the host issues
+// ceil(W / kReducePass) launches in order and every launch after the first accumulates (DESIGN.md section 3).
+// ---------------------------------------------------------------------------
+#ifndef DGB_REDUCE_PASS_ARCHIVES
+#define DGB_REDUCE_PASS_ARCHIVES 4
+#endif
+constexpr uint32_t kReducePass = DGB_REDUCE_PASS_ARCHIVES;
+constexpr int kReduceWarps = 8;
+// writer kinds of the decode-and-sum: the dense kind | kAddWriter adds the decoded word to the output's word
+constexpr int kAddWriter = 0x10;
+
+template <int KIND>
+__device__ __forceinline__ uint32_t addWord(uint32_t a, uint32_t b) {
+  if constexpr (KIND == kKindF32) {
+    return __float_as_uint(__fadd_rn(__uint_as_float(a), __uint_as_float(b)));
+  } else {
+    unsigned short r;
+    if constexpr (KIND == kKindF16)
+      asm("add.rn.f16 %0, %1, %2;" : "=h"(r) : "h"((unsigned short)a), "h"((unsigned short)b));
+    else
+      asm("add.rn.bf16 %0, %1, %2;" : "=h"(r) : "h"((unsigned short)a), "h"((unsigned short)b));
+    return r;
+  }
+}
+// running-sum loads of a row group, volatile so that they are issued when the group starts
+__device__ __forceinline__ uint32_t ldGlobalU16(const uint16_t* p) {
+  uint32_t v;
+  asm volatile("ld.global.u16 %0, [%1];" : "=r"(v) : "l"(__cvta_generic_to_global(p)));
+  return v;
+}
+__device__ __forceinline__ uint32_t ldGlobalU32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.global.u32 %0, [%1];" : "=r"(v) : "l"(__cvta_generic_to_global(p)));
+  return v;
+}
+
+template <int KIND>
+struct RowWriterAdd16 : RowWriter16<KIND> {
+  typedef RowWriter16<KIND> B;
+  struct Cursor { uint16_t* o; uint32_t s; uint32_t prev[kGroupRows]; };
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    Cursor c;
+    c.o = B::out + row * 32u;
+    c.s = B::ring + slot * B::kRingSlotBytes + B::lane;
+#pragma unroll
+    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU16(c.o + j * 32);
+    return c;
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)addWord<KIND>(c.prev[J], B::join(entry, ldsU8<J * 32>(c.s)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint16_t* o = B::out + row * 32u;
+    *o = (uint16_t)addWord<KIND>(*o, B::join(entry, __ldg(B::non + row * 32u)));
+  }
+};
+template <> struct RowWriter<kKindF16 | kAddWriter> : RowWriterAdd16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kAddWriter> : RowWriterAdd16<kKindBF16> {};
+
+template <>
+struct RowWriter<kKindF32 | kAddWriter> : RowWriter<kKindF32> {
+  typedef RowWriter<kKindF32> B;
+  struct Cursor { uint32_t* o; uint32_t s2, s1; uint32_t prev[kGroupRows]; };
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    const typename B::Cursor b = B::at(row, slot);
+    Cursor c;
+    c.o = b.o;
+    c.s2 = b.s2;
+    c.s1 = b.s1;
+#pragma unroll
+    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU32(c.o + j * 32);
+    return c;
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = addWord<kKindF32>(c.prev[J], join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = out + row * 32u;
+    *o = addWord<kKindF32>(*o, join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)));
+  }
+};
+
+// An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
+// consistent with its word count, and that word count is the group's output size.
+template <int KIND, int PB>
+__device__ __forceinline__ bool reduceArchiveOk(const void* in, uint32_t words) {
+  const ArchiveView av = openArchive<KIND>(static_cast<const uint8_t*>(in));
+  if (!av.ok || av.floatWords != words) return false;
+  const uint4 h0 = __ldg(reinterpret_cast<const uint4*>(av.ans));
+  const uint4 h1 = __ldg(reinterpret_cast<const uint4*>(av.ans) + 1);
+  return h0.x == kAnsMagicVersion && (int)(h1.x & 0xfu) == PB && h0.z == words && h0.y == divUp(words, kBlockBytes);
+}
+
+// block `block` of one archive through writer kind WK (the single-launch decoder's block body)
+template <int WK, int PB>
+__device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, uint32_t block, uint32_t nb,
+                                                  const typename Lut<PB, false>::Entry* __restrict__ lut,
+                                                  uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
+                                                  uint32_t slotWords, uint32_t lane) {
+  const ArchiveView av = openArchive<WK & ~kAddWriter>(in);
+  const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
+  const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
+  const uint16_t* pData = reinterpret_cast<const uint16_t*>(
+      reinterpret_cast<const uint8_t*>(pBlockWords) + 8u * (size_t)roundUp(nb, 2u));
+  RowWriter<WK> wr;
+  wr.setRing(ring, lane);
+  wr.setBlock(av, out, block, lane);
+  const uint2 bw = __ldg(pBlockWords + block);
+  const uint32_t blockLen = bw.x >> 16, words = bw.x & 0xffffu;
+  const uint16_t* stream = pData + bw.y;
+  if ((reinterpret_cast<uintptr_t>(av.ans) & 15u) == 0 && words <= slotWords && (bw.y & 7u) == 0u) {
+    const uint32_t streamBytes = roundUp(words, 8u) * 2u;
+    __syncwarp();
+    if (lane == 0) {
+      mbarExpectTx(myBar, 128u + streamBytes);
+      bulkLoad(smemAddr(mySlot), pStates + 128u * (size_t)block, 128u, myBar);
+      if (streamBytes) bulkLoad(smemAddr(mySlot + 128), stream, streamBytes, myBar);
+    }
+    mbarWait(myBar, phase);
+    phase ^= 1u;
+    const uint32_t state = reinterpret_cast<const uint32_t*>(mySlot)[lane];
+    SmemStream st{smemAddr(mySlot + 128) + 2u * words};
+    decodeBlockWarp<WK, PB, false>(state, st, blockLen, lut, wr, lane);
+  } else {
+    const uint32_t state = __ldg(reinterpret_cast<const uint32_t*>(pStates) + block * 32u + lane);
+    GmemStream st{stream + words};
+    decodeBlockWarp<WK, PB, false>(state, st, blockLen, lut, wr, lane);
+  }
+}
+
+// One pass: archives [a0, a1) of every group.  Member table entry g * width + j = {archive (g, j), out[g],
+// out_size[g], block cap of group g}.  addFirst: archive a0 adds too (accumulate, or a later pass).  Only the
+// first pass (a0 == 0) reports outSuccess.
+template <int KIND, int PB>
+__global__ void __launch_bounds__(kReduceWarps * 32, 4)
+decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
+                   uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
+  constexpr int WARPS = kReduceWarps;
+  extern __shared__ __align__(128) uint8_t smem[];
+  constexpr uint32_t K = 1u << PB;
+  typedef typename Lut<PB, false>::Entry Entry;
+  static_assert(kReducePass * K * sizeof(Entry) <= 40 * 1024, "the pass's LUTs must fit static shared memory");
+  __shared__ __align__(16) Entry lut[kReducePass][K];
+  uint32_t* sPdf = reinterpret_cast<uint32_t*>(smem);
+  uint32_t* sCdf = sPdf + kNumSymbols;
+  uint32_t* sWarp = sCdf + kNumSymbols;
+  uint32_t* sMisc = sWarp + 32;
+  unsigned long long* sBar = reinterpret_cast<unsigned long long*>(sMisc + 32);
+  uint8_t* sRing = reinterpret_cast<uint8_t*>(sBar + ((WARPS + 1) & ~1));
+  constexpr uint32_t ringBytes = kRingSlots * RowWriter<KIND>::kRingSlotBytes;
+  static_assert(RowWriter<KIND | kAddWriter>::kRingSlotBytes == RowWriter<KIND>::kRingSlotBytes, "");
+  uint8_t* sSlots = sRing + WARPS * ringBytes;
+  const uint32_t slotBytes = 128u + slotWords * 2u;
+
+  const uint32_t t = threadIdx.x, lane = t & 31u;
+  const uint32_t warp = __shfl_sync(0xffffffffu, t >> 5, 0);
+  uint8_t* mySlot = sSlots + (size_t)warp * slotBytes;
+  const uint32_t myBar = smemAddr(sBar + warp);
+  const uint32_t ring = smemAddr(sRing + warp * ringBytes);
+  uint32_t phase = 0;
+  if (lane == 0) mbarInit(myBar, 1);
+  fenceBarrierInit();
+  __syncthreads();
+
+  uint32_t cursor = (uint32_t)((uint64_t)blockIdx.x * groups / gridDim.x);
+  for (;;) {
+    // ---- lease a group (decodeFusedKernel's lease over groups); the first CTA to lease it reports its status ----
+    if (warp == 0) {
+      uint32_t pick = kNoMember, firstBlock = 0, tries = 0;
+      while (tries < groups) {
+        uint32_t gg = cursor + lane;
+        if (gg >= groups) gg -= groups;
+        bool has = false;
+        if (tries + lane < groups)
+          has = *reinterpret_cast<volatile uint32_t*>(sc.next + gg) < memberWork0(im, sc.members, gg * width);
+        const uint32_t mask = __ballot_sync(0xffffffffu, has);
+        if (mask == 0u) {
+          tries += 32u;
+          cursor = (cursor + 32u) % groups;
+          continue;
+        }
+        const uint32_t first = (uint32_t)__ffs((int)mask) - 1u;
+        uint32_t cand = cursor + first;
+        if (cand >= groups) cand -= groups;
+        uint32_t c = 0;
+        if (lane == 0) c = atomicAdd(sc.next + cand, 1u);
+        c = __shfl_sync(0xffffffffu, c, 0);
+        if (c < memberWork0(im, sc.members, cand * width)) {
+          pick = cand;
+          firstBlock = c;
+          cursor = cand;
+          break;
+        }
+        tries += first + 1u;
+        cursor = cand + 1 == groups ? 0u : cand + 1;
+      }
+      if (lane == 0) {
+        sMisc[0] = pick;
+        sMisc[1] = firstBlock;
+        sMisc[2] = pick != kNoMember && a0 == 0 && outSuccess && atomicExch(sc.seen + pick, 1u) == 0u;
+      }
+    }
+    __syncthreads();
+    const uint32_t g = sMisc[0];
+    if (g == kNoMember) break;
+    const bool report = sMisc[2] != 0;
+    const MemberDesc gd = memberAt(im, sc.members, g * width);
+    const uint32_t blocksCap = gd.work0, nb = divUp(gd.size, kBlockBytes);
+
+    // ---- every archive of the group is checked before anything is stored to it: the decision depends on the
+    //      headers and out_size alone, so every CTA and every pass takes the same one ----
+    bool ok = true;
+    for (uint32_t j = t; j < width; j += WARPS * 32) {
+      const bool v = reduceArchiveOk<KIND, PB>(memberAt(im, sc.members, g * width + j).in, gd.size);
+      if (report) outSuccess[g * width + j] = v ? 1 : 0;
+      ok = ok && v;
+    }
+    const bool work = __syncthreads_and(ok) && nb > 0;
+    if (work) {
+      for (uint32_t a = a0; a < a1; ++a)
+        buildLut<PB, false, WARPS>(openArchive<KIND>(static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in)).ans,
+                                   lut[a - a0], sPdf, sCdf, sWarp);
+    }
+
+    // ---- every warp claims block indices of the group until none are left; block k of every archive ----
+    uint32_t block = sMisc[1];
+    if (warp != 0) {
+      if (lane == 0) block = atomicAdd(sc.next + g, 1u);
+      block = __shfl_sync(0xffffffffu, block, 0);
+    }
+    while (block < blocksCap) {
+      uint32_t nextBlock = 0;
+      if (lane == 0) nextBlock = atomicAdd(sc.next + g, 1u);
+      if (work && block < nb) {
+        for (uint32_t a = a0; a < a1; ++a) {
+          const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
+          if (a == a0 && !addFirst)
+            decodeReduceBlock<KIND, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane);
+          else
+            decodeReduceBlock<KIND | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring, mySlot, myBar, phase,
+                                                     slotWords, lane);
+        }
+      }
+      block = __shfl_sync(0xffffffffu, nextBlock, 0);
+    }
+    __syncthreads();  // every warp is done with the LUTs (and sMisc) before the next lease
+  }
+}
+
+template <int KIND, int PB>
+int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
+                       uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream) {
+  auto kern = decodeReduceKernel<KIND, PB>;
+  uint32_t slotWords;
+  const size_t smemBytes = decoderSmem<KIND, PB>(kReduceWarps, opt, &slotWords);
+  int perSm = 1;
+  const int rc = residentCtasPerSm((const void*)kern, kReduceWarps * 32, smemBytes, 160 * 1024, &perSm);
+  if (rc != DGB_OK) return rc;
+  const uint64_t resident = (uint64_t)perSm * smCount();
+  const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(resident, totalChunks));
+  for (uint32_t a0 = 0; a0 < width; a0 += kReducePass) {
+    // claim counters and `seen` start at zero in every pass
+    DGB_CUDA_TRY(cudaMemsetAsync(sc.next, 0, 8 * (size_t)groups * width, stream));
+    timerBegin(opt, kSlotDecode, stream);
+    kern<<<grid, kReduceWarps * 32, smemBytes, stream>>>(sc, im, groups, width, a0, std::min(width, a0 + kReducePass),
+                                                         accumulate || a0 > 0, slotWords, outSuccess);
+    DGB_CUDA_TRY(cudaGetLastError());
+    timerEnd(opt, kSlotDecode, stream);
+  }
+  return DGB_OK;
+}
+
 }  // namespace
 
 size_t decodeTempBytes(int /*kind*/, uint32_t n) { return planDecodeScratch(n).total + 256; }
@@ -1275,6 +1561,61 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     if (bad) return DGB_ERR_CHECKSUM;
   }
   return DGB_OK;
+}
+
+int decodeReduce(int kind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
+                 const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
+                 uint8_t* outSuccess_dev, cudaStream_t stream) {
+  if (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32) return DGB_ERR_INVALID_ARG;
+  if (pb < 9 || pb > 11 || width == 0) return DGB_ERR_INVALID_ARG;
+  if (groups == 0) return DGB_OK;
+  if (!in || !out || !outSize) return DGB_ERR_INVALID_ARG;
+  const uint64_t n64 = (uint64_t)groups * width;
+  if (n64 > 0xffffffffull) return DGB_ERR_INVALID_ARG;
+  const uint32_t n = (uint32_t)n64;
+  const DecodePlan dp = planDecodeScratch(n);
+  if (!temp || tempBytes < dp.total) return DGB_ERR_TEMP_TOO_SMALL;
+  if (reinterpret_cast<uintptr_t>(temp) & 255u) return DGB_ERR_INVALID_ARG;
+
+  const Options opt = options();  // one snapshot per call
+  HostStage& hs = hostStage();
+  hs.decodeTable.resize(n);
+  MemberDesc* desc = hs.decodeTable.data();
+  const uint32_t elemBytes = wordBytes(kind);
+  uint64_t totalChunks = 0;
+  for (uint32_t g = 0; g < groups; ++g) {
+    if ((outSize[g] && !out[g]) || (reinterpret_cast<uintptr_t>(out[g]) & (elemBytes - 1u))) return DGB_ERR_INVALID_ARG;
+    // block cap >= 1: every group's headers are visited, so its status is reported
+    const uint32_t blocks = std::max(1u, divUp(outSize[g], kBlockBytes));
+    totalChunks += divUp(blocks, 8u);
+    for (uint32_t j = 0; j < width; ++j) {
+      const void* a = in[(size_t)g * width + j];
+      if (!a || (reinterpret_cast<uintptr_t>(a) & 15u)) return DGB_ERR_INVALID_ARG;
+      desc[(size_t)g * width + j] = MemberDesc{a, out[g], outSize[g], blocks};
+    }
+  }
+  uint8_t* base = static_cast<uint8_t*>(temp);
+  DecodeScratch sc{};
+  sc.members = reinterpret_cast<MemberDesc*>(base + dp.members);
+  sc.next = reinterpret_cast<uint32_t*>(base + dp.next);
+  sc.seen = sc.next + n;
+  static thread_local InlineMembers im;
+  const bool inlined = opt.inline_members != 0 && n <= kInlineMembers;
+  im.count = inlined ? n : 0u;
+  if (inlined) {
+    std::memcpy(im.m, desc, sizeof(MemberDesc) * n);
+  } else {
+    const int rc = uploadTable(sc.members, desc, sizeof(MemberDesc) * n, stream);
+    if (rc != DGB_OK) return rc;
+  }
+  return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
+    constexpr int KIND = decltype(K)::value;
+    if constexpr (KIND == kKindF16 || KIND == kKindBF16 || KIND == kKindF32)
+      return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
+                                                         outSuccess_dev, stream);
+    else
+      return (int)DGB_ERR_INVALID_ARG;  // not reached (checked above)
+  }); });
 }
 
 // ---------------------------------------------------------------------------

@@ -345,6 +345,52 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
     return tmp.need
 
 
+_REDUCE_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32}
+
+
+def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequence[torch.Tensor],
+                           accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
+                           out_status: Optional[torch.Tensor] = None, *,
+                           prob_bits: int = K_DEFAULT_PRECISION) -> int:
+    """Decode-and-sum (dgb_float_decompress_reduce): ts_in is G lists of W uint8 float archives each, ts_out G
+    contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
+    (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
+    that dtype, where x(g, j) is archive ts_in[g][j] decoded; each archive must hold exactly ts_out[g].numel()
+    words.  A group with an invalid archive is left untouched; out_status (CUDA uint8, G * W entries, group-major)
+    receives 1 / 0 per archive.  Returns the scratch bytes used."""
+    _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
+    width = len(ts_in[0])
+    _check(width > 0, "a group needs at least one archive")
+    dtype = ts_out[0].dtype
+    if dtype not in _REDUCE_TYPES:
+        raise ValueError(f"decompress_data_reduce sums float16, bfloat16 or float32 outputs, not {dtype}")
+    dev = ts_out[0].device
+    ins = []
+    for group, to in zip(ts_in, ts_out):
+        _check(len(group) == width, "every group needs the same number of archives")
+        _check(to.is_cuda and to.device == dev and to.is_contiguous() and to.dtype == dtype,
+               "outputs must be contiguous CUDA tensors of one dtype on one device")
+        _check(to.numel() <= 0xFFFFFFFF)
+        for ti in group:
+            _check(ti.is_cuda and ti.device == dev and ti.is_contiguous() and ti.dtype == torch.uint8)
+            _check_archive_aligned(ti)
+            ins.append(ti)
+    g, n = len(ts_out), len(ins)
+    st_ptr, _ = _validate_status(out_status, None, n, dev)
+    ft = _REDUCE_TYPES[dtype]
+    L = capi.lib()
+    with torch.cuda.device(dev):
+        need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
+        tmp = _Temp(temp_mem, need, dev)
+        rc = L.dgb_float_decompress_reduce(tmp.ptr, tmp.bytes, ft, prob_bits, g, width,
+                                           capi.ptr_array([t.data_ptr() for t in ins]),
+                                           capi.ptr_array([t.data_ptr() for t in ts_out]),
+                                           capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
+                                           st_ptr, _stream())
+    capi.check(rc, "decompress_data_reduce")
+    return tmp.need
+
+
 def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Tensor], t_out: torch.Tensor,
                                t_out_split_sizes: torch.Tensor, checksum: bool = False,
                                temp_mem: Optional[torch.Tensor] = None,

@@ -198,6 +198,23 @@ int dgb_float_decompress_split_size(void* temp_dev, size_t temp_bytes, int float
                                     uint32_t* out_size_dev, uint8_t* checksum_mismatch_host,
                                     void* stream);
 
+/* Decode-and-sum (new; no reference counterpart): out[g] = (accumulate ? out[g] : x(g,0)) + x(g,1) + ... +
+ * x(g,W-1) in archive order, where x(g,j) is the decoded content of archive (g, j) = in[g * W + j] and each + is
+ * one IEEE-754 round-to-nearest-even addition in the element type, subnormals kept (for fp16 / bf16 the same
+ * result as torch's a + b).  Without accumulate and with W = 1 this is a plain decode (NaN payloads and -0 kept).
+ * float_type: DGB_FLOAT16, DGB_BFLOAT16 or DGB_FLOAT32 (else DGB_ERR_INVALID_ARG).  in: host array of G * W
+ * device pointers (16 B aligned), group-major; out / out_size: host arrays of G (out_size in words, outputs
+ * aligned to the word size; outputs must not overlap each other or any archive).  An archive is valid when its
+ * headers have float_type and prob_bits, a consistent block count and exactly out_size[g] words;
+ * out_success_dev (optional, device u8[G * W]) receives 1 or 0 per archive, and a group with an invalid archive
+ * is not written at all.  Stored checksums are not verified.  num_groups = 0 returns DGB_OK and does nothing.
+ * Never synchronises; capturable into a CUDA graph.  Scratch: dgb_float_decompress_temp_bytes(float_type,
+ * G * W, 0). */
+int dgb_float_decompress_reduce(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
+                                uint32_t num_groups, uint32_t archives_per_group, const void* const* in,
+                                void* const* out, const uint32_t* out_size, int accumulate,
+                                uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

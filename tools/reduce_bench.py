@@ -1,0 +1,137 @@
+"""Decode-and-sum (ops.decompress_data_reduce) against decoding the same archives separately, on one GPU.
+
+    python tools/reduce_bench.py [--iters 30] [--json out.json]
+
+For each shape (G groups x W archives x N words of N(0,1) data, seeded) three ways are timed on the same archives,
+alternating within the run:
+  (1) decompress_data_reduce: one call, every group summed;
+  (2) decompress_data of the G * W archives into separate outputs;
+  (3) (2) followed by the W - 1 torch adds per group (what a caller does without (1)).
+Reported: event time per call, the decoder's kernel time with option timing=1 (slot "decode"), and for (1) and (2)
+algorithmic bytes over kernel time as a share of the H100 SXM data sheet's 3.35 TB/s HBM3 bandwidth (archives read
+once + outputs written once: G * N words for (1), G * W * N for (2)).  (1)'s result is checked bit for bit against
+(3)'s.  The card name and power limit are read in the same run; DIETGPU_B200_LIB selects an experiment build of
+the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_ARCHIVES=2).
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+
+from dietgpu_b200 import capi, ops  # noqa: E402
+
+PEAK_GBS = 3350.0  # H100 SXM data sheet, HBM3
+SHAPES = [  # (dtype, groups, archives per group, words)
+    (torch.bfloat16, 8, 8, 2 << 20),
+    (torch.bfloat16, 8, 7, 4 << 20),  # what one rank of an 8-GPU reduce-scatter of 256 Mi words receives
+    (torch.float32, 16, 4, 1 << 20),
+    (torch.float16, 64, 2, 512 << 10),
+]
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = "power limit unknown"
+    return f"{name} ({q})"
+
+
+def timed(fn, iters):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(iters):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / iters * 1e3  # us
+
+
+def kernel_us(fn, iters):
+    capi.set_option("timing", 1)
+    try:
+        capi.kernel_times()
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+        ms, _ = capi.kernel_times()["decode"]
+    finally:
+        capi.set_option("timing", 0)
+    return ms / iters * 1e3
+
+
+def bench(dtype, groups, width, n, iters):
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [torch.randn(n, generator=g, device="cuda").to(dtype) for _ in range(groups * width)]
+    comp, sizes, _ = ops.compress_data(True, xs)
+    hs = sizes.cpu().tolist()
+    arch = [comp[i, :hs[i]] for i in range(len(xs))]
+    del xs
+    groups_in = [arch[k * width:(k + 1) * width] for k in range(groups)]
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    red = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups)]
+    sep = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups * width)]
+    fold = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups)]
+
+    def one():
+        ops.decompress_data_reduce(groups_in, red, False, temp)
+
+    def two():
+        ops.decompress_data(True, arch, sep, False, temp)
+
+    def three():
+        two()
+        for k in range(groups):
+            torch.add(sep[k * width], sep[k * width + 1], out=fold[k]) if width > 1 else fold[k].copy_(sep[k * width])
+            for j in range(2, width):
+                fold[k].add_(sep[k * width + j])
+
+    for f in (one, two, three):  # warm-up
+        f()
+    torch.cuda.synchronize()
+    for k in range(groups):
+        assert torch.equal(red[k].view(torch.int16 if dtype != torch.float32 else torch.int32),
+                           fold[k].view(torch.int16 if dtype != torch.float32 else torch.int32)), k
+    t = {"1": [], "2": [], "3": []}
+    for _ in range(3):  # alternate
+        t["1"].append(timed(one, iters))
+        t["2"].append(timed(two, iters))
+        t["3"].append(timed(three, iters))
+    k1, k2 = kernel_us(one, iters), kernel_us(two, iters)
+    es = torch.empty(0, dtype=dtype).element_size()
+    abytes = sum(hs)
+    bw1 = (abytes + groups * n * es) / (k1 * 1e-6) / 1e9
+    bw2 = (abytes + groups * width * n * es) / (k2 * 1e-6) / 1e9
+    r = {"shape": f"{str(dtype).split('.')[-1]} {groups}x{width}x{n}", "archive_MB": abytes / 1e6,
+         "call_us": {k: min(v) for k, v in t.items()}, "call_us_max": {k: max(v) for k, v in t.items()},
+         "kernel_us": {"1": k1, "2": k2}, "hbm_share": {"1": bw1 / PEAK_GBS, "2": bw2 / PEAK_GBS}}
+    r["1_over_3"] = r["call_us"]["1"] / r["call_us"]["3"]
+    r["1_over_2"] = r["call_us"]["1"] / r["call_us"]["2"]
+    return r
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=30)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
+    print(info["card"], flush=True)
+    for shape in SHAPES:
+        r = bench(*shape, args.iters)
+        info["results"].append(r)
+        print(json.dumps(r), flush=True)
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(info, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
