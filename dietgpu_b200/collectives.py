@@ -488,15 +488,23 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
 _REDUCE_DTYPES = (torch.float16, torch.bfloat16, torch.float32)
 
 
-def _check_reducible(t: torch.Tensor, what: str) -> None:
+def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dtype]) -> torch.dtype:
+    """The dtype the sum is taken in: t's, or float32 for a float16 / bfloat16 t with reduce_dtype=float32."""
     if not t.is_cuda or not t.is_contiguous():
         raise ValueError(f"{what}: contiguous CUDA tensor expected (no CPU fallback)")
     if t.dtype not in _REDUCE_DTYPES:
         raise ValueError(f"{what}: float16, bfloat16 or float32 tensor expected, not {t.dtype}")
+    if reduce_dtype is None or reduce_dtype == t.dtype:
+        return t.dtype
+    if reduce_dtype == torch.float32 and t.dtype in (torch.float16, torch.bfloat16):
+        return reduce_dtype
+    raise ValueError(f"{what}: reduce_dtype is None, t.dtype or float32 for a float16 / bfloat16 tensor, "
+                     f"not {reduce_dtype} for {t.dtype}")
 
 
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
-                              temp_mem: Optional[torch.Tensor] = None, check: bool = True) -> torch.Tensor:
+                              temp_mem: Optional[torch.Tensor] = None, check: bool = True,
+                              reduce_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -504,15 +512,20 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     (ops.decompress_data_reduce) without a decoded temporary per source.  The sum is the left fold over ranks in
     rank order, with torch's adds in t's dtype, for every element on every rank: the result is bit-identical to
     ((t_0 + t_1) + t_2) + ... whatever `members` and the backend.  `check` raises RuntimeError when a received
-    archive fails to decode."""
-    _check_reducible(t, "reduce_scatter_compressed")
+    archive fails to decode.
+
+    reduce_dtype=torch.float32 with a float16 / bfloat16 t (mixed-precision gradients summed in fp32): the wire
+    still carries the 16-bit archives, the result is float32 and equals the fp32 fold
+    ((t_0.float() + t_1.float()) + t_2.float()) + ... bit for bit.  None or t.dtype sums in t's dtype; any other
+    value raises ValueError."""
+    acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     world = _world(group)
     flat = t.reshape(-1)
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
     if world == 1 or n == 0:
-        return flat[: n // world].clone()
+        return flat[: n // world].to(acc_dtype, copy=True)
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
@@ -547,22 +560,24 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
             row.append(recv[o:o + int(a)])
             o += _round_up(int(a), _ALIGN)
         archives.append(row)
-    out = torch.empty(shard, dtype=t.dtype, device=dev)
+    out = torch.empty(shard, dtype=acc_dtype, device=dev)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
     own = flat[rank * shard:(rank + 1) * shard]
     statuses = []
-    # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add), + r+1..world-1
+    # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add; fp32 += fp16 /
+    # bf16 is the same fp32 add of the widened word), + r+1..world-1
     if rank == 0:
         out.copy_(own)
     else:
         st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
-        ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
+                                   archive_dtype=t.dtype)
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st)
+                                   temp_mem, st, archive_dtype=t.dtype)
         statuses.append(st)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
@@ -570,19 +585,21 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
 
 
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
-                          check: bool = True) -> torch.Tensor:
+                          check: bool = True, reduce_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
-    for the exchange.  Bit-identical on every rank to the rank-order left fold with torch's adds."""
-    _check_reducible(t, "all_reduce_compressed")
+    for the exchange.  Bit-identical on every rank to the rank-order left fold with torch's adds.
+    reduce_dtype=torch.float32 with a float16 / bfloat16 t sums in fp32 as reduce_scatter_compressed does and
+    all-gathers the fp32 shards: the float32 result is the fp32 fold on every rank."""
+    acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
     world = _world(group)
     flat = t.reshape(-1)
     n = flat.numel()
     if world == 1 or n == 0:
-        return t.clone()
+        return t.to(acc_dtype, copy=True)
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
-    shard = reduce_scatter_compressed(src, group, members, temp_mem, check)
+    shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype)
     full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check)
     return full[:n].view(t.shape)

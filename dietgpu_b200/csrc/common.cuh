@@ -197,7 +197,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, uint32_t n,
                 const HostMember* members, uint8_t* outSuccess_dev, uint32_t* outSize_dev,
                 uint8_t* mismatchHost, cudaStream_t stream);
-int decodeReduce(int kind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
+int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, cudaStream_t stream);
 size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize);

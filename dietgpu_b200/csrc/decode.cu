@@ -1154,14 +1154,21 @@ int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineM
 // instead of once per row on the decode loop), adds, and stores.
 // LUTs cost shared memory, so at most kReducePass archives are decoded per launch; the host issues
 // ceil(W / kReducePass) launches in order and every launch after the first accumulates (DESIGN.md section 3).
+// Widening sums (dgb_float_decompress_reduce_to): fp16 / bf16 archives summed into fp32 outputs.  The kernel's
+// kind is then the archive kind | kWidenF32; every decoded word is converted exactly to fp32 and each add is one
+// fp32 round-to-nearest-even add, which is torch's acc.float() + x.float() fold.
 // ---------------------------------------------------------------------------
 #ifndef DGB_REDUCE_PASS_ARCHIVES
 #define DGB_REDUCE_PASS_ARCHIVES 4
 #endif
 constexpr uint32_t kReducePass = DGB_REDUCE_PASS_ARCHIVES;
 constexpr int kReduceWarps = 8;
-// writer kinds of the decode-and-sum: the dense kind | kAddWriter adds the decoded word to the output's word
+// writer kinds of the decode-and-sum: the dense kind | kAddWriter adds the decoded word to the output's word;
+// | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives
 constexpr int kAddWriter = 0x10;
+constexpr int kWidenF32 = 0x20;
+// the archive kind of a decode-and-sum kernel or writer kind
+__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32); }
 
 template <int KIND>
 __device__ __forceinline__ uint32_t addWord(uint32_t a, uint32_t b) {
@@ -1236,6 +1243,70 @@ struct RowWriter<kKindF32 | kAddWriter> : RowWriter<kKindF32> {
   }
 };
 
+// The exact fp32 value of a joined fp16 / bf16 word.  join leaves garbage above bit 15 (the 16-bit store drops
+// it), so the widening takes the low half only.
+template <int KIND>
+__device__ __forceinline__ uint32_t widenWord(uint32_t w) {
+  if constexpr (KIND == kKindBF16) {
+    return w << 16;
+  } else {
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)w));
+    return __float_as_uint(f);
+  }
+}
+
+// Widening writers: the 16-bit kind's ring, copies and join; each lane stores one u32 per row, so a row is one
+// 128 B store.  The store writer takes archive 0 of a non-accumulating call, the add writer every later archive.
+template <int KIND>
+struct RowWriterWiden16 : RowWriter16<KIND> {
+  typedef RowWriter16<KIND> B;
+  uint32_t* out32;
+  struct Cursor { uint32_t* o; uint32_t s; };
+  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
+    B::setBlock(av, outBase, block, l);
+    out32 = static_cast<uint32_t*>(outBase) + (size_t)block * kBlockBytes + l;
+    __builtin_assume(__isGlobal(out32));
+  }
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    return Cursor{out32 + row * 32u, B::ring + slot * B::kRingSlotBytes + B::lane};
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = widenWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    out32[row * 32u] = widenWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)));
+  }
+};
+
+template <int KIND>
+struct RowWriterWidenAdd16 : RowWriterWiden16<KIND> {
+  typedef RowWriterWiden16<KIND> W;
+  typedef RowWriter16<KIND> B;
+  struct Cursor { uint32_t* o; uint32_t s; uint32_t prev[kGroupRows]; };
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    Cursor c;
+    c.o = W::out32 + row * 32u;
+    c.s = B::ring + slot * B::kRingSlotBytes + B::lane;
+#pragma unroll
+    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU32(c.o + j * 32);
+    return c;
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = addWord<kKindF32>(c.prev[J], widenWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s))));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = W::out32 + row * 32u;
+    *o = addWord<kKindF32>(*o, widenWord<KIND>(B::join(entry, __ldg(B::non + row * 32u))));
+  }
+};
+template <> struct RowWriter<kKindF16 | kWidenF32> : RowWriterWiden16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32> : RowWriterWiden16<kKindBF16> {};
+template <> struct RowWriter<kKindF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindBF16> {};
+
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
 // consistent with its word count, and that word count is the group's output size.
 template <int KIND, int PB>
@@ -1253,7 +1324,7 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
                                                   const typename Lut<PB, false>::Entry* __restrict__ lut,
                                                   uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
                                                   uint32_t slotWords, uint32_t lane) {
-  const ArchiveView av = openArchive<WK & ~kAddWriter>(in);
+  const ArchiveView av = openArchive<reduceArchiveKind(WK)>(in);
   const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
   const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
   const uint16_t* pData = reinterpret_cast<const uint16_t*>(
@@ -1286,11 +1357,12 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
 
 // One pass: archives [a0, a1) of every group.  Member table entry g * width + j = {archive (g, j), out[g],
 // out_size[g], block cap of group g}.  addFirst: archive a0 adds too (accumulate, or a later pass).  Only the
-// first pass (a0 == 0) reports outSuccess.
+// first pass (a0 == 0) reports outSuccess.  KIND is the archive kind, | kWidenF32 for fp32 outputs.
 template <int KIND, int PB>
 __global__ void __launch_bounds__(kReduceWarps * 32, 4)
 decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
                    uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
+  constexpr int AK = reduceArchiveKind(KIND);
   constexpr int WARPS = kReduceWarps;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t K = 1u << PB;
@@ -1303,8 +1375,9 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
   uint32_t* sMisc = sWarp + 32;
   unsigned long long* sBar = reinterpret_cast<unsigned long long*>(sMisc + 32);
   uint8_t* sRing = reinterpret_cast<uint8_t*>(sBar + ((WARPS + 1) & ~1));
-  constexpr uint32_t ringBytes = kRingSlots * RowWriter<KIND>::kRingSlotBytes;
-  static_assert(RowWriter<KIND | kAddWriter>::kRingSlotBytes == RowWriter<KIND>::kRingSlotBytes, "");
+  constexpr uint32_t ringBytes = kRingSlots * RowWriter<AK>::kRingSlotBytes;
+  static_assert(RowWriter<KIND | kAddWriter>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
+  static_assert(RowWriter<KIND>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
   uint8_t* sSlots = sRing + WARPS * ringBytes;
   const uint32_t slotBytes = 128u + slotWords * 2u;
 
@@ -1367,14 +1440,14 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
     //      headers and out_size alone, so every CTA and every pass takes the same one ----
     bool ok = true;
     for (uint32_t j = t; j < width; j += WARPS * 32) {
-      const bool v = reduceArchiveOk<KIND, PB>(memberAt(im, sc.members, g * width + j).in, gd.size);
+      const bool v = reduceArchiveOk<AK, PB>(memberAt(im, sc.members, g * width + j).in, gd.size);
       if (report) outSuccess[g * width + j] = v ? 1 : 0;
       ok = ok && v;
     }
     const bool work = __syncthreads_and(ok) && nb > 0;
     if (work) {
       for (uint32_t a = a0; a < a1; ++a)
-        buildLut<PB, false, WARPS>(openArchive<KIND>(static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in)).ans,
+        buildLut<PB, false, WARPS>(openArchive<AK>(static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in)).ans,
                                    lut[a - a0], sPdf, sCdf, sWarp);
     }
 
@@ -1408,7 +1481,7 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
                        uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream) {
   auto kern = decodeReduceKernel<KIND, PB>;
   uint32_t slotWords;
-  const size_t smemBytes = decoderSmem<KIND, PB>(kReduceWarps, opt, &slotWords);
+  const size_t smemBytes = decoderSmem<reduceArchiveKind(KIND), PB>(kReduceWarps, opt, &slotWords);
   int perSm = 1;
   const int rc = residentCtasPerSm((const void*)kern, kReduceWarps * 32, smemBytes, 160 * 1024, &perSm);
   if (rc != DGB_OK) return rc;
@@ -1563,10 +1636,13 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   return DGB_OK;
 }
 
-int decodeReduce(int kind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
+int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, cudaStream_t stream) {
   if (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32) return DGB_ERR_INVALID_ARG;
+  // outputs of the archive kind, or fp32 sums of fp16 / bf16 archives
+  const bool widen = outKind != kind;
+  if (widen && !(outKind == kKindF32 && (kind == kKindF16 || kind == kKindBF16))) return DGB_ERR_INVALID_ARG;
   if (pb < 9 || pb > 11 || width == 0) return DGB_ERR_INVALID_ARG;
   if (groups == 0) return DGB_OK;
   if (!in || !out || !outSize) return DGB_ERR_INVALID_ARG;
@@ -1581,7 +1657,7 @@ int decodeReduce(int kind, void* temp, size_t tempBytes, int pb, uint32_t groups
   HostStage& hs = hostStage();
   hs.decodeTable.resize(n);
   MemberDesc* desc = hs.decodeTable.data();
-  const uint32_t elemBytes = wordBytes(kind);
+  const uint32_t elemBytes = wordBytes(outKind);
   uint64_t totalChunks = 0;
   for (uint32_t g = 0; g < groups; ++g) {
     if ((outSize[g] && !out[g]) || (reinterpret_cast<uintptr_t>(out[g]) & (elemBytes - 1u))) return DGB_ERR_INVALID_ARG;
@@ -1610,7 +1686,13 @@ int decodeReduce(int kind, void* temp, size_t tempBytes, int pb, uint32_t groups
   }
   return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
     constexpr int KIND = decltype(K)::value;
-    if constexpr (KIND == kKindF16 || KIND == kKindBF16 || KIND == kKindF32)
+    if constexpr (KIND == kKindF16 || KIND == kKindBF16) {
+      if (widen)
+        return launchDecodeReduce<KIND | kWidenF32, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
+                                                                       accumulate, outSuccess_dev, stream);
+      return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
+                                                         outSuccess_dev, stream);
+    } else if constexpr (KIND == kKindF32)
       return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
                                                          outSuccess_dev, stream);
     else

@@ -351,19 +351,30 @@ _REDUCE_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, tor
 def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequence[torch.Tensor],
                            accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
                            out_status: Optional[torch.Tensor] = None, *,
-                           prob_bits: int = K_DEFAULT_PRECISION) -> int:
-    """Decode-and-sum (dgb_float_decompress_reduce): ts_in is G lists of W uint8 float archives each, ts_out G
+                           prob_bits: int = K_DEFAULT_PRECISION,
+                           archive_dtype: Optional[torch.dtype] = None) -> int:
+    """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
     that dtype, where x(g, j) is archive ts_in[g][j] decoded; each archive must hold exactly ts_out[g].numel()
     words.  A group with an invalid archive is left untouched; out_status (CUDA uint8, G * W entries, group-major)
-    receives 1 / 0 per archive.  Returns the scratch bytes used."""
+    receives 1 / 0 per archive.  Returns the scratch bytes used.
+
+    archive_dtype: the archives' dtype; None (or the outputs' dtype) means the outputs' dtype.  float16 or
+    bfloat16 archives with float32 outputs are summed in float32: the result is
+    torch's fold acc = x(g, 0).float(); acc = acc + x(g, 1).float(); ... bit for bit.  Any other pair raises
+    ValueError."""
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
     dtype = ts_out[0].dtype
     if dtype not in _REDUCE_TYPES:
         raise ValueError(f"decompress_data_reduce sums float16, bfloat16 or float32 outputs, not {dtype}")
+    if archive_dtype is None:
+        archive_dtype = dtype
+    if archive_dtype != dtype and not (dtype == torch.float32 and archive_dtype in (torch.float16, torch.bfloat16)):
+        raise ValueError(f"decompress_data_reduce sums {archive_dtype} archives into {archive_dtype} outputs, or "
+                         f"float16 / bfloat16 archives into float32 outputs; not into {dtype}")
     dev = ts_out[0].device
     ins = []
     for group, to in zip(ts_in, ts_out):
@@ -377,16 +388,16 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
             ins.append(ti)
     g, n = len(ts_out), len(ins)
     st_ptr, _ = _validate_status(out_status, None, n, dev)
-    ft = _REDUCE_TYPES[dtype]
+    ft, out_ft = _REDUCE_TYPES[archive_dtype], _REDUCE_TYPES[dtype]
     L = capi.lib()
     with torch.cuda.device(dev):
         need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
         tmp = _Temp(temp_mem, need, dev)
-        rc = L.dgb_float_decompress_reduce(tmp.ptr, tmp.bytes, ft, prob_bits, g, width,
-                                           capi.ptr_array([t.data_ptr() for t in ins]),
-                                           capi.ptr_array([t.data_ptr() for t in ts_out]),
-                                           capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
-                                           st_ptr, _stream())
+        rc = L.dgb_float_decompress_reduce_to(tmp.ptr, tmp.bytes, ft, out_ft, prob_bits, g, width,
+                                              capi.ptr_array([t.data_ptr() for t in ins]),
+                                              capi.ptr_array([t.data_ptr() for t in ts_out]),
+                                              capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
+                                              st_ptr, _stream())
     capi.check(rc, "decompress_data_reduce")
     return tmp.need
 

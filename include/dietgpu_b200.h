@@ -215,6 +215,23 @@ int dgb_float_decompress_reduce(void* temp_dev, size_t temp_bytes, int float_typ
                                 void* const* out, const uint32_t* out_size, int accumulate,
                                 uint8_t* out_success_dev, void* stream);
 
+/* Decode-and-sum into outputs of out_float_type (new; no reference counterpart).  The allowed pairs
+ * (float_type, out_float_type) are (DGB_FLOAT16, DGB_FLOAT16), (DGB_BFLOAT16, DGB_BFLOAT16) and
+ * (DGB_FLOAT32, DGB_FLOAT32), which give exactly what dgb_float_decompress_reduce gives, and the widening pairs
+ * (DGB_FLOAT16, DGB_FLOAT32) and (DGB_BFLOAT16, DGB_FLOAT32); any other pair returns DGB_ERR_INVALID_ARG.
+ * Widening: out[g] = (accumulate ? out[g] : f(x(g,0))) + f(x(g,1)) + ... + f(x(g,W-1)) in archive order, where
+ * f is the exact conversion of a 16-bit word to fp32 and each + is one fp32 round-to-nearest-even addition,
+ * subnormals kept: bit-identical to torch's fold acc = x0.float(); acc = acc + x1.float(); ...  With W = 1 and
+ * no accumulate this is a plain decode widened to fp32 (-0, infinities and subnormals exact; a NaN stays a
+ * NaN).  Outputs are fp32 (4 B aligned) and out_size counts their elements, which must equal every archive's
+ * word count.  Everything else is as in dgb_float_decompress_reduce: the validity rule (the archives have
+ * float_type), statuses, groups with an invalid archive left unwritten, no synchronisation, graph capture and
+ * the scratch size dgb_float_decompress_temp_bytes(float_type, G * W, 0). */
+int dgb_float_decompress_reduce_to(void* temp_dev, size_t temp_bytes, int float_type, int out_float_type,
+                                   int prob_bits, uint32_t num_groups, uint32_t archives_per_group,
+                                   const void* const* in, void* const* out, const uint32_t* out_size,
+                                   int accumulate, uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

@@ -1,6 +1,6 @@
 """Decode-and-sum (ops.decompress_data_reduce) against decoding the same archives separately, on one GPU.
 
-    python tools/reduce_bench.py [--iters 30] [--json out.json]
+    python tools/reduce_bench.py [--iters 30] [--json out.json] [--reduce-dtype float32]
 
 For each shape (G groups x W archives x N words of N(0,1) data, seeded) three ways are timed on the same archives,
 alternating within the run:
@@ -117,15 +117,78 @@ def bench(dtype, groups, width, n, iters):
     return r
 
 
+SHAPES32 = [s for s in SHAPES if s[0] != torch.float32]
+
+
+def bench32(dtype, groups, width, n, iters):
+    """--reduce-dtype float32: 16-bit archives summed into fp32 outputs, three ways on the same archives:
+    (1) decompress_data_reduce(archive_dtype=dtype) into fp32; (2) decompress_data into 16-bit temporaries, then
+    acc.copy_(tmp_0) and acc.add_(tmp_j) in fp32 (torch's widening adds); (3) the same-type decode-and-sum into 16-bit
+    outputs, for reference.  Algorithmic bytes per element and accumulated archive (r = archive bytes / input
+    bytes): (1) 2r + 8 (archive, fp32 read, fp32 write); (2) 2r + 2 + 6 + 4 (archive, 16-bit write; 16-bit and fp32
+    read; fp32 write)."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [torch.randn(n, generator=g, device="cuda").to(dtype) for _ in range(groups * width)]
+    comp, sizes, _ = ops.compress_data(True, xs)
+    hs = sizes.cpu().tolist()
+    arch = [comp[i, :hs[i]] for i in range(len(xs))]
+    del xs
+    groups_in = [arch[k * width:(k + 1) * width] for k in range(groups)]
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    red = [torch.empty(n, dtype=torch.float32, device="cuda") for _ in range(groups)]
+    sep = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups * width)]
+    acc = [torch.empty(n, dtype=torch.float32, device="cuda") for _ in range(groups)]
+    red16 = [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups)]
+
+    def one():
+        ops.decompress_data_reduce(groups_in, red, False, temp, archive_dtype=dtype)
+
+    def decode():
+        ops.decompress_data(True, arch, sep, False, temp)
+
+    def two():
+        decode()
+        for k in range(groups):
+            acc[k].copy_(sep[k * width])
+            for j in range(1, width):
+                acc[k].add_(sep[k * width + j])
+
+    def three():
+        ops.decompress_data_reduce(groups_in, red16, False, temp)
+
+    for f in (one, two, three):  # warm-up
+        f()
+    torch.cuda.synchronize()
+    for k in range(groups):
+        assert torch.equal(red[k].view(torch.int32), acc[k].view(torch.int32)), k
+    t = {"1": [], "2": [], "3": []}
+    for _ in range(3):  # alternate
+        t["1"].append(timed(one, iters))
+        t["2"].append(timed(two, iters))
+        t["3"].append(timed(three, iters))
+    k1, k2, k3 = kernel_us(one, iters), kernel_us(decode, iters), kernel_us(three, iters)
+    ratio = sum(hs) / (groups * width * n * 2)
+    r = {"shape": f"{str(dtype).split('.')[-1]}->float32 {groups}x{width}x{n}", "archive_MB": sum(hs) / 1e6,
+         "ratio": ratio, "bytes_per_elem_archive": {"1": 2 * ratio + 8, "2": 2 * ratio + 12},
+         "call_us": {k: min(v) for k, v in t.items()}, "call_us_max": {k: max(v) for k, v in t.items()},
+         "kernel_us": {"1": k1, "2_decode": k2, "3": k3}}
+    r["1_over_2"] = r["call_us"]["1"] / r["call_us"]["2"]
+    r["1_over_3"] = r["call_us"]["1"] / r["call_us"]["3"]
+    r["kernel_1_over_3"] = k1 / k3
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--reduce-dtype", choices=["same", "float32"], default="same",
+                    help="float32: sum the 16-bit shapes' archives into fp32 outputs (bench32)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    for shape in SHAPES:
-        r = bench(*shape, args.iters)
+    for shape in (SHAPES32 if args.reduce_dtype == "float32" else SHAPES):
+        r = (bench32 if args.reduce_dtype == "float32" else bench)(*shape, args.iters)
         info["results"].append(r)
         print(json.dumps(r), flush=True)
     if args.json:
