@@ -9,8 +9,10 @@
 //                    reference's -- reads it.
 //   tileDecompress : the inverse, one CTA per archive, decoded tile handed on through shared memory.
 //
-// tests/test_gpu_device_api.py drives both through the extern "C" launchers below and checks the
-// archives byte for byte against the CPU oracle and through the library's own decoder.
+// Both are templates on the probability precision PB (9, 10 or 11, the archive's probBits); the
+// extern "C" launchers below take it at run time and dispatch.  tests/test_gpu_device_api.py drives
+// them and checks the archives byte for byte against the CPU oracle and through the library's own
+// decoder.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -19,25 +21,26 @@
 namespace dd = dietgpu_b200::device;
 
 constexpr int kWarps = 8;
-constexpr int kProbBits = 10;
 constexpr uint32_t kTileMax = kWarps * dd::kBlockBytes;
 
+template <int PB>
 struct TileSmem {
   uint32_t hist[dd::kNumSymbols];
   dd::EncodeTable table;
   uint16_t pdf[dd::kNumSymbols];
   uint32_t words[kWarps];
   uint32_t offset[kWarps + 1];
-  uint32_t lut[1u << kProbBits];
+  uint32_t lut[1u << PB];
   alignas(16) uint8_t tile[kTileMax];
-  alignas(16) uint16_t stream[kWarps][dd::maxBlockWords(kProbBits)];
+  alignas(16) uint16_t stream[kWarps][dd::maxBlockWords(PB)];
 };
 
+template <int PB>
 __global__ void __launch_bounds__(kWarps * 32)
 tileCompress(const uint8_t* __restrict__ in, uint32_t totalBytes, uint32_t tileBytes, uint8_t* __restrict__ out,
              uint32_t outStride, uint32_t* __restrict__ outSize) {
   extern __shared__ __align__(16) uint8_t raw[];
-  TileSmem& s = *reinterpret_cast<TileSmem*>(raw);
+  TileSmem<PB>& s = *reinterpret_cast<TileSmem<PB>*>(raw);
   const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
   const uint32_t begin = blockIdx.x * tileBytes;
   const uint32_t n = min(tileBytes, totalBytes - begin);
@@ -52,13 +55,13 @@ tileCompress(const uint8_t* __restrict__ in, uint32_t totalBytes, uint32_t tileB
     atomicAdd(&s.hist[b], 1u);
   }
   __syncthreads();
-  dd::blockBuildEncodeTable(s.hist, n, kProbBits, &s.table, s.pdf);
+  dd::blockBuildEncodeTable(s.hist, n, PB, &s.table, s.pdf);
 
   // one 4 KiB block per warp, shared memory to shared memory
   uint32_t state = 0, words = 0;
   const uint32_t blockLen = warp < nb ? min(dd::kBlockBytes, n - warp * dd::kBlockBytes) : 0u;
   if (warp < nb) {
-    words = dd::warpEncodeBlock(s.tile + warp * dd::kBlockBytes, blockLen, &s.table, kProbBits, s.stream[warp], &state);
+    words = dd::warpEncodeBlock(s.tile + warp * dd::kBlockBytes, blockLen, &s.table, PB, s.stream[warp], &state);
     if (lane == 0) s.words[warp] = words;
   }
   __syncthreads();
@@ -82,26 +85,27 @@ tileCompress(const uint8_t* __restrict__ in, uint32_t totalBytes, uint32_t tileB
   }
   if (t == 0) {
     if (nb & 1u) a.blockWords[nb] = make_uint2(0u, 0u);
-    dd::writeArchiveHeader(archive, nb, n, s.offset[nb], kProbBits);
+    dd::writeArchiveHeader(archive, nb, n, s.offset[nb], PB);
     outSize[blockIdx.x] = dd::archiveOverhead(nb) + 2u * s.offset[nb];
   }
 }
 
+template <int PB>
 __global__ void __launch_bounds__(kWarps * 32)
 tileDecompress(const uint8_t* __restrict__ in, uint32_t inStride, uint8_t* __restrict__ out, uint32_t tileBytes,
                uint32_t* __restrict__ okOut) {
   extern __shared__ __align__(16) uint8_t raw[];
-  TileSmem& s = *reinterpret_cast<TileSmem*>(raw);
+  TileSmem<PB>& s = *reinterpret_cast<TileSmem<PB>*>(raw);
   const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
   const uint8_t* archive = in + (size_t)blockIdx.x * inStride;
   const uint4 h0 = *reinterpret_cast<const uint4*>(archive);
   const uint32_t nb = h0.y, n = h0.z;
   bool ok = h0.x == dd::kAnsMagicVersion && nb <= kWarps && n <= kTileMax;
   const dd::ArchiveLayout a = dd::archiveLayout(const_cast<uint8_t*>(archive), ok ? nb : 0u);
-  ok = ok && dd::blockBuildDecodeLut<kProbBits, kWarps * 32>(a.pdf, s.lut);
+  ok = ok && dd::blockBuildDecodeLut<PB, kWarps * 32>(a.pdf, s.lut);
   if (ok && warp < nb) {
     const uint2 bw = a.blockWords[warp];
-    ok = dd::warpDecodeBlock<kProbBits>(a.states[warp * 32 + lane], a.data + bw.y, bw.x & 0xffffu, bw.x >> 16, s.lut,
+    ok = dd::warpDecodeBlock<PB>(a.states[warp * 32 + lane], a.data + bw.y, bw.x & 0xffffu, bw.x >> 16, s.lut,
                                         s.tile + warp * dd::kBlockBytes);
   }
   const int allOk = __syncthreads_and(ok ? 1 : 0);
@@ -111,20 +115,45 @@ tileDecompress(const uint8_t* __restrict__ in, uint32_t inStride, uint8_t* __res
   if (t == 0) okOut[blockIdx.x] = (uint32_t)allOk;
 }
 
-extern "C" int example_tile_compress(const void* in, uint32_t totalBytes, uint32_t tileBytes, void* out,
-                                     uint32_t outStride, uint32_t* outSize, void* stream) {
-  if (tileBytes == 0 || tileBytes > kTileMax || totalBytes == 0) return 1;
+template <int PB>
+int launchCompress(const void* in, uint32_t totalBytes, uint32_t tileBytes, void* out, uint32_t outStride,
+                   uint32_t* outSize, cudaStream_t stream) {
   const uint32_t tiles = (totalBytes + tileBytes - 1) / tileBytes;
-  cudaFuncSetAttribute(tileCompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
-  tileCompress<<<tiles, kWarps * 32, sizeof(TileSmem), (cudaStream_t)stream>>>(
+  cudaFuncSetAttribute(tileCompress<PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<PB>));
+  tileCompress<PB><<<tiles, kWarps * 32, sizeof(TileSmem<PB>), stream>>>(
       static_cast<const uint8_t*>(in), totalBytes, tileBytes, static_cast<uint8_t*>(out), outStride, outSize);
   return (int)cudaGetLastError();
 }
 
-extern "C" int example_tile_decompress(const void* in, uint32_t inStride, uint32_t tiles, void* out, uint32_t tileBytes,
-                                       uint32_t* okOut, void* stream) {
-  cudaFuncSetAttribute(tileDecompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
-  tileDecompress<<<tiles, kWarps * 32, sizeof(TileSmem), (cudaStream_t)stream>>>(
+template <int PB>
+int launchDecompress(const void* in, uint32_t inStride, uint32_t tiles, void* out, uint32_t tileBytes,
+                     uint32_t* okOut, cudaStream_t stream) {
+  cudaFuncSetAttribute(tileDecompress<PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<PB>));
+  tileDecompress<PB><<<tiles, kWarps * 32, sizeof(TileSmem<PB>), stream>>>(
       static_cast<const uint8_t*>(in), inStride, static_cast<uint8_t*>(out), tileBytes, okOut);
   return (int)cudaGetLastError();
+}
+
+// probBits: 9, 10 or 11 (the archive's); anything else returns nonzero without launching.
+extern "C" int example_tile_compress(const void* in, uint32_t totalBytes, uint32_t tileBytes, void* out,
+                                     uint32_t outStride, uint32_t* outSize, int probBits, void* stream) {
+  if (tileBytes == 0 || tileBytes > kTileMax || totalBytes == 0) return 1;
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (probBits) {
+    case 9: return launchCompress<9>(in, totalBytes, tileBytes, out, outStride, outSize, st);
+    case 10: return launchCompress<10>(in, totalBytes, tileBytes, out, outStride, outSize, st);
+    case 11: return launchCompress<11>(in, totalBytes, tileBytes, out, outStride, outSize, st);
+    default: return 1;
+  }
+}
+
+extern "C" int example_tile_decompress(const void* in, uint32_t inStride, uint32_t tiles, void* out, uint32_t tileBytes,
+                                       uint32_t* okOut, int probBits, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (probBits) {
+    case 9: return launchDecompress<9>(in, inStride, tiles, out, tileBytes, okOut, st);
+    case 10: return launchDecompress<10>(in, inStride, tiles, out, tileBytes, okOut, st);
+    case 11: return launchDecompress<11>(in, inStride, tiles, out, tileBytes, okOut, st);
+    default: return 1;
+  }
 }
