@@ -26,7 +26,7 @@ SYMBOLS = [
     "dgb_ans_encode_pointer", "dgb_ans_encode_stride", "dgb_ans_encode_split_size",
     "dgb_ans_decode_pointer", "dgb_ans_decode_stride", "dgb_ans_decode_split_size",
     "dgb_ans_get_compressed_info",
-    "dgb_float_compress_pointer", "dgb_float_compress_split_size",
+    "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_split_size",
     "dgb_float_decompress_pointer", "dgb_float_decompress_split_size", "dgb_float_decompress_reduce",
     "dgb_float_decompress_reduce_to", "dgb_float_get_compressed_info",
     "dgb_copy_async", "dgb_copy_rows_async", "dgb_archives_pull",
@@ -95,6 +95,8 @@ def lib():
     L.dgb_ans_get_compressed_info.argtypes = [vp, sz, vp, i32, u32, vp, vp, vp]
     L.dgb_float_compress_pointer.restype = i32
     L.dgb_float_compress_pointer.argtypes = [vp, sz, i32, i32, i32, u32, vp, vp, vp, vp, vp]
+    L.dgb_float_compress_to.restype = i32
+    L.dgb_float_compress_to.argtypes = [vp, sz, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp]
     L.dgb_float_compress_split_size.restype = i32
     L.dgb_float_compress_split_size.argtypes = [vp, sz, i32, i32, i32, u32, vp, vp, vp, u32, vp, vp]
     L.dgb_float_decompress_pointer.restype = i32

@@ -317,10 +317,19 @@ def _split(n: int, parts: int, quantum: int) -> List[int]:
     return [i * per for i in range(parts)] + [n]
 
 
+def _check_wire(t: torch.Tensor, what: str, wire_dtype: Optional[torch.dtype]) -> None:
+    """wire_dtype: None, or float16 / bfloat16 for a float32 t (narrowing compress on the send side)."""
+    if wire_dtype is None:
+        return
+    if wire_dtype not in (torch.float16, torch.bfloat16) or t.dtype != torch.float32:
+        raise ValueError(f"{what}: wire_dtype is None, or float16 / bfloat16 for a float32 tensor; "
+                         f"not {wire_dtype} for {t.dtype}")
+
+
 def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, stages: int = 2,
                           peer: Optional[PeerWorkspace] = None, check: bool = True,
-                          peer_mode: str = "auto") -> torch.Tensor:
+                          peer_mode: str = "auto", wire_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Every rank contributes the CUDA tensor `t` (same shape and dtype on every rank; fp16 / bf16 / fp32 go
     through the float codec, anything else through the byte codec) and receives the concatenation
     [world * t.numel()] in rank order, bit-exact.  `members` = archives per rank (the codec's parallelism
@@ -330,9 +339,17 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
     unit u is decoded; the fastest at 8 GPUs), "push" (the mover writes each coded group into the peers' inboxes
     and flags it; no barrier; the fastest at 2 GPUs) or "direct" (after a barrier the decode kernel reads peer
     memory itself); `stages` = pipeline groups per peer;
-    `check=False` then skips the only host synchronisation (the read of the decode status)."""
+    `check=False` then skips the only host synchronisation (the read of the decode status).
+
+    wire_dtype=torch.float16 / torch.bfloat16 with a float32 t (fp32 master weights gathered as 16-bit
+    parameters, FSDP's param_dtype): each member is rounded to wire_dtype inside the compress kernels, the 16-bit
+    archives go over the wire, and the result has wire_dtype and equals cat([t_r.to(wire_dtype) for every rank r])
+    bit for bit.  NCCL / gloo transport only: with `peer` it raises ValueError."""
     if not t.is_cuda or not t.is_contiguous():
         raise ValueError("all_gather_compressed: contiguous CUDA tensor expected (no CPU fallback)")
+    _check_wire(t, "all_gather_compressed", wire_dtype)
+    if wire_dtype is not None and peer is not None:
+        raise ValueError("all_gather_compressed: wire_dtype is not supported with the peer-memory transports")
     as_float = t.dtype in (torch.float16, torch.bfloat16, torch.float32)
     flat = t.reshape(-1) if as_float else t.reshape(-1).view(torch.uint8)
     n = flat.numel()
@@ -353,13 +370,14 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
             out = _all_gather_peer(flat, as_float, bounds, peer, checksum, temp_mem, check, peer_mode == "direct", stages)
         return out if as_float else out.view(t.dtype)
     world = _world(group)
-    out = torch.empty(world * n, dtype=flat.dtype, device=t.device)
+    out = torch.empty(world * n, dtype=wire_dtype or flat.dtype, device=t.device)
     stages = max(1, min(int(stages), members))
     cuts = [round(k * members / stages) for k in range(stages + 1)]
     pieces = [(cuts[k], cuts[k + 1]) for k in range(stages) if cuts[k + 1] > cuts[k]]
 
     def compress(a, b):
-        comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem)
+        comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem,
+                                           archive_dtype=wire_dtype)
         return comp, sizes
 
     def decompress(a, b, gathered):
@@ -504,7 +522,8 @@ def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dt
 
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               temp_mem: Optional[torch.Tensor] = None, check: bool = True,
-                              reduce_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                              reduce_dtype: Optional[torch.dtype] = None,
+                              wire_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -517,22 +536,31 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     reduce_dtype=torch.float32 with a float16 / bfloat16 t (mixed-precision gradients summed in fp32): the wire
     still carries the 16-bit archives, the result is float32 and equals the fp32 fold
     ((t_0.float() + t_1.float()) + t_2.float()) + ... bit for bit.  None or t.dtype sums in t's dtype; any other
-    value raises ValueError."""
+    value raises ValueError.
+
+    wire_dtype=torch.float16 / torch.bfloat16 with a float32 t (fp32 gradients sent as 16 bits, DeepSpeed's
+    communication_data_type, Megatron's bf16 gradient communication): every chunk is rounded to wire_dtype inside
+    the compress kernels, the 16-bit archives go over the wire and are summed in fp32, and the float32 result is
+    ((t_0.to(w).float() + t_1.to(w).float()) + t_2.to(w).float()) + ... bit for bit, on every rank and for every
+    `members`.  reduce_dtype must then be None or float32."""
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
+    _check_wire(t, "reduce_scatter_compressed", wire_dtype)
     world = _world(group)
     flat = t.reshape(-1)
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
+    arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     if world == 1 or n == 0:
-        return flat[: n // world].to(acc_dtype, copy=True)
+        return flat[: n // world].to(arch_dtype).to(acc_dtype, copy=True)
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
     m = len(bounds) - 1
     dests = [d for d in range(world) if d != rank]
     comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
-                                              for d in dests for i in range(m)], False, temp_mem)
+                                              for d in dests for i in range(m)], False, temp_mem,
+                                       archive_dtype=arch_dtype)
     on_device = _device_collectives(group)
     cdev = dev if on_device else torch.device("cpu")
     hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
@@ -562,7 +590,7 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
         archives.append(row)
     out = torch.empty(shard, dtype=acc_dtype, device=dev)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
-    own = flat[rank * shard:(rank + 1) * shard]
+    own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
     statuses = []
     # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add; fp32 += fp16 /
     # bf16 is the same fp32 add of the widened word), + r+1..world-1
@@ -571,13 +599,13 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     else:
         st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
-                                   archive_dtype=t.dtype)
+                                   archive_dtype=arch_dtype)
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st, archive_dtype=t.dtype)
+                                   temp_mem, st, archive_dtype=arch_dtype)
         statuses.append(st)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")

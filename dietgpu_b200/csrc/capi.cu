@@ -421,6 +421,24 @@ int dgb_float_compress_pointer(void* temp, size_t tempBytes, int ft, int pb, int
                      (cudaStream_t)stream);
 }
 
+int dgb_float_compress_to(void* temp, size_t tempBytes, int inFt, int ft, int pb, int useChecksum, uint32_t n,
+                          const void* const* in, const uint32_t* inSize, void* const* out, uint32_t* outSize_dev,
+                          void* stream) {
+  int kind;
+  if (inFt == ft && (ft == DGB_FLOAT16 || ft == DGB_BFLOAT16 || ft == DGB_FLOAT32))
+    kind = ft;  // dgb_float_compress_pointer
+  else if (inFt == DGB_FLOAT32 && ft == DGB_FLOAT16)
+    kind = kKindF32toF16;
+  else if (inFt == DGB_FLOAT32 && ft == DGB_BFLOAT16)
+    kind = kKindF32toBF16;
+  else
+    return DGB_ERR_INVALID_ARG;
+  HostMember* v = nullptr;
+  int rc = buildPointer(n, in, inSize, out, &v);
+  if (rc) return rc;
+  return encodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev, (cudaStream_t)stream);
+}
+
 int dgb_float_compress_split_size(void* temp, size_t tempBytes, int ft, int pb, int useChecksum,
                                   uint32_t n, const void* in_dev, const uint32_t* splitSizes,
                                   void* out_dev, uint32_t outStride, uint32_t* outSize_dev,

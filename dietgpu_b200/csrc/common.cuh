@@ -113,8 +113,17 @@ enum CodecKind : int {
   kKindF64 = DGB_FLOAT64,
   kKindF16S = DGB_FLOAT16_SPARSE,
   kKindBF16S = DGB_BFLOAT16_SPARSE,
-  kKindF32S = DGB_FLOAT32_SPARSE
+  kKindF32S = DGB_FLOAT32_SPARSE,
+  // Narrowing encoder kinds (dgb_float_compress_to), 0x40 | the archive type, never written to the wire: the
+  // encoder reads float32 words and rounds each to the archive type's 16-bit word (cvt.rn, torch's CUDA cast)
+  // before it takes the coded and stored bytes out of it, so the archive is an ordinary fp16 / bf16 archive.
+  // Encoder only: decode.cu never dispatches them.
+  kKindF32toF16 = 0x40 | DGB_FLOAT16,
+  kKindF32toBF16 = 0x40 | DGB_BFLOAT16
 };
+__host__ __device__ constexpr bool isNarrowKind(int k) { return k == kKindF32toF16 || k == kKindF32toBF16; }
+// the float type a kind's archives carry (header, size bound, plane layout, table format)
+__host__ __device__ constexpr int archiveKind(int k) { return isNarrowKind(k) ? (k & ~0x40) : k; }
 
 struct MemberDesc {
   const void* in;     // encode: raw input (bytes / float words); decode: archive
@@ -210,8 +219,9 @@ int pullArchives(int kind, uint32_t n, const void* const* src, void* const* dst,
 
 void setLastCudaError(cudaError_t e);
 
-inline uint32_t wordBytes(int kind) {
-  return kind == kKindF64 ? 8u : (kind == kKindF32 || kind == kKindF32S ? 4u : (kind == kKindBytes ? 1u : 2u));
+inline uint32_t wordBytes(int kind) {  // the narrowing kinds: their float32 input words
+  return kind == kKindF64 ? 8u
+                          : (kind == kKindF32 || kind == kKindF32S || isNarrowKind(kind) ? 4u : (kind == kKindBytes ? 1u : 2u));
 }
 inline size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
 int smCount();  // SMs of the current device, cached per device

@@ -1,4 +1,5 @@
-// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16/fp32)
+// encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16/fp32, and
+// float32 inputs narrowed to fp16/bf16 archives)
 // for sm_90a (H100).  Two launches per call, whatever the batch size:
 //
 //   K1  stats*Kernel     a pure read of the raw input: 256-bin histogram of the coded byte, taken out of
@@ -358,8 +359,32 @@ __device__ __forceinline__ uint32_t histOffHi(uint32_t w) {  // high half of a 1
 __device__ __forceinline__ void histAdd(uint32_t* wh, uint32_t byteOff) {
   atomicAdd(reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(wh) + byteOff), 1u);
 }
+// Narrowing kinds: two float32 words rounded to the archive type's 16-bit words at once (lo -> bits 0..15,
+// hi -> bits 16..31), round to nearest even: the packed form of the instruction torch's CUDA cast uses
+// (__float2half: cvt.rn.f16.f32, __float2bfloat16: cvt.rn.bf16.f32), with the same result for every float32
+// bit pattern, NaNs included (tests/test_gpu_narrow.py checks all 2^32).
+template <int KIND>
+__device__ __forceinline__ uint32_t narrowPair(uint32_t lo, uint32_t hi) {
+  uint32_t r;
+  if (KIND == kKindF32toF16)
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
+  else
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
+  return r;
+}
+// One word, in bits 0..15 (the high half rounds +0 to 0).  Not the scalar cvt.rn.f16.f32: ptxas lowers a byte
+// store of that instruction's 16-bit result as a float-to-integer conversion (F2I.U8.F16), not as its low byte.
+template <int KIND>
+__device__ __forceinline__ uint32_t narrowWord(uint32_t w) {
+  return narrowPair<KIND>(w, 0u);
+}
+
 template <int FT>
 __device__ __forceinline__ uint32_t codedScalar(const uint8_t* in, uint32_t e) {
+  if constexpr (isNarrowKind(FT)) {
+    const uint32_t w = narrowWord<FT>(reinterpret_cast<const uint32_t*>(in)[e]);
+    return archiveKind(FT) == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8;
+  }
   if (FT == DGB_FLOAT64) return (reinterpret_cast<const uint32_t*>(in)[2u * (size_t)e + 1u] >> 23) & 0xffu;
   if (FT == DGB_FLOAT32) return (reinterpret_cast<const uint32_t*>(in)[e] >> 23) & 0xffu;
   const uint32_t w = reinterpret_cast<const uint16_t*>(in)[e];
@@ -382,6 +407,15 @@ __device__ __forceinline__ void histVectors(const uint4* __restrict__ vec, const
     for (int k = 0; k < kStatsUnroll; ++k) {
       const uint32_t i = i0 + k * kStatsThreads;
       if (i >= v1) break;
+      if constexpr (isNarrowKind(FT)) {  // four float32 words -> two packed pairs of the archive type
+        constexpr int AT = archiveKind(FT);
+        const uint32_t p0 = narrowPair<FT>(vv[k].x, vv[k].y), p1 = narrowPair<FT>(vv[k].z, vv[k].w);
+        histAdd(wh, histOffLo<AT>(p0));
+        histAdd(wh, histOffHi<AT>(p0));
+        histAdd(wh, histOffLo<AT>(p1));
+        histAdd(wh, histOffHi<AT>(p1));
+        continue;
+      }
       if (FT == DGB_FLOAT64) {  // two words per vector: the coded byte is in each odd 32-bit half
         histAdd(wh, histOffLo<FT>(vv[k].y));
         histAdd(wh, histOffLo<FT>(vv[k].w));
@@ -615,15 +649,17 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
                                                const StatsStage& stage = StatsStage()) {
   constexpr bool SPARSE = isSparseKind(FT);
   constexpr int BT = denseKind(FT);  // the dense type whose natural symbols the histogram counts
-  constexpr uint32_t EPV = (BT == DGB_FLOAT64) ? 2u : (BT == DGB_FLOAT32) ? 4u : 8u;  // elements per 16 B vector
-  constexpr uint32_t WB = 16u / EPV;                                                 // word bytes
+  constexpr bool NARROW = isNarrowKind(FT);  // float32 input words, archives of type AT
+  constexpr int AT = archiveKind(FT);
+  constexpr uint32_t EPV = (BT == DGB_FLOAT64) ? 2u : (BT == DGB_FLOAT32 || NARROW) ? 4u : 8u;  // input elements per 16 B vector
+  constexpr uint32_t WB = 16u / EPV;                                                           // input word bytes
   // shuffle => the histogram base is provably warp-uniform (ATOMS [R + UR], no per-symbol add)
   const uint32_t t = threadIdx.x, warp = __shfl_sync(0xffffffffu, t >> 5, 0);
   const uint8_t* in = static_cast<const uint8_t*>(md.in);
   const uint32_t size = md.size;  // float words
   uint8_t* archive = static_cast<uint8_t*>(md.out);
   uint8_t* non = archive + kFloatHeaderBytes;
-  const uint32_t nonBytes = floatNonCompBytes(FT, size);
+  const uint32_t nonBytes = floatNonCompBytes(AT, size);
   uint8_t* ansArchive = non + nonBytes;
 
   const uint32_t head = floatHeadLen(in, size, WB);
@@ -714,7 +750,7 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
       if (t == 0) {
         // float-level checksum is patched in by the epilogue CTA
         *reinterpret_cast<uint4*>(archive) =
-            make_uint4(kFloatMagicVersion, size, (uint32_t)FT | ((useChecksum ? 1u : 0u) << 4), 0u);
+            make_uint4(kFloatMagicVersion, size, (uint32_t)AT | ((useChecksum ? 1u : 0u) << 4), 0u);
       }
       if (FT == DGB_FLOAT64) {
         const uint32_t p16 = floatU16PlaneOffset<uint32_t>(FT, size), p8 = floatU8PlaneOffset<uint32_t>(FT, size);
@@ -729,7 +765,14 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
         for (uint32_t i = size + t; i < nonBytes; i += kStatsThreads) non[i] = 0;
       }
     }
-    if (useChecksum) {
+    if (NARROW && useChecksum) {
+      // the same rule over the ROUNDED data: its first size / 2 16-bit words, then the low byte of the next
+      // one when size is odd (foldXor folds both bytes of a word into the byte checksum)
+      const uint32_t* in32 = reinterpret_cast<const uint32_t*>(in);
+      for (uint32_t j = y * kStatsThreads + t; j < (size >> 1); j += participants * kStatsThreads)
+        xorAcc ^= narrowWord<FT>(in32[j]);
+      if ((size & 1u) && y == 0 && t == 0) xorAcc ^= narrowWord<FT>(in32[size >> 1]) & 0xffu;
+    } else if (useChecksum) {
       // SURVEY A.6 / B6: the float checksum covers the first `size` BYTES only (fp64: the first size / 8 words)
       const uint32_t cbytes = size;  // bytes, not words
       for (uint32_t i = y * kStatsThreads + t; i < cbytes; i += participants * kStatsThreads)
@@ -748,7 +791,7 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
   if (size == 0) {
     if (t == 0) {
       *reinterpret_cast<uint4*>(archive) =
-          make_uint4(kFloatMagicVersion, 0u, (uint32_t)FT | ((useChecksum ? 1u : 0u) << 4), 0u);
+          make_uint4(kFloatMagicVersion, 0u, (uint32_t)AT | ((useChecksum ? 1u : 0u) << 4), 0u);
     }
     publishEmptyMember(ansArchive, pb, false, outSize, m, kFloatHeaderBytes + nonBytes);
     return true;
@@ -1011,6 +1054,40 @@ struct EncIn<kKindF32> {
   }
 };
 
+// Narrowing kinds: float32 words in the ring (fp32's geometry, 2 KiB per group of 16 rows), each rounded to the
+// archive type's 16-bit word before the archive type's own coded-byte and stored-byte rules apply.  loadWord
+// returns the rounded word, so the scalar paths use the 16-bit kind's tabOffsetOf and storeScalar unchanged.
+template <int KIND>
+struct EncInNarrow : EncIn16<archiveKind(KIND)> {
+  static constexpr int AT = archiveKind(KIND);
+  static constexpr uint32_t kWordBytes = 4, kRingSlots = 3;
+  template <int J, uint32_t STRIDE>
+  static __device__ __forceinline__ uint32_t tabOffset(uint32_t ringLane) {
+    uint32_t w;
+    asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(w) : "r"(ringLane), "n"(J * 128));
+    return EncIn16<AT>::template tabOffsetOf<STRIDE>(narrowWord<KIND>(w));
+  }
+  static __device__ __forceinline__ uint32_t loadWord(const uint8_t* in, uint32_t e) {
+    return narrowWord<KIND>(__ldg(reinterpret_cast<const uint32_t*>(in) + e));
+  }
+  // one group of 16 rows = 512 words = 2 KiB in the ring slot: lane l handles vectors l + 32 h, as fp32 does, so
+  // every shared load is conflict-free; a vector's four words round to two pairs whose stored bytes are one
+  // 4 B store, and the warp's 32 stores of a step cover 128 contiguous bytes of the plane
+  static __device__ __forceinline__ void storeGroup(uint32_t slot, const StoredPlanes& pl, uint32_t elem0,
+                                                    uint32_t lane) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const uint32_t v = lane + 32u * h;
+      uint4 x;
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w) : "r"(slot + v * 16u));
+      const uint32_t r0 = rot16x2<AT>(narrowPair<KIND>(x.x, x.y)), r1 = rot16x2<AT>(narrowPair<KIND>(x.z, x.w));
+      *reinterpret_cast<uint32_t*>(pl.non + elem0 + v * 4u) = __byte_perm(r0, r1, 0x6420);
+    }
+  }
+};
+template <> struct EncIn<kKindF32toF16> : EncInNarrow<kKindF32toF16> {};
+template <> struct EncIn<kKindF32toBF16> : EncInNarrow<kKindF32toBF16> {};
+
 // Sparse fp32: a +0 / -0 word looks up table entry 256 / 257, every other word its exponent symbol.  The kept words'
 // 16 + 8 stored bits are compacted into the u16 and u8 planes in element order.  A group of 16 rows (512 words in the
 // ring slot) goes in two steps: lane l takes words 16 l .. 16 l + 15 and one warp scan of the lanes' kept counts
@@ -1190,7 +1267,8 @@ __host__ __device__ constexpr uint32_t encRingBytes(int kind) {  // sparse fp32:
          : kind == kKindF64 ? (uint32_t)DGB_ENC_RING64 * kEncGroupRows * 256u
          : kind == kKindBytes
              ? 4u * kEncGroupRows * 32u
-             : (kind == kKindF32 ? 3u * kEncGroupRows * 128u : (uint32_t)DGB_ENC_RING16 * kEncGroupRows * 64u);
+             : (kind == kKindF32 || isNarrowKind(kind) ? 3u * kEncGroupRows * 128u
+                                                       : (uint32_t)DGB_ENC_RING16 * kEncGroupRows * 64u);
 }
 
 // One rANS step for a full row (ans/GpuANSEncode.cuh:49-90 restated).  The
@@ -1642,7 +1720,7 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
       extraBytes = sparsePlanes<KIND>(md.out, size, planes);
       ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
     } else {
-      extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
+      extraBytes = kFloatHeaderBytes + floatNonCompBytes(archiveKind(kind), size);
       ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
       planes.non = static_cast<uint8_t*>(md.out) + kFloatHeaderBytes;
       if (kind == kKindF64) {
@@ -1798,7 +1876,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
     extraBytes = sparsePlanes<KIND>(md.out, size, planes);
     ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
   } else {
-    extraBytes = kFloatHeaderBytes + floatNonCompBytes(kind, size);
+    extraBytes = kFloatHeaderBytes + floatNonCompBytes(archiveKind(kind), size);
     ansOut = static_cast<uint8_t*>(md.out) + extraBytes;
     planes.non = static_cast<uint8_t*>(md.out) + kFloatHeaderBytes;
     if (kind == kKindF64) {
@@ -2083,6 +2161,16 @@ ScratchPlan planScratch(int kind, uint32_t n, uint32_t maxSize, uint32_t totalTi
 
 uint32_t ticketsFor(uint32_t size) { return divUp(size, kBlockBytes); }
 
+// withKind plus the encoder-only narrowing kinds (their kernels are instantiated here and nowhere else)
+template <class F>
+int withEncodeKind(int kind, F&& f) {
+  switch (kind) {
+    case kKindF32toF16: return f(IntC<kKindF32toF16>{});
+    case kKindF32toBF16: return f(IntC<kKindF32toBF16>{});
+    default: return withKind(kind, f);
+  }
+}
+
 // fp64 staging slot of the fast coder: the smallest the coder allows.  The fp64 ring is 12 KiB per warp, and a
 // smaller slot is what lets a second 8-warp CTA fit on an SM; fp64's coded byte (the high exponent byte)
 // compresses so well that a block rarely emits more than the slot holds (those that do spill, see Spill).
@@ -2107,10 +2195,10 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   const uint32_t W = (uint32_t)std::max(1, std::min(opt.encode_warps, 8));  // warps per CTA (two-kernel path)
   const uint32_t elemBytes = wordBytes(kind);
   const bool canonical = opt.encode_canonical != 0;
-  // the sparse kinds have neither the fused launch nor the staged statistics kernel: those options run the
-  // default kernels for them (INTEGRATION.md section 4)
-  const bool sparse = isSparseKind(kind);
-  const bool fused = !canonical && opt.encode_fused != 0 && !sparse;
+  // the sparse and the narrowing kinds have neither the fused launch nor the staged statistics kernel: those
+  // options run the default kernels for them (INTEGRATION.md section 4)
+  const bool defaultOnly = isSparseKind(kind) || isNarrowKind(kind);
+  const bool fused = !canonical && opt.encode_fused != 0 && !defaultOnly;
   // staging slot of the fast / fused encoder (spills to global scratch when a block needs more)
   uint32_t slotWords = opt.encode_slot_words > 0 ? (uint32_t)opt.encode_slot_words
                                                  : (kind == kKindBytes ? 2304u : (kind == kKindF64 ? kEncSlotWordsF64 : 1536u));
@@ -2143,7 +2231,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     if (reinterpret_cast<uintptr_t>(hm.in) & (elemBytes - 1u)) return DGB_ERR_INVALID_ARG;
     // the reference refuses members whose worst-case archive does not fit 32 bits
     // (ans/GpuANSEncode.cu:13-25 CHECK_LE(rawSize, INT32_MAX)): the caller cannot have sized `out`
-    if ((kind == kKindBytes ? dgb_ans_max_compressed_size(hm.size) : dgb_float_max_compressed_size(kind, hm.size)) == 0u)
+    if ((kind == kKindBytes ? dgb_ans_max_compressed_size(hm.size) : dgb_float_max_compressed_size(archiveKind(kind), hm.size)) == 0u)
       return DGB_ERR_TOO_LARGE;
     desc[i].in = hm.in;
     desc[i].out = hm.out;
@@ -2179,7 +2267,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   sc.spill = base + sp.spill;
   sc.table = reinterpret_cast<uint4*>(base + sp.table);
   sc.blockZerosOff = sp.blockZerosOff;
-  const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0 && !sparse;
+  const bool stagedK1 = kind != kKindBytes && opt.stats_stage != 0 && !defaultOnly;
 
   // member table: inside the kernel parameters when it fits and the default kernels run, else uploaded to scratch
   static thread_local InlineMembers im;
@@ -2194,10 +2282,11 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   DGB_CUDA_TRY(cudaMemsetAsync(base + sp.zeroBegin, 0, (canonical ? sp.lookbackEnd : sp.zeroEnd) - sp.zeroBegin, stream));
 
   const int sms = smCount();
-  // encoder table format (see EncSym in this file): wide entries for exponent-byte planes
+  // encoder table format (see EncSym in this file): wide entries for exponent-byte planes (by the archive type)
+  const int ak = archiveKind(kind);
   const bool wideTable = !canonical && opt.encode_wide_table != 0 &&
-                         (opt.encode_wide_table > 0 || kind == DGB_BFLOAT16 || kind == DGB_FLOAT32 || kind == DGB_FLOAT64 ||
-                          kind == DGB_BFLOAT16_SPARSE || kind == DGB_FLOAT32_SPARSE);
+                         (opt.encode_wide_table > 0 || ak == DGB_BFLOAT16 || ak == DGB_FLOAT32 || ak == DGB_FLOAT64 ||
+                          ak == DGB_BFLOAT16_SPARSE || ak == DGB_FLOAT32_SPARSE);
   sc.wideTable = wideTable;
 
   if (fused) {
@@ -2237,7 +2326,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   // K2 launch configuration (same for every part)
   const size_t smemBytes = (size_t)W * (canonical ? encWarpSmem(pb, kind) : encFastWarpSmem(slotWords, kind));
 
-  return withKind(kind, [&](auto K) { return withBool(wideTable, [&](auto WD) {
+  return withEncodeKind(kind, [&](auto K) { return withBool(wideTable, [&](auto WD) {
     constexpr int KIND = decltype(K)::value;
     constexpr bool WIDE = decltype(WD)::value;
     // K2: the canonical coder (ordered, packed table; wideTable is false) or the fast coder
@@ -2271,7 +2360,7 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
       timerBegin(opt, kSlotStats, ps);
       if constexpr (KIND == kKindBytes) {
         statsBytesKernel<<<grid1, kStatsThreads, 0, ps>>>(sc, im, histogram_dev, pb, checksum, slabVecs, m0, outSize_dev);
-      } else if constexpr (isSparseKind(KIND)) {
+      } else if constexpr (isSparseKind(KIND) || isNarrowKind(KIND)) {
         statsFloatKernel<KIND><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
       } else if (stagedK1 && gridY * (uint64_t)slabVecsK1 >= maxVecs) {
         rc = residentCtasPerSm((const void*)statsFloatStagedKernel<KIND>, kStatsThreads, 0, 128 * 1024, nullptr);

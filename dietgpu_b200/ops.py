@@ -159,10 +159,36 @@ def _validate_out(out_compressed, out_sizes, n: int, cols: int, dev):
     return comp, sizes
 
 
+_NARROW_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16}
+
+
+def _narrow_type(compress_as_float: bool, ts_in: Sequence[torch.Tensor], sparse: bool,
+                 archive_dtype: Optional[torch.dtype]) -> Optional[int]:
+    """The archive float type of a narrowing compress, or None for an ordinary one (archive_dtype None or the
+    inputs' dtype).  Decided from dtypes alone, before any tensor is touched."""
+    if archive_dtype is None or (len(ts_in) > 0 and archive_dtype == ts_in[0].dtype):
+        return None
+    if not compress_as_float or sparse or len(ts_in) == 0 or ts_in[0].dtype != torch.float32 \
+            or archive_dtype not in _NARROW_TYPES:
+        raise ValueError("compress_data: archive_dtype narrows float32 inputs to float16 or bfloat16 archives "
+                         "(compress_as_float=True, sparse=False); got "
+                         f"{ts_in[0].dtype if len(ts_in) else None} inputs, archive_dtype={archive_dtype}, "
+                         f"compress_as_float={compress_as_float}, sparse={sparse}")
+    return _NARROW_TYPES[archive_dtype]
+
+
 def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checksum: bool = False,
                   temp_mem: Optional[torch.Tensor] = None, out_compressed: Optional[torch.Tensor] = None,
                   out_compressed_bytes: Optional[torch.Tensor] = None, *,
-                  prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False):
+                  prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False,
+                  archive_dtype: Optional[torch.dtype] = None):
+    """archive_dtype (float16 / bfloat16, with float32 inputs): narrowing compress (dgb_float_compress_to).
+    Every member's archive is exactly the archive of t.to(archive_dtype) (torch's CUDA cast), with rows sized by
+    that type's bound, and no 16-bit temporary is made.  None, or the inputs' dtype, is the ordinary call; any
+    other combination raises ValueError."""
+    narrow = _narrow_type(compress_as_float, ts_in, sparse, archive_dtype)
+    if narrow is not None:
+        return _compress_narrow(ts_in, narrow, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits)
     _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0, "empty batch")
     dev = ts_in[0].device
@@ -193,6 +219,28 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
             tmp = _Temp(temp_mem, need, dev)
             rc = L.dgb_ans_encode_pointer(tmp.ptr, tmp.bytes, prob_bits, int(checksum), n, in_ptrs,
                                           in_sizes, None, out_ptrs, sizes.data_ptr(), _stream())
+    capi.check(rc, "compress_data")
+    return comp, sizes, tmp.need
+
+
+def _compress_narrow(ts_in, ft: int, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits):
+    dev = ts_in[0].device
+    for t in ts_in:
+        _check(t.is_cuda and t.is_contiguous() and t.device == dev and t.dtype == torch.float32)
+    n = len(ts_in)
+    mx, _ = _max_numel_and_bytes(ts_in)
+    L = capi.lib()
+    cols = _bound(L.dgb_float_max_compressed_size(ft, mx), mx)
+    comp, sizes = _validate_out(out_compressed, out_compressed_bytes, n, cols, dev)
+    row = comp.size(1)
+    with torch.cuda.device(dev):
+        need = L.dgb_float_compress_temp_bytes(ft, n, mx)
+        tmp = _Temp(temp_mem, need, dev)
+        rc = L.dgb_float_compress_to(tmp.ptr, tmp.bytes, capi.FLOAT32, ft, prob_bits, int(checksum), n,
+                                     capi.ptr_array([t.data_ptr() for t in ts_in]),
+                                     capi.u32_array([t.numel() for t in ts_in]),
+                                     capi.ptr_array([comp.data_ptr() + i * row for i in range(n)]),
+                                     sizes.data_ptr(), _stream())
     capi.check(rc, "compress_data")
     return comp, sizes, tmp.need
 

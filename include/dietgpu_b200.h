@@ -174,6 +174,24 @@ int dgb_float_compress_pointer(void* temp_dev, size_t temp_bytes, int float_type
                                const uint32_t* in_size, void* const* out, uint32_t* out_size_dev,
                                void* stream);
 
+/* Compress with a narrowing cast (new; no reference counterpart).  The allowed pairs (in_float_type, float_type)
+ * are (DGB_FLOAT16, DGB_FLOAT16), (DGB_BFLOAT16, DGB_BFLOAT16) and (DGB_FLOAT32, DGB_FLOAT32), which are exactly
+ * dgb_float_compress_pointer, and the narrowing pairs (DGB_FLOAT32, DGB_FLOAT16) and (DGB_FLOAT32, DGB_BFLOAT16);
+ * any other pair returns DGB_ERR_INVALID_ARG before any CUDA call.
+ * Narrowing: in[i] holds in_size[i] float32 words (4 B aligned), and out[i] receives exactly the archive
+ * dgb_float_compress_pointer(float_type, ...) writes for r = the words rounded to float_type, round to nearest
+ * even as torch's CUDA cast rounds (cvt.rn.f16.f32 / cvt.rn.bf16.f32, NaNs included):
+ * the same size, header, pdf, lane states, block table and streams (with encode_canonical = 1 the same bytes;
+ * by default the streams are in completion order, as for every type), and the checksum of r (its first
+ * in_size[i] bytes).  The archive is an ordinary float_type archive: every decoder, the decode-and-sum and the
+ * reference read it.  No temporary of r exists; the input is not modified.  out[i] must hold
+ * dgb_float_max_compressed_size(float_type, in_size[i]) bytes, the scratch is
+ * dgb_float_compress_temp_bytes(float_type, n, max in_size), and the refusals and error codes are
+ * dgb_float_compress_pointer's.  Never synchronises; capturable into a CUDA graph. */
+int dgb_float_compress_to(void* temp_dev, size_t temp_bytes, int in_float_type, int float_type, int prob_bits,
+                          int use_checksum, uint32_t num_in_batch, const void* const* in, const uint32_t* in_size,
+                          void* const* out, uint32_t* out_size_dev, void* stream);
+
 /* float/GpuFloatCodec.h:141-170 / float/GpuFloatCompress.cu:103-159 floatCompressSplitSize. */
 int dgb_float_compress_split_size(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
                                   int use_checksum, uint32_t num_in_batch, const void* in_dev,
