@@ -326,10 +326,25 @@ def _check_wire(t: torch.Tensor, what: str, wire_dtype: Optional[torch.dtype]) -
                          f"not {wire_dtype} for {t.dtype}")
 
 
+def _check_sparse_wire(dtype: torch.dtype, what: str, sparse: bool, wire_dtype: Optional[torch.dtype] = None,
+                       peer: Optional[PeerWorkspace] = None) -> None:
+    """sparse=True: sparse fp16 / bf16 / fp32 archives on the NCCL / gloo transport, without narrowing."""
+    if not sparse:
+        return
+    if dtype not in _REDUCE_DTYPES:
+        raise ValueError(f"{what}: sparse=True needs a float16, bfloat16 or float32 tensor, not {dtype}")
+    if wire_dtype is not None:
+        raise ValueError(f"{what}: sparse=True cannot be combined with wire_dtype (there is no narrowing compress "
+                         "into sparse archives)")
+    if peer is not None:
+        raise ValueError(f"{what}: sparse=True is not supported with the peer-memory transports")
+
+
 def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, stages: int = 2,
                           peer: Optional[PeerWorkspace] = None, check: bool = True,
-                          peer_mode: str = "auto", wire_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                          peer_mode: str = "auto", wire_dtype: Optional[torch.dtype] = None,
+                          sparse: bool = False) -> torch.Tensor:
     """Every rank contributes the CUDA tensor `t` (same shape and dtype on every rank; fp16 / bf16 / fp32 go
     through the float codec, anything else through the byte codec) and receives the concatenation
     [world * t.numel()] in rank order, bit-exact.  `members` = archives per rank (the codec's parallelism
@@ -344,7 +359,13 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
     wire_dtype=torch.float16 / torch.bfloat16 with a float32 t (fp32 master weights gathered as 16-bit
     parameters, FSDP's param_dtype): each member is rounded to wire_dtype inside the compress kernels, the 16-bit
     archives go over the wire, and the result has wire_dtype and equals cat([t_r.to(wire_dtype) for every rank r])
-    bit for bit.  NCCL / gloo transport only: with `peer` it raises ValueError."""
+    bit for bit.  NCCL / gloo transport only: with `peer` it raises ValueError.
+
+    sparse=True (float16 / bfloat16 / float32 t): the archives are sparse ones (ops.compress_data(sparse=True)),
+    which store no bits for +0 and -0 words, so mostly-zero tensors (ReLU activations, pruned weights) take fewer
+    bytes on the wire; the result is the same, bit for bit.  NCCL / gloo transport only, and not with wire_dtype:
+    either raises ValueError before any communication."""
+    _check_sparse_wire(t.dtype, "all_gather_compressed", sparse, wire_dtype, peer)
     if not t.is_cuda or not t.is_contiguous():
         raise ValueError("all_gather_compressed: contiguous CUDA tensor expected (no CPU fallback)")
     _check_wire(t, "all_gather_compressed", wire_dtype)
@@ -377,7 +398,7 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
 
     def compress(a, b):
         comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem,
-                                           archive_dtype=wire_dtype)
+                                           archive_dtype=wire_dtype, sparse=sparse)
         return comp, sizes
 
     def decompress(a, b, gathered):
@@ -388,7 +409,7 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
                 outs.append(out[w * n + bounds[i]: w * n + bounds[i + 1]])
         # gathered views are 16 B aligned inside the receive buffer; the decoder needs nothing else
         status = torch.zeros(len(ins), dtype=torch.uint8, device=t.device)
-        ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status)
+        ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status, sparse=sparse)
         return status
 
     statuses = []
@@ -452,15 +473,17 @@ def _all_to_all_bytes(send: torch.Tensor, send_sizes: List[int], recv_sizes: Lis
 
 def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, peer: Optional[PeerWorkspace] = None,
-                          check: bool = True, peer_mode: str = "pull") -> List[torch.Tensor]:
+                          check: bool = True, peer_mode: str = "pull", sparse: bool = False) -> List[torch.Tensor]:
     """chunks[d] (CUDA, contiguous, same dtype and shape on every rank for a given (source, destination) pair is
     NOT required: sizes travel with the data) goes to rank d; returns [world] tensors, entry s = what rank s
     sent here, bit-exact.  One archive per destination; the payload moves with all_to_all_single and exact
-    split sizes, so each link carries only its own compressed chunk."""
+    split sizes, so each link carries only its own compressed chunk.  sparse=True (float16 / bfloat16 / float32
+    chunks, NCCL / gloo transport): sparse archives on the wire, as in all_gather_compressed; same result."""
     world = _world(group)
     if len(chunks) != world:
         raise ValueError("all_to_all_compressed: one chunk per rank expected")
     dt, dev = chunks[0].dtype, chunks[0].device
+    _check_sparse_wire(dt, "all_to_all_compressed", sparse, peer=peer)
     for c in chunks:
         if not c.is_cuda or not c.is_contiguous() or c.dtype != dt or c.device != dev:
             raise ValueError("all_to_all_compressed: contiguous CUDA tensors of one dtype on one device expected")
@@ -469,10 +492,10 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
     if peer is not None:
         outs = _all_to_all_peer(flats, as_float, peer, checksum, temp_mem, check, peer_mode == "direct")
         return [x if as_float else x.view(dt) for x in outs]
-    comp, sizes, _ = ops.compress_data(as_float, flats, checksum, temp_mem)
+    comp, sizes, _ = ops.compress_data(as_float, flats, checksum, temp_mem, sparse=sparse)
     if world == 1:
         out = torch.empty_like(flats[0])
-        ops.decompress_data(as_float, [comp[0, :int(sizes[0])]], [out], checksum, temp_mem)
+        ops.decompress_data(as_float, [comp[0, :int(sizes[0])]], [out], checksum, temp_mem, sparse=sparse)
         return [out.view(chunks[0].shape) if as_float else out.view(dt).view(chunks[0].shape)]
     on_device = _device_collectives(group)
     cdev = dev if on_device else torch.device("cpu")
@@ -497,7 +520,7 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
         outs.append(torch.empty(elems, dtype=flats[0].dtype, device=dev))
         o += recv_sizes[s]
     status = torch.zeros(world, dtype=torch.uint8, device=dev)
-    ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status)
+    ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status, sparse=sparse)
     if not bool(status.all()):
         raise RuntimeError("all_to_all_compressed: a received archive failed to decode")
     return [x if as_float else x.view(dt) for x in outs]
@@ -523,7 +546,7 @@ def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dt
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               temp_mem: Optional[torch.Tensor] = None, check: bool = True,
                               reduce_dtype: Optional[torch.dtype] = None,
-                              wire_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                              wire_dtype: Optional[torch.dtype] = None, sparse: bool = False) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -542,7 +565,12 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     communication_data_type, Megatron's bf16 gradient communication): every chunk is rounded to wire_dtype inside
     the compress kernels, the 16-bit archives go over the wire and are summed in fp32, and the float32 result is
     ((t_0.to(w).float() + t_1.to(w).float()) + t_2.to(w).float()) + ... bit for bit, on every rank and for every
-    `members`.  reduce_dtype must then be None or float32."""
+    `members`.  reduce_dtype must then be None or float32.
+
+    sparse=True: sparse archives on the wire (no stored bits for +0 and -0 words), summed by the sparse
+    decode-and-sum (ops.decompress_data_reduce(sparse=True)); the result is the same fold, bit for bit, with
+    reduce_dtype too.  Not with wire_dtype: that raises ValueError before any communication."""
+    _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
     world = _world(group)
@@ -560,7 +588,7 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     dests = [d for d in range(world) if d != rank]
     comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
                                               for d in dests for i in range(m)], False, temp_mem,
-                                       archive_dtype=arch_dtype)
+                                       archive_dtype=arch_dtype, sparse=sparse)
     on_device = _device_collectives(group)
     cdev = dev if on_device else torch.device("cpu")
     hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
@@ -599,13 +627,13 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     else:
         st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
-                                   archive_dtype=arch_dtype)
+                                   archive_dtype=arch_dtype, sparse=sparse)
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st, archive_dtype=arch_dtype)
+                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse)
         statuses.append(st)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
@@ -613,13 +641,16 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
 
 
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
-                          check: bool = True, reduce_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                          check: bool = True, reduce_dtype: Optional[torch.dtype] = None,
+                          sparse: bool = False) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
     for the exchange.  Bit-identical on every rank to the rank-order left fold with torch's adds.
     reduce_dtype=torch.float32 with a float16 / bfloat16 t sums in fp32 as reduce_scatter_compressed does and
-    all-gathers the fp32 shards: the float32 result is the fp32 fold on every rank."""
+    all-gathers the fp32 shards: the float32 result is the fp32 fold on every rank.  sparse=True sends sparse
+    archives in both phases (see reduce_scatter_compressed); the result is the same."""
+    _check_sparse_wire(t.dtype, "all_reduce_compressed", sparse)
     acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
     world = _world(group)
     flat = t.reshape(-1)
@@ -628,6 +659,6 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
         return t.to(acc_dtype, copy=True)
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
-    shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype)
-    full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check)
+    shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse)
+    full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check, sparse=sparse)
     return full[:n].view(t.shape)

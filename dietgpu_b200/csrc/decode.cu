@@ -149,6 +149,13 @@ planKernel(DecodeScratch sc, uint32_t m0, uint32_t m1, uint32_t part, int pb,
 constexpr int kGroupRows = DGB_DEC_GROUP_ROWS;  // rows per prefetch group (8 or 16)
 constexpr uint32_t kRingSlots = 3;              // groups resident per warp: current + 2 in flight
 
+// writer kinds of the decode-and-sum (further down): the archive kind | kAddWriter adds the decoded word to the
+// output's word; | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives (dense or sparse)
+constexpr int kAddWriter = 0x10;
+constexpr int kWidenF32 = 0x20;
+// the archive kind of a decode-and-sum kernel or writer kind
+__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32); }
+
 template <int KIND>
 struct RowWriter;
 
@@ -714,7 +721,7 @@ __device__ __forceinline__ void decodeBlockWarp(uint32_t state, Stream st, uint3
   if (rem) {
     const bool valid = lane < rem;
     const uint32_t e = decodeStepPartial<PB, LUT64>(valid, state, lut, st, geMask);
-    if constexpr (isSparseKind(KIND))
+    if constexpr (isSparseKind(reduceArchiveKind(KIND)))
       wr.writePartial(row, e, valid);  // its ballot needs every lane
     else if (valid)
       wr.writeSlow(row, e);
@@ -1157,18 +1164,16 @@ int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineM
 // Widening sums (dgb_float_decompress_reduce_to): fp16 / bf16 archives summed into fp32 outputs.  The kernel's
 // kind is then the archive kind | kWidenF32; every decoded word is converted exactly to fp32 and each add is one
 // fp32 round-to-nearest-even add, which is torch's acc.float() + x.float() fold.
+// Sparse sums (dgb_float_decompress_reduce_sparse): archives of type 5, 6 or 8 into outputs of the dense type, or
+// types 5 and 6 into fp32.  The kernel's kind is then the sparse kind (| kWidenF32); its writers take each word
+// from the sparse decoder's writer and add it as the dense writers do, so the result is the dense sum of the same
+// words bit for bit.
 // ---------------------------------------------------------------------------
 #ifndef DGB_REDUCE_PASS_ARCHIVES
 #define DGB_REDUCE_PASS_ARCHIVES 4
 #endif
 constexpr uint32_t kReducePass = DGB_REDUCE_PASS_ARCHIVES;
 constexpr int kReduceWarps = 8;
-// writer kinds of the decode-and-sum: the dense kind | kAddWriter adds the decoded word to the output's word;
-// | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives
-constexpr int kAddWriter = 0x10;
-constexpr int kWidenF32 = 0x20;
-// the archive kind of a decode-and-sum kernel or writer kind
-__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32); }
 
 template <int KIND>
 __device__ __forceinline__ uint32_t addWord(uint32_t a, uint32_t b) {
@@ -1307,6 +1312,68 @@ template <> struct RowWriter<kKindBF16 | kWidenF32> : RowWriterWiden16<kKindBF16
 template <> struct RowWriter<kKindF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindF16> {};
 template <> struct RowWriter<kKindBF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindBF16> {};
 
+// Sparse decode-and-sum writers (dgb_float_decompress_reduce_sparse): the sparse kind's word (its ring, segment copy
+// or windows, and kept-word cursor), then the dense kind's add, widening or widening add.  An elided word is the +0
+// or -0 it stands for and goes through the add like any other (-0 + -0 = -0, -0 + +0 = +0).  word() votes across
+// the warp, so every row, the partial one too, runs on the whole warp.  WK = the sparse kind | kAddWriter and / or
+// | kWidenF32 (fp32 outputs of types 5 and 6); the plain store of archive 0 is the sparse decoder's own writer.
+template <int WK>
+struct RowWriterSparseReduce : RowWriter<reduceArchiveKind(WK)> {
+  typedef RowWriter<reduceArchiveKind(WK)> B;
+  static constexpr int BT = denseKind(reduceArchiveKind(WK));
+  static constexpr bool kAdd = (WK & kAddWriter) != 0, kWiden = (WK & kWidenF32) != 0;
+  static constexpr int kSumKind = kWiden ? kKindF32 : BT;  // the output words' type, in which the adds are taken
+  typedef typename std::conditional<kSumKind == kKindF32, uint32_t, uint16_t>::type T;
+  T* sum;
+  struct Cursor { T* o; uint32_t prev[kGroupRows]; };
+  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
+    B::setBlock(av, outBase, block, l);
+    sum = static_cast<T*>(outBase) + (size_t)block * kBlockBytes + l;
+    __builtin_assume(__isGlobal(sum));
+  }
+  static __device__ __forceinline__ uint32_t value(uint32_t w) {
+    if constexpr (kWiden) return widenWord<BT>(w);
+    else return w;
+  }
+  // the output word from the running sum `prev` (ignored by the store writer) and the decoded word `w`
+  static __device__ __forceinline__ T combine(uint32_t prev, uint32_t w) {
+    if constexpr (kAdd) return (T)addWord<kSumKind>(prev, value(w));
+    else return (T)value(w);
+  }
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t) const {
+    Cursor c;
+    c.o = sum + row * 32u;
+    if constexpr (kAdd) {
+#pragma unroll
+      for (int j = 0; j < kGroupRows; ++j)
+        c.prev[j] = sizeof(T) == 4 ? ldGlobalU32(reinterpret_cast<const uint32_t*>(c.o + j * 32))
+                                   : ldGlobalU16(reinterpret_cast<const uint16_t*>(c.o + j * 32));
+    }
+    return c;
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    const uint32_t w = B::word(entry, true);
+    if constexpr (kAdd) c.o[J * 32] = combine(c.prev[J], w);
+    else c.o[J * 32] = combine(0u, w);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
+  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
+    const uint32_t w = B::word(entry, valid);
+    if (valid) {
+      T* o = sum + row * 32u;
+      *o = combine(kAdd ? (uint32_t)*o : 0u, w);
+    }
+  }
+};
+template <> struct RowWriter<kKindF16S | kAddWriter> : RowWriterSparseReduce<kKindF16S | kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kAddWriter> : RowWriterSparseReduce<kKindBF16S | kAddWriter> {};
+template <> struct RowWriter<kKindF32S | kAddWriter> : RowWriterSparseReduce<kKindF32S | kAddWriter> {};
+template <> struct RowWriter<kKindF16S | kWidenF32> : RowWriterSparseReduce<kKindF16S | kWidenF32> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32> : RowWriterSparseReduce<kKindBF16S | kWidenF32> {};
+template <> struct RowWriter<kKindF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindF16S | kWidenF32 | kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindBF16S | kWidenF32 | kAddWriter> {};
+
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
 // consistent with its word count, and that word count is the group's output size.
 template <int KIND, int PB>
@@ -1339,7 +1406,13 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
     const uint32_t streamBytes = roundUp(words, 8u) * 2u;
     __syncwarp();
     if (lane == 0) {
-      mbarExpectTx(myBar, 128u + streamBytes);
+      if constexpr (copiesSegment(reduceArchiveKind(WK))) {
+        // sparse fp16 / bf16: the block's stored bytes ride on the same mbarrier (decodeFusedKernel)
+        mbarExpectTx(myBar, 128u + streamBytes + wr.bulkBytes());
+        wr.bulkIssue(myBar);
+      } else {
+        mbarExpectTx(myBar, 128u + streamBytes);
+      }
       bulkLoad(smemAddr(mySlot), pStates + 128u * (size_t)block, 128u, myBar);
       if (streamBytes) bulkLoad(smemAddr(mySlot + 128), stream, streamBytes, myBar);
     }
@@ -1349,6 +1422,7 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
     SmemStream st{smemAddr(mySlot + 128) + 2u * words};
     decodeBlockWarp<WK, PB, false>(state, st, blockLen, lut, wr, lane);
   } else {
+    if constexpr (copiesSegment(reduceArchiveKind(WK))) wr.copySync();
     const uint32_t state = __ldg(reinterpret_cast<const uint32_t*>(pStates) + block * 32u + lane);
     GmemStream st{stream + words};
     decodeBlockWarp<WK, PB, false>(state, st, blockLen, lut, wr, lane);
@@ -1638,11 +1712,13 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
-                 uint8_t* outSuccess_dev, cudaStream_t stream) {
-  if (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32) return DGB_ERR_INVALID_ARG;
-  // outputs of the archive kind, or fp32 sums of fp16 / bf16 archives
-  const bool widen = outKind != kind;
-  if (widen && !(outKind == kKindF32 && (kind == kKindF16 || kind == kKindBF16))) return DGB_ERR_INVALID_ARG;
+                 uint8_t* outSuccess_dev, bool sparse, cudaStream_t stream) {
+  // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8
+  if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
+  // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
+  const int dk = denseKind(kind);
+  const bool widen = outKind != dk;
+  if (widen && !(outKind == kKindF32 && (dk == kKindF16 || dk == kKindBF16))) return DGB_ERR_INVALID_ARG;
   if (pb < 9 || pb > 11 || width == 0) return DGB_ERR_INVALID_ARG;
   if (groups == 0) return DGB_OK;
   if (!in || !out || !outSize) return DGB_ERR_INVALID_ARG;
@@ -1686,13 +1762,14 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   }
   return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
     constexpr int KIND = decltype(K)::value;
-    if constexpr (KIND == kKindF16 || KIND == kKindBF16) {
+    constexpr int DK = denseKind(KIND);
+    if constexpr (DK == kKindF16 || DK == kKindBF16) {
       if (widen)
         return launchDecodeReduce<KIND | kWidenF32, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
                                                                        accumulate, outSuccess_dev, stream);
       return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
                                                          outSuccess_dev, stream);
-    } else if constexpr (KIND == kKindF32)
+    } else if constexpr (DK == kKindF32)
       return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
                                                          outSuccess_dev, stream);
     else

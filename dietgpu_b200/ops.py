@@ -400,7 +400,7 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                            accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
                            out_status: Optional[torch.Tensor] = None, *,
                            prob_bits: int = K_DEFAULT_PRECISION,
-                           archive_dtype: Optional[torch.dtype] = None) -> int:
+                           archive_dtype: Optional[torch.dtype] = None, sparse: bool = False) -> int:
     """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
@@ -411,7 +411,11 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     archive_dtype: the archives' dtype; None (or the outputs' dtype) means the outputs' dtype.  float16 or
     bfloat16 archives with float32 outputs are summed in float32: the result is
     torch's fold acc = x(g, 0).float(); acc = acc + x(g, 1).float(); ... bit for bit.  Any other pair raises
-    ValueError."""
+    ValueError.
+
+    sparse=True: the archives were made with compress_data(..., sparse=True) from archive_dtype tensors
+    (dgb_float_decompress_reduce_sparse).  The same dtype pairs are allowed, and the result is bit-identical to this
+    call on dense archives of the same words; a dense archive in such a group is invalid."""
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
@@ -436,16 +440,17 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
             ins.append(ti)
     g, n = len(ts_out), len(ins)
     st_ptr, _ = _validate_status(out_status, None, n, dev)
-    ft, out_ft = _REDUCE_TYPES[archive_dtype], _REDUCE_TYPES[dtype]
+    ft, out_ft = (_SPARSE_TYPES if sparse else _REDUCE_TYPES)[archive_dtype], _REDUCE_TYPES[dtype]
     L = capi.lib()
+    entry = L.dgb_float_decompress_reduce_sparse if sparse else L.dgb_float_decompress_reduce_to
     with torch.cuda.device(dev):
         need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
         tmp = _Temp(temp_mem, need, dev)
-        rc = L.dgb_float_decompress_reduce_to(tmp.ptr, tmp.bytes, ft, out_ft, prob_bits, g, width,
-                                              capi.ptr_array([t.data_ptr() for t in ins]),
-                                              capi.ptr_array([t.data_ptr() for t in ts_out]),
-                                              capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
-                                              st_ptr, _stream())
+        rc = entry(tmp.ptr, tmp.bytes, ft, out_ft, prob_bits, g, width,
+                   capi.ptr_array([t.data_ptr() for t in ins]),
+                   capi.ptr_array([t.data_ptr() for t in ts_out]),
+                   capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
+                   st_ptr, _stream())
     capi.check(rc, "decompress_data_reduce")
     return tmp.need
 

@@ -250,6 +250,21 @@ int dgb_float_decompress_reduce_to(void* temp_dev, size_t temp_bytes, int float_
                                    const void* const* in, void* const* out, const uint32_t* out_size,
                                    int accumulate, uint8_t* out_success_dev, void* stream);
 
+/* Decode-and-sum of sparse archives (new; no reference counterpart).  The allowed pairs (float_type,
+ * out_float_type) are (DGB_FLOAT16_SPARSE, DGB_FLOAT16), (DGB_BFLOAT16_SPARSE, DGB_BFLOAT16),
+ * (DGB_FLOAT32_SPARSE, DGB_FLOAT32), (DGB_FLOAT16_SPARSE, DGB_FLOAT32) and (DGB_BFLOAT16_SPARSE, DGB_FLOAT32); any
+ * other pair returns DGB_ERR_INVALID_ARG.  For every input the result is bit-identical to
+ * dgb_float_decompress_reduce_to(float_type's dense type, out_float_type) on dense archives of the same words:
+ * an elided word is the +0 or -0 it stands for and is added as such.  An archive is valid when its headers have
+ * float_type (a dense archive in a sparse group is invalid) and prob_bits, a consistent block count and exactly
+ * out_size[g] words.  Everything else is as in dgb_float_decompress_reduce_to: the sum order, statuses, groups
+ * with an invalid archive left unwritten, no synchronisation, graph capture, num_groups = 0 returning DGB_OK and
+ * the scratch size dgb_float_decompress_temp_bytes(float_type, G * W, 0). */
+int dgb_float_decompress_reduce_sparse(void* temp_dev, size_t temp_bytes, int float_type, int out_float_type,
+                                       int prob_bits, uint32_t num_groups, uint32_t archives_per_group,
+                                       const void* const* in, void* const* out, const uint32_t* out_size,
+                                       int accumulate, uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

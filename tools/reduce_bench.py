@@ -1,6 +1,6 @@
 """Decode-and-sum (ops.decompress_data_reduce) against decoding the same archives separately, on one GPU.
 
-    python tools/reduce_bench.py [--iters 30] [--json out.json] [--reduce-dtype float32]
+    python tools/reduce_bench.py [--iters 30] [--json out.json] [--reduce-dtype float32] [--sparse]
 
 For each shape (G groups x W archives x N words of N(0,1) data, seeded) three ways are timed on the same archives,
 alternating within the run:
@@ -12,6 +12,8 @@ algorithmic bytes over kernel time as a share of the H100 SXM data sheet's 3.35 
 once + outputs written once: G * N words for (1), G * W * N for (2)).  (1)'s result is checked bit for bit against
 (3)'s.  The card name and power limit are read in the same run; DIETGPU_B200_LIB selects an experiment build of
 the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_ARCHIVES=2).
+
+--sparse: sparse against dense decode-and-sum (bench_sparse) at zero fractions 0 %, ReLU (about 50 %), 90 % and 99 %.
 """
 import argparse
 import json
@@ -178,16 +180,82 @@ def bench32(dtype, groups, width, n, iters):
     return r
 
 
+SPARSE_SHAPES = [s for s in SHAPES if s[1:] != (8, 7, 4 << 20)]
+ZEROS = ["0", "relu", "0.9", "0.99"]
+
+
+def sparse_data(dtype, n, zeros, g):
+    x = torch.randn(n, generator=g, device="cuda")
+    if zeros == "relu":
+        x = x.clamp_min(0)
+    elif zeros != "0":
+        x[torch.rand(n, generator=g, device="cuda") < float(zeros)] = 0
+    return x.to(dtype)
+
+
+def bench_sparse(dtype, groups, width, n, iters, zeros, out_dtype):
+    """The same words as sparse and as dense archives: (1) decompress_data_reduce(sparse=True), (2) the dense call.
+    Reported: call and kernel time of both, and the bytes on the wire (the summed archive sizes)."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [sparse_data(dtype, n, zeros, g) for _ in range(groups * width)]
+    arch = {}
+    for sp in (True, False):
+        comp, sizes, _ = ops.compress_data(True, xs, sparse=sp)
+        hs = sizes.cpu().tolist()
+        arch[sp] = ([comp[i, :hs[i]].clone() for i in range(len(xs))], sum(hs))
+        del comp
+    del xs
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    outs = {sp: [torch.empty(n, dtype=out_dtype, device="cuda") for _ in range(groups)] for sp in (True, False)}
+    calls = {}
+    for sp in (True, False):
+        gi = [arch[sp][0][k * width:(k + 1) * width] for k in range(groups)]
+        calls[sp] = (lambda gi=gi, sp=sp: ops.decompress_data_reduce(gi, outs[sp], False, temp, archive_dtype=dtype,
+                                                                      sparse=sp))
+        calls[sp]()
+    torch.cuda.synchronize()
+    it = torch.int32 if out_dtype == torch.float32 else torch.int16
+    for k in range(groups):
+        assert torch.equal(outs[True][k].view(it), outs[False][k].view(it)), k
+    t = {True: [], False: []}
+    for _ in range(3):  # alternate
+        for sp in (True, False):
+            t[sp].append(timed(calls[sp], iters))
+    kt = {sp: kernel_us(calls[sp], iters) for sp in (True, False)}
+    raw = groups * width * n * torch.empty(0, dtype=dtype).element_size()
+    r = {"shape": f"{str(dtype).split('.')[-1]}->{str(out_dtype).split('.')[-1]} {groups}x{width}x{n}",
+         "zeros": zeros, "wire_MB": {"sparse": arch[True][1] / 1e6, "dense": arch[False][1] / 1e6},
+         "wire_ratio": {"sparse": arch[True][1] / raw, "dense": arch[False][1] / raw},
+         "call_us": {"sparse": min(t[True]), "dense": min(t[False])},
+         "call_us_max": {"sparse": max(t[True]), "dense": max(t[False])},
+         "kernel_us": {"sparse": kt[True], "dense": kt[False]}}
+    r["kernel_sparse_over_dense"] = kt[True] / kt[False]
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--json", default=None)
     ap.add_argument("--reduce-dtype", choices=["same", "float32"], default="same",
                     help="float32: sum the 16-bit shapes' archives into fp32 outputs (bench32)")
+    ap.add_argument("--sparse", action="store_true", help="sparse against dense archives (bench_sparse)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    for shape in (SHAPES32 if args.reduce_dtype == "float32" else SHAPES):
+    if args.sparse:
+        for dtype, groups, width, n in SPARSE_SHAPES:
+            if args.reduce_dtype == "float32" and dtype == torch.float32:
+                continue
+            out_dtype = torch.float32 if args.reduce_dtype == "float32" else dtype
+            for zeros in ZEROS:
+                r = bench_sparse(dtype, groups, width, n, args.iters, zeros, out_dtype)
+                info["results"].append(r)
+                print(json.dumps(r), flush=True)
+        shapes = []
+    else:
+        shapes = SHAPES32 if args.reduce_dtype == "float32" else SHAPES
+    for shape in shapes:
         r = (bench32 if args.reduce_dtype == "float32" else bench)(*shape, args.iters)
         info["results"].append(r)
         print(json.dumps(r), flush=True)
