@@ -41,6 +41,7 @@ from __future__ import annotations
 
 from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -543,10 +544,27 @@ def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dt
                      f"not {reduce_dtype} for {t.dtype}")
 
 
+def _check_scale(what: str, scale, average: bool) -> Optional[np.float32]:
+    """The float32 pre-multiplier a scale argument stands for (None: a plain sum); average is resolved later, once
+    the world size is known."""
+    if average and scale is not None:
+        raise ValueError(f"{what}: pass average=True or a scale, not both")
+    return ops._scale32(scale)
+
+
+def _term(x: torch.Tensor, acc_dtype: torch.dtype, s32: Optional[np.float32]) -> torch.Tensor:
+    """What the scaled decode-and-sum adds for the words x: (x.float() * s32).to(acc_dtype), one float32 multiply
+    by a float32 tensor and one rounding; x.to(acc_dtype) without a scale."""
+    if s32 is None:
+        return x.to(acc_dtype)
+    return (x.float() * torch.tensor(float(s32), dtype=torch.float32, device=x.device)).to(acc_dtype)
+
+
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               temp_mem: Optional[torch.Tensor] = None, check: bool = True,
                               reduce_dtype: Optional[torch.dtype] = None,
-                              wire_dtype: Optional[torch.dtype] = None, sparse: bool = False) -> torch.Tensor:
+                              wire_dtype: Optional[torch.dtype] = None, sparse: bool = False,
+                              scale: Optional[float] = None, average: bool = False) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -569,17 +587,31 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
 
     sparse=True: sparse archives on the wire (no stored bits for +0 and -0 words), summed by the sparse
     decode-and-sum (ops.decompress_data_reduce(sparse=True)); the result is the same fold, bit for bit, with
-    reduce_dtype too.  Not with wire_dtype: that raises ValueError before any communication."""
+    reduce_dtype too.  Not with wire_dtype: that raises ValueError before any communication.
+
+    scale=s (a real number, rounded once to float32: np.float32(s)) pre-multiplies every rank's term before the sum,
+    as NCCL's average and FSDP / DeepSpeed's gradient pre-division do; average=True means s = np.float32(1 / world),
+    and passing both raises ValueError before any communication.  The term of rank r is
+    term(x) = (x.float() * s32).to(acc) with s32 = torch.tensor(s, dtype=torch.float32) and x = t_r's chunk in the
+    archive dtype (the wire dtype's word with wire_dtype), acc the result's dtype, and the result is the rank-order
+    fold ((term(x_0) + term(x_1)) + term(x_2)) + ... bit for bit on every rank, with reduce_dtype, wire_dtype and
+    sparse too.  The received archives are scaled inside the decode-and-sum kernel
+    (ops.decompress_data_reduce(scale=)), so no rank makes a scaled copy of its input."""
+    s32 = _check_scale("reduce_scatter_compressed", scale, average)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
     world = _world(group)
+    if average:
+        s32 = np.float32(1 / world)
     flat = t.reshape(-1)
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
     arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     if world == 1 or n == 0:
+        if s32 is not None:
+            return _term(flat[: n // world].to(arch_dtype), acc_dtype, s32)
         return flat[: n // world].to(arch_dtype).to(acc_dtype, copy=True)
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
@@ -619,6 +651,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     out = torch.empty(shard, dtype=acc_dtype, device=dev)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
     own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
+    if s32 is not None:
+        own = _term(own, acc_dtype, s32)  # the kernel's term of the own chunk, already in the result's dtype
     statuses = []
     # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add; fp32 += fp16 /
     # bf16 is the same fp32 add of the widened word), + r+1..world-1
@@ -627,13 +661,13 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     else:
         st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
-                                   archive_dtype=arch_dtype, sparse=sparse)
+                                   archive_dtype=arch_dtype, sparse=sparse, scale=s32)
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse)
+                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse, scale=s32)
         statuses.append(st)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
@@ -642,23 +676,30 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
 
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
                           check: bool = True, reduce_dtype: Optional[torch.dtype] = None,
-                          sparse: bool = False) -> torch.Tensor:
+                          sparse: bool = False, scale: Optional[float] = None,
+                          average: bool = False) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
     for the exchange.  Bit-identical on every rank to the rank-order left fold with torch's adds.
     reduce_dtype=torch.float32 with a float16 / bfloat16 t sums in fp32 as reduce_scatter_compressed does and
     all-gathers the fp32 shards: the float32 result is the fp32 fold on every rank.  sparse=True sends sparse
-    archives in both phases (see reduce_scatter_compressed); the result is the same."""
+    archives in both phases (see reduce_scatter_compressed); the result is the same.  scale=s or average=True
+    (s = np.float32(1 / world); not both) pre-multiplies every rank's term as in reduce_scatter_compressed: the
+    result is the rank-order fold of (t_r.float() * s32).to(acc) on every rank, bit for bit."""
+    s32 = _check_scale("all_reduce_compressed", scale, average)
     _check_sparse_wire(t.dtype, "all_reduce_compressed", sparse)
     acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
     world = _world(group)
+    if average:
+        s32 = np.float32(1 / world)
     flat = t.reshape(-1)
     n = flat.numel()
     if world == 1 or n == 0:
-        return t.to(acc_dtype, copy=True)
+        return t.to(acc_dtype, copy=True) if s32 is None else _term(t, acc_dtype, s32)
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
-    shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse)
+    shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse,
+                                      scale=s32)
     full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check, sparse=sparse)
     return full[:n].view(t.shape)

@@ -535,21 +535,30 @@ int dgb_float_decompress_reduce(void* temp, size_t tempBytes, int ft, int pb, ui
                                 uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                 const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, ft, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, false, (cudaStream_t)stream);
+                      outSuccess_dev, false, nullptr, (cudaStream_t)stream);
 }
 
 int dgb_float_decompress_reduce_to(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
                                    uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                    const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, false, (cudaStream_t)stream);
+                      outSuccess_dev, false, nullptr, (cudaStream_t)stream);
 }
 
 int dgb_float_decompress_reduce_sparse(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
                                        uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                        const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, true, (cudaStream_t)stream);
+                      outSuccess_dev, true, nullptr, (cudaStream_t)stream);
+}
+
+int dgb_float_decompress_reduce_scaled(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
+                                       uint32_t archivesPerGroup, const void* const* in, void* const* out,
+                                       const uint32_t* outSize, int accumulate, float scale, uint8_t* outSuccess_dev,
+                                       void* stream) {
+  // the dense pairs of dgb_float_decompress_reduce_to and the sparse pairs of dgb_float_decompress_reduce_sparse
+  return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
+                      outSuccess_dev, isSparseKind(ft), &scale, (cudaStream_t)stream);
 }
 
 // ---- info ------------------------------------------------------------------

@@ -150,11 +150,13 @@ constexpr int kGroupRows = DGB_DEC_GROUP_ROWS;  // rows per prefetch group (8 or
 constexpr uint32_t kRingSlots = 3;              // groups resident per warp: current + 2 in flight
 
 // writer kinds of the decode-and-sum (further down): the archive kind | kAddWriter adds the decoded word to the
-// output's word; | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives (dense or sparse)
+// output's word; | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives (dense or sparse);
+// | kScaled multiplies every decoded word by the call's scale first (0x40 is the encoder's narrowing bit)
 constexpr int kAddWriter = 0x10;
 constexpr int kWidenF32 = 0x20;
+constexpr int kScaled = 0x80;
 // the archive kind of a decode-and-sum kernel or writer kind
-__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32); }
+__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32 | kScaled); }
 
 template <int KIND>
 struct RowWriter;
@@ -1168,6 +1170,10 @@ int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineM
 // types 5 and 6 into fp32.  The kernel's kind is then the sparse kind (| kWidenF32); its writers take each word
 // from the sparse decoder's writer and add it as the dense writers do, so the result is the dense sum of the same
 // words bit for bit.
+// Scaled sums (dgb_float_decompress_reduce_scaled): any of the ten kinds above | kScaled.  Every writer, the store
+// of archive 0 included, replaces the decoded word x by its term s(x) (scaleWord / scaleWiden) before it stores or
+// adds it; the running sum an add writer loads is not scaled.  The scale is a kernel parameter (InlineMembers::scale)
+// read by these kinds only.
 // ---------------------------------------------------------------------------
 #ifndef DGB_REDUCE_PASS_ARCHIVES
 #define DGB_REDUCE_PASS_ARCHIVES 4
@@ -1259,6 +1265,29 @@ __device__ __forceinline__ uint32_t widenWord(uint32_t w) {
     asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)w));
     return __float_as_uint(f);
   }
+}
+
+// The terms of the scaled sums.  __fmul_rn is one mul.rn.f32 that nvcc never contracts with the add that follows
+// into an FFMA (a fused multiply-add rounds once, the contract twice).  scaleWord: a word of dense kind KIND times s,
+// in that kind: fp32 products as they are, 16-bit words widened exactly and the fp32 product rounded back to the
+// 16-bit type with round-to-nearest-even.  scaleWiden: a 16-bit word's fp32 product, left in fp32.
+template <int KIND>
+__device__ __forceinline__ uint32_t scaleWord(uint32_t w, float s) {
+  if constexpr (KIND == kKindF32) {
+    return __float_as_uint(__fmul_rn(__uint_as_float(w), s));
+  } else {
+    const float p = __fmul_rn(__uint_as_float(widenWord<KIND>(w)), s);
+    unsigned short r;
+    if constexpr (KIND == kKindF16)
+      asm("cvt.rn.f16.f32 %0, %1;" : "=h"(r) : "f"(p));
+    else
+      asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(p));
+    return r;
+  }
+}
+template <int KIND>
+__device__ __forceinline__ uint32_t scaleWiden(uint32_t w, float s) {
+  return __float_as_uint(__fmul_rn(__uint_as_float(widenWord<KIND>(w)), s));
 }
 
 // Widening writers: the 16-bit kind's ring, copies and join; each lane stores one u32 per row, so a row is one
@@ -1374,6 +1403,138 @@ template <> struct RowWriter<kKindBF16S | kWidenF32> : RowWriterSparseReduce<kKi
 template <> struct RowWriter<kKindF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindF16S | kWidenF32 | kAddWriter> {};
 template <> struct RowWriter<kKindBF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindBF16S | kWidenF32 | kAddWriter> {};
 
+// Scaled writers (| kScaled): the unscaled writer of the same kind with the term s(x) in place of the decoded word
+// x.  Each keeps its base's ring, copies, cursor and running-sum loads, and has its own `scale` (decodeReduceBlock
+// sets it).
+template <int KIND>
+struct RowWriterScale16 : RowWriter16<KIND> {
+  typedef RowWriter16<KIND> B;
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const typename B::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    B::out[row * 32u] = (uint16_t)scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale);
+  }
+};
+template <int KIND>
+struct RowWriterScaleAdd16 : RowWriterAdd16<KIND> {
+  typedef RowWriterAdd16<KIND> A;
+  typedef RowWriter16<KIND> B;
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)addWord<KIND>(c.prev[J], scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint16_t* o = B::out + row * 32u;
+    *o = (uint16_t)addWord<KIND>(*o, scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale));
+  }
+};
+struct RowWriterScale32 : RowWriter<kKindF32> {
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    out[row * 32u] = scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale);
+  }
+};
+struct RowWriterScaleAdd32 : RowWriter<kKindF32 | kAddWriter> {
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = addWord<kKindF32>(c.prev[J], scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)),
+                                                                   scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = out + row * 32u;
+    *o = addWord<kKindF32>(*o, scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale));
+  }
+};
+template <int KIND>
+struct RowWriterScaleWiden16 : RowWriterWiden16<KIND> {
+  typedef RowWriterWiden16<KIND> W;
+  typedef RowWriter16<KIND> B;
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const typename W::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    W::out32[row * 32u] = scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale);
+  }
+};
+template <int KIND>
+struct RowWriterScaleWidenAdd16 : RowWriterWidenAdd16<KIND> {
+  typedef RowWriterWidenAdd16<KIND> A;
+  typedef RowWriter16<KIND> B;
+  float scale;
+  template <int J>
+  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = addWord<kKindF32>(c.prev[J], scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = A::out32 + row * 32u;
+    *o = addWord<kKindF32>(*o, scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale));
+  }
+};
+template <> struct RowWriter<kKindF16 | kScaled> : RowWriterScale16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kScaled> : RowWriterScale16<kKindBF16> {};
+template <> struct RowWriter<kKindF16 | kScaled | kAddWriter> : RowWriterScaleAdd16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kScaled | kAddWriter> : RowWriterScaleAdd16<kKindBF16> {};
+template <> struct RowWriter<kKindF32 | kScaled> : RowWriterScale32 {};
+template <> struct RowWriter<kKindF32 | kScaled | kAddWriter> : RowWriterScaleAdd32 {};
+template <> struct RowWriter<kKindF16 | kWidenF32 | kScaled> : RowWriterScaleWiden16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaled> : RowWriterScaleWiden16<kKindBF16> {};
+template <> struct RowWriter<kKindF16 | kWidenF32 | kScaled | kAddWriter> : RowWriterScaleWidenAdd16<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaled | kAddWriter> : RowWriterScaleWidenAdd16<kKindBF16> {};
+// Sparse: RowWriterSparseReduce's word, cursor and running sums with the term in place of the word, for archive 0
+// as well (the sparse decoder's own writer stores unscaled words).  WK = the sparse kind | kScaled, | kAddWriter
+// and / or | kWidenF32.
+template <int WK>
+struct RowWriterSparseScaled : RowWriterSparseReduce<WK & ~kScaled> {
+  typedef RowWriterSparseReduce<WK & ~kScaled> R;
+  typedef typename R::B B;
+  typedef typename R::T T;
+  float scale;
+  __device__ __forceinline__ T combine(uint32_t prev, uint32_t w) const {
+    uint32_t v;
+    if constexpr (R::kWiden) v = scaleWiden<R::BT>(w, scale);
+    else v = scaleWord<R::BT>(w, scale);
+    if constexpr (R::kAdd) return (T)addWord<R::kSumKind>(prev, v);
+    else return (T)v;
+  }
+  template <int J>
+  __device__ __forceinline__ void write(const typename R::Cursor& c, uint32_t entry) const {
+    const uint32_t w = B::word(entry, true);
+    if constexpr (R::kAdd) c.o[J * 32] = combine(c.prev[J], w);
+    else c.o[J * 32] = combine(0u, w);
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
+  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
+    const uint32_t w = B::word(entry, valid);
+    if (valid) {
+      T* o = R::sum + row * 32u;
+      *o = combine(R::kAdd ? (uint32_t)*o : 0u, w);
+    }
+  }
+};
+template <int SK, int EXTRA>
+using SparseScaled = RowWriterSparseScaled<SK | kScaled | EXTRA>;
+template <> struct RowWriter<kKindF16S | kScaled> : SparseScaled<kKindF16S, 0> {};
+template <> struct RowWriter<kKindBF16S | kScaled> : SparseScaled<kKindBF16S, 0> {};
+template <> struct RowWriter<kKindF32S | kScaled> : SparseScaled<kKindF32S, 0> {};
+template <> struct RowWriter<kKindF16S | kScaled | kAddWriter> : SparseScaled<kKindF16S, kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kScaled | kAddWriter> : SparseScaled<kKindBF16S, kAddWriter> {};
+template <> struct RowWriter<kKindF32S | kScaled | kAddWriter> : SparseScaled<kKindF32S, kAddWriter> {};
+template <> struct RowWriter<kKindF16S | kWidenF32 | kScaled> : SparseScaled<kKindF16S, kWidenF32> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled> : SparseScaled<kKindBF16S, kWidenF32> {};
+template <> struct RowWriter<kKindF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindF16S, kWidenF32 | kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindBF16S, kWidenF32 | kAddWriter> {};
+
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
 // consistent with its word count, and that word count is the group's output size.
 template <int KIND, int PB>
@@ -1390,7 +1551,7 @@ template <int WK, int PB>
 __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, uint32_t block, uint32_t nb,
                                                   const typename Lut<PB, false>::Entry* __restrict__ lut,
                                                   uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
-                                                  uint32_t slotWords, uint32_t lane) {
+                                                  uint32_t slotWords, uint32_t lane, float scale) {
   const ArchiveView av = openArchive<reduceArchiveKind(WK)>(in);
   const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
   const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
@@ -1399,6 +1560,7 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
   RowWriter<WK> wr;
   wr.setRing(ring, lane);
   wr.setBlock(av, out, block, lane);
+  if constexpr ((WK & kScaled) != 0) wr.scale = scale;
   const uint2 bw = __ldg(pBlockWords + block);
   const uint32_t blockLen = bw.x >> 16, words = bw.x & 0xffffu;
   const uint16_t* stream = pData + bw.y;
@@ -1431,12 +1593,14 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
 
 // One pass: archives [a0, a1) of every group.  Member table entry g * width + j = {archive (g, j), out[g],
 // out_size[g], block cap of group g}.  addFirst: archive a0 adds too (accumulate, or a later pass).  Only the
-// first pass (a0 == 0) reports outSuccess.  KIND is the archive kind, | kWidenF32 for fp32 outputs.
+// first pass (a0 == 0) reports outSuccess.  KIND is the archive kind, | kWidenF32 for fp32 outputs, | kScaled for
+// scaled sums (the scale is im.scale, in every pass).
 template <int KIND, int PB>
 __global__ void __launch_bounds__(kReduceWarps * 32, 4)
 decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
                    uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
   constexpr int AK = reduceArchiveKind(KIND);
+  const float scale = (KIND & kScaled) != 0 ? im.scale : 1.0f;  // the unscaled kinds never read it
   constexpr int WARPS = kReduceWarps;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t K = 1u << PB;
@@ -1538,10 +1702,11 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
         for (uint32_t a = a0; a < a1; ++a) {
           const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
           if (a == a0 && !addFirst)
-            decodeReduceBlock<KIND, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane);
+            decodeReduceBlock<KIND, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane,
+                                        scale);
           else
             decodeReduceBlock<KIND | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring, mySlot, myBar, phase,
-                                                     slotWords, lane);
+                                                     slotWords, lane, scale);
         }
       }
       block = __shfl_sync(0xffffffffu, nextBlock, 0);
@@ -1712,8 +1877,9 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
-                 uint8_t* outSuccess_dev, bool sparse, cudaStream_t stream) {
-  // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8
+                 uint8_t* outSuccess_dev, bool sparse, const float* scale, cudaStream_t stream) {
+  // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8; scale: null for a plain sum, else
+  // the multiplier of the scaled kinds
   if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
   // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
   const int dk = denseKind(kind);
@@ -1760,18 +1926,23 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
     const int rc = uploadTable(sc.members, desc, sizeof(MemberDesc) * n, stream);
     if (rc != DGB_OK) return rc;
   }
+  im.scale = scale ? *scale : 1.0f;  // a kernel parameter: a captured launch keeps the value it was captured with
   return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
     constexpr int KIND = decltype(K)::value;
     constexpr int DK = denseKind(KIND);
+    // the kernel of writer kind WK, or of WK | kScaled
+    auto launch = [&](auto WK) {
+      if (scale)
+        return launchDecodeReduce<decltype(WK)::value | kScaled, decltype(P)::value>(
+            opt, sc, im, groups, width, totalChunks, accumulate, outSuccess_dev, stream);
+      return launchDecodeReduce<decltype(WK)::value, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
+                                                                        accumulate, outSuccess_dev, stream);
+    };
     if constexpr (DK == kKindF16 || DK == kKindBF16) {
-      if (widen)
-        return launchDecodeReduce<KIND | kWidenF32, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
-                                                                       accumulate, outSuccess_dev, stream);
-      return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
-                                                         outSuccess_dev, stream);
+      if (widen) return launch(std::integral_constant<int, KIND | kWidenF32>());
+      return launch(std::integral_constant<int, KIND>());
     } else if constexpr (DK == kKindF32)
-      return launchDecodeReduce<KIND, decltype(P)::value>(opt, sc, im, groups, width, totalChunks, accumulate,
-                                                         outSuccess_dev, stream);
+      return launch(std::integral_constant<int, KIND>());
     else
       return (int)DGB_ERR_INVALID_ARG;  // not reached (checked above)
   }); });

@@ -21,8 +21,10 @@ dtype, and archives and output rows must be 16 B aligned.
 """
 from __future__ import annotations
 
+import numbers
 from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import capi
@@ -396,11 +398,21 @@ def decompress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], ts_o
 _REDUCE_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16, torch.float32: capi.FLOAT32}
 
 
+def _scale32(scale) -> Optional[np.float32]:
+    """None, or a host real number rounded once to float32 (the scale of the scaled decode-and-sum)."""
+    if scale is None:
+        return None
+    if isinstance(scale, bool) or not isinstance(scale, numbers.Real):
+        raise TypeError(f"scale is None or a real number (a host value, rounded to float32), not {type(scale).__name__}")
+    return np.float32(scale)
+
+
 def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequence[torch.Tensor],
                            accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
                            out_status: Optional[torch.Tensor] = None, *,
                            prob_bits: int = K_DEFAULT_PRECISION,
-                           archive_dtype: Optional[torch.dtype] = None, sparse: bool = False) -> int:
+                           archive_dtype: Optional[torch.dtype] = None, sparse: bool = False,
+                           scale: Optional[float] = None) -> int:
     """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
@@ -415,7 +427,16 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
 
     sparse=True: the archives were made with compress_data(..., sparse=True) from archive_dtype tensors
     (dgb_float_decompress_reduce_sparse).  The same dtype pairs are allowed, and the result is bit-identical to this
-    call on dense archives of the same words; a dense archive in such a group is invalid."""
+    call on dense archives of the same words; a dense archive in such a group is invalid.
+
+    scale (dgb_float_decompress_reduce_scaled): a real number s, rounded once to float32 (np.float32(s)).  Every
+    decoded word x is multiplied by s before it is added: its term is (x.float() * s32).to(out dtype) with s32 =
+    torch.tensor(s, dtype=torch.float32), so a 16-bit same-type sum rounds each product to the 16-bit type first,
+    while float32 and widening sums keep it in float32.  The result is torch's fold acc = term(x(g, 0)) (or
+    ts_out[g] unscaled when accumulating); acc = acc + term(x(g, 1)); ... bit for bit, with archive_dtype and sparse
+    too (an elided zero is scaled like any other word, so s < 0 turns +0 into -0).  scale=1.0 gives the unscaled
+    result; None (the default) calls the unscaled entries.  A scale is a host value: a tensor raises TypeError."""
+    scale32 = _scale32(scale)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
@@ -443,13 +464,16 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     ft, out_ft = (_SPARSE_TYPES if sparse else _REDUCE_TYPES)[archive_dtype], _REDUCE_TYPES[dtype]
     L = capi.lib()
     entry = L.dgb_float_decompress_reduce_sparse if sparse else L.dgb_float_decompress_reduce_to
+    extra = ()
+    if scale32 is not None:
+        entry, extra = L.dgb_float_decompress_reduce_scaled, (float(scale32),)
     with torch.cuda.device(dev):
         need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
         tmp = _Temp(temp_mem, need, dev)
         rc = entry(tmp.ptr, tmp.bytes, ft, out_ft, prob_bits, g, width,
                    capi.ptr_array([t.data_ptr() for t in ins]),
                    capi.ptr_array([t.data_ptr() for t in ts_out]),
-                   capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)),
+                   capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)), *extra,
                    st_ptr, _stream())
     capi.check(rc, "decompress_data_reduce")
     return tmp.need

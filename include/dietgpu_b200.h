@@ -265,6 +265,30 @@ int dgb_float_decompress_reduce_sparse(void* temp_dev, size_t temp_bytes, int fl
                                        const void* const* in, void* const* out, const uint32_t* out_size,
                                        int accumulate, uint8_t* out_success_dev, void* stream);
 
+/* Pre-multiplied decode-and-sum (new; no reference counterpart): every decoded word x is multiplied by `scale`
+ * before it is summed, as an average over ranks (scale = 1 / W) or a gradient pre-division needs, without a scaled
+ * copy of any input.  The allowed pairs (float_type, out_float_type) are the five of dgb_float_decompress_reduce_to
+ * and the five of dgb_float_decompress_reduce_sparse; any other pair returns DGB_ERR_INVALID_ARG before any CUDA
+ * call.  The term of a word is
+ *   fp16 / bf16 archives, outputs of the same type:  round_T(fp32(x) * scale), one fp32 round-to-nearest-even
+ *                                                     multiply, then one round-to-nearest-even conversion to T;
+ *   fp32 archives:                                   x * scale, one fp32 round-to-nearest-even multiply;
+ *   fp16 / bf16 archives, fp32 outputs:              fp32(x) * scale, left in fp32;
+ * sparse archives take the rule of their dense type for the word they stand for: an elided word is the +0 or -0 it
+ * stands for and is multiplied like any other (a negative scale turns +0 into -0; an infinite or NaN scale makes it
+ * NaN).  out[g] = (accumulate ? out[g] : term(x(g,0))) + term(x(g,1)) + ... + term(x(g,W-1)) in archive order with
+ * the output type's add; the value taken in by accumulate is not scaled, so a sum may be split over several calls.
+ * This is torch's fold with term(x) = (x.float() * s).to(out dtype) for a float32 tensor s, bit for bit (NaN
+ * payloads aside); with scale = 1 it is exactly the unscaled entries' result.  Everything else is as in
+ * dgb_float_decompress_reduce_to / dgb_float_decompress_reduce_sparse: the validity rule, statuses, groups with an
+ * invalid archive left unwritten, no synchronisation, num_groups = 0 returning DGB_OK and the scratch size
+ * dgb_float_decompress_temp_bytes(float_type, G * W, 0).  The scale travels by value in the kernels' parameters: a
+ * call captured into a CUDA graph replays with the scale it was captured with. */
+int dgb_float_decompress_reduce_scaled(void* temp_dev, size_t temp_bytes, int float_type, int out_float_type,
+                                       int prob_bits, uint32_t num_groups, uint32_t archives_per_group,
+                                       const void* const* in, void* const* out, const uint32_t* out_size,
+                                       int accumulate, float scale, uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

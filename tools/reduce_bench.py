@@ -14,6 +14,7 @@ once + outputs written once: G * N words for (1), G * W * N for (2)).  (1)'s res
 the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_ARCHIVES=2).
 
 --sparse: sparse against dense decode-and-sum (bench_sparse) at zero fractions 0 %, ReLU (about 50 %), 90 % and 99 %.
+--scale: the scaled decode-and-sum against the unscaled one and against scaling the inputs with torch (bench_scale).
 """
 import argparse
 import json
@@ -233,6 +234,77 @@ def bench_sparse(dtype, groups, width, n, iters, zeros, out_dtype):
     return r
 
 
+SCALE_SHAPES = [  # (dtype, groups, width, words, out dtype, sparse ReLU data)
+    (torch.bfloat16, 8, 8, 2 << 20, torch.bfloat16, False),
+    (torch.float32, 16, 4, 1 << 20, torch.float32, False),
+    (torch.float16, 64, 2, 512 << 10, torch.float16, False),
+    (torch.bfloat16, 8, 8, 2 << 20, torch.float32, False),
+    (torch.bfloat16, 8, 8, 2 << 20, torch.bfloat16, True),
+]
+
+
+def bench_scale(dtype, groups, width, n, iters, out_dtype, sparse):
+    """--scale, s = fp32(1 / W) on the same inputs, alternated:
+    (1) the scaled decode-and-sum of the archives; (2) the unscaled one (same archives, same kernel shape);
+    (3) the caller's way without (1): term(t) = (t.float() * s32).to(out dtype) with torch, compress, unscaled sum
+    (bit-identical to (1), checked).  Reported: call time of (1) and (2), of compress + (1) ("1c"), of (3) and of its
+    torch multiply alone ("3_mul"); kernel time (timing=1) of (1) and (2)."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [sparse_data(dtype, n, "relu" if sparse else "0", g) for _ in range(groups * width)]
+    s32 = torch.tensor(1.0 / width, dtype=torch.float32, device="cuda")
+    s = float(s32)
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    comp, sizes, _ = ops.compress_data(True, xs, sparse=sparse)
+    hs = sizes.cpu().tolist()
+    gi = [[comp[k * width + j, :hs[k * width + j]] for j in range(width)] for k in range(groups)]
+    outs = {k: [torch.empty(n, dtype=out_dtype, device="cuda") for _ in range(groups)] for k in ("1", "2", "3")}
+    terms = [torch.empty(n, dtype=out_dtype, device="cuda") for _ in range(groups * width)]
+
+    def one():
+        ops.decompress_data_reduce(gi, outs["1"], False, temp, archive_dtype=dtype, sparse=sparse, scale=s)
+
+    def two():
+        ops.decompress_data_reduce(gi, outs["2"], False, temp, archive_dtype=dtype, sparse=sparse)
+
+    def one_c():
+        c, sz, _ = ops.compress_data(True, xs, sparse=sparse)
+        ops.decompress_data_reduce([[c[k * width + j] for j in range(width)] for k in range(groups)], outs["1"], False,
+                                   temp, archive_dtype=dtype, sparse=sparse, scale=s)
+
+    def mul():
+        # one torch kernel per input: a 16-bit x times the float32 0-dim tensor stays 16-bit and is computed in fp32,
+        # which is the same-type term; the widening term needs the fp32 product itself
+        for x, t in zip(xs, terms):
+            torch.mul(x.float() if out_dtype != dtype else x, s32, out=t)
+
+    def three():
+        mul()
+        c, sz, _ = ops.compress_data(True, terms, sparse=sparse)
+        ops.decompress_data_reduce([[c[k * width + j] for j in range(width)] for k in range(groups)], outs["3"], False,
+                                   temp, sparse=sparse)
+
+    fns = {"1": one, "2": two, "1c": one_c, "3": three, "3_mul": mul}
+    for f in fns.values():  # warm-up
+        f()
+    torch.cuda.synchronize()
+    it = torch.int32 if out_dtype == torch.float32 else torch.int16
+    for k in range(groups):
+        same = (outs["1"][k].view(it) == outs["3"][k].view(it)) | (outs["1"][k].isnan() & outs["3"][k].isnan())
+        assert bool(same.all()), k
+    t = {k: [] for k in fns}
+    for _ in range(3):  # alternate
+        for k, f in fns.items():
+            t[k].append(timed(f, iters))
+    kt = {"1": kernel_us(one, iters), "2": kernel_us(two, iters)}
+    r = {"shape": f"{'sparse relu ' if sparse else ''}{str(dtype).split('.')[-1]}->{str(out_dtype).split('.')[-1]} "
+                  f"{groups}x{width}x{n}", "scale": s,
+         "call_us": {k: min(v) for k, v in t.items()}, "call_us_max": {k: max(v) for k, v in t.items()},
+         "kernel_us": kt}
+    r["kernel_scaled_over_plain"] = kt["1"] / kt["2"]
+    r["1c_over_3"] = r["call_us"]["1c"] / r["call_us"]["3"]
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -240,10 +312,17 @@ def main():
     ap.add_argument("--reduce-dtype", choices=["same", "float32"], default="same",
                     help="float32: sum the 16-bit shapes' archives into fp32 outputs (bench32)")
     ap.add_argument("--sparse", action="store_true", help="sparse against dense archives (bench_sparse)")
+    ap.add_argument("--scale", action="store_true", help="scaled against unscaled sums and torch's scaling (bench_scale)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    if args.sparse:
+    if args.scale:
+        for shape in SCALE_SHAPES:
+            r = bench_scale(*shape[:4], args.iters, *shape[4:])
+            info["results"].append(r)
+            print(json.dumps(r), flush=True)
+        shapes = []
+    elif args.sparse:
         for dtype, groups, width, n in SPARSE_SHAPES:
             if args.reduce_dtype == "float32" and dtype == torch.float32:
                 continue
