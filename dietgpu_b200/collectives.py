@@ -544,27 +544,50 @@ def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dt
                      f"not {reduce_dtype} for {t.dtype}")
 
 
-def _check_scale(what: str, scale, average: bool) -> Optional[np.float32]:
-    """The float32 pre-multiplier a scale argument stands for (None: a plain sum); average is resolved later, once
-    the world size is known."""
+def _check_scale(what: str, scale, average: bool, scale_tensor=None, found_inf=None,
+                 dev=None) -> Optional[np.float32]:
+    """The float32 pre-multiplier a scale argument stands for (None: a plain sum, or a device scale_tensor); average
+    is resolved later, once the world size is known.  scale_tensor and found_inf are checked as
+    ops.decompress_data_reduce checks them, on dev (t's device)."""
     if average and scale is not None:
         raise ValueError(f"{what}: pass average=True or a scale, not both")
-    return ops._scale32(scale)
+    if scale_tensor is not None and (scale is not None or average):
+        raise ValueError(f"{what}: scale_tensor replaces scale and average=True (divide it by the world size on the "
+                         "device)")
+    if found_inf is not None and scale_tensor is None:
+        raise ValueError(f"{what}: found_inf needs scale_tensor (torch.ones(1) for the unscaled sum)")
+    s32 = ops._scale32(scale)
+    if scale_tensor is not None:
+        ops._check_flag_tensor(f"{what}: scale_tensor", scale_tensor, dev)
+    if found_inf is not None:
+        ops._check_flag_tensor(f"{what}: found_inf", found_inf, dev)
+    return s32
 
 
-def _term(x: torch.Tensor, acc_dtype: torch.dtype, s32: Optional[np.float32]) -> torch.Tensor:
+def _term(x: torch.Tensor, acc_dtype: torch.dtype, s32) -> torch.Tensor:
     """What the scaled decode-and-sum adds for the words x: (x.float() * s32).to(acc_dtype), one float32 multiply
-    by a float32 tensor and one rounding; x.to(acc_dtype) without a scale."""
+    by a float32 tensor and one rounding; x.to(acc_dtype) without a scale.  s32: a float32 number, or a device
+    scale_tensor (one element)."""
     if s32 is None:
         return x.to(acc_dtype)
+    if isinstance(s32, torch.Tensor):
+        return (x.float() * s32.reshape(())).to(acc_dtype)
     return (x.float() * torch.tensor(float(s32), dtype=torch.float32, device=x.device)).to(acc_dtype)
+
+
+def _flag_non_finite(found_inf: Optional[torch.Tensor], x: torch.Tensor) -> None:
+    """found_inf = max(found_inf, 1 if x has an inf or NaN else 0), on the device (no host sync, never cleared)."""
+    if found_inf is not None:
+        torch.maximum(found_inf, (~x.isfinite()).any().float(), out=found_inf)
 
 
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               temp_mem: Optional[torch.Tensor] = None, check: bool = True,
                               reduce_dtype: Optional[torch.dtype] = None,
                               wire_dtype: Optional[torch.dtype] = None, sparse: bool = False,
-                              scale: Optional[float] = None, average: bool = False) -> torch.Tensor:
+                              scale: Optional[float] = None, average: bool = False,
+                              scale_tensor: Optional[torch.Tensor] = None,
+                              found_inf: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -596,23 +619,33 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     archive dtype (the wire dtype's word with wire_dtype), acc the result's dtype, and the result is the rank-order
     fold ((term(x_0) + term(x_1)) + term(x_2)) + ... bit for bit on every rank, with reduce_dtype, wire_dtype and
     sparse too.  The received archives are scaled inside the decode-and-sum kernel
-    (ops.decompress_data_reduce(scale=)), so no rank makes a scaled copy of its input."""
-    s32 = _check_scale("reduce_scatter_compressed", scale, average)
+    (ops.decompress_data_reduce(scale=)), so no rank makes a scaled copy of its input.
+
+    scale_tensor (a one-element float32 CUDA tensor on t's device) is the scale kept on the device, e.g. a
+    GradScaler's inverse scale divided by the world size: the kernels read it, the host never does, and the result
+    is bit-identical to this call with scale=float(scale_tensor).  Not with scale or average=True.  found_inf (with
+    scale_tensor; the same kind of tensor) is set to 1.0 when any element of the returned shard is inf or NaN, and
+    never cleared (torch.amp's found_inf convention), without a host sync.  These keywords raise ValueError before
+    any communication."""
+    s32 = _check_scale("reduce_scatter_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
     world = _world(group)
     if average:
         s32 = np.float32(1 / world)
+    sd = s32 if scale_tensor is None else scale_tensor  # the terms' scale: a float32, a device tensor or None
     flat = t.reshape(-1)
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
     arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     if world == 1 or n == 0:
-        if s32 is not None:
-            return _term(flat[: n // world].to(arch_dtype), acc_dtype, s32)
-        return flat[: n // world].to(arch_dtype).to(acc_dtype, copy=True)
+        if sd is None:
+            return flat[: n // world].to(arch_dtype).to(acc_dtype, copy=True)
+        res = _term(flat[: n // world].to(arch_dtype), acc_dtype, sd)
+        _flag_non_finite(found_inf, res)
+        return res
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
@@ -651,8 +684,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     out = torch.empty(shard, dtype=acc_dtype, device=dev)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
     own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
-    if s32 is not None:
-        own = _term(own, acc_dtype, s32)  # the kernel's term of the own chunk, already in the result's dtype
+    if sd is not None:
+        own = _term(own, acc_dtype, sd)  # the kernel's term of the own chunk, already in the result's dtype
     statuses = []
     # rank order: sources 0..r-1 decoded and summed, + own chunk (torch's add is the kernel's add; fp32 += fp16 /
     # bf16 is the same fp32 add of the widened word), + r+1..world-1
@@ -661,14 +694,18 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     else:
         st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
-                                   archive_dtype=arch_dtype, sparse=sparse, scale=s32)
+                                   archive_dtype=arch_dtype, sparse=sparse, scale=s32, scale_tensor=scale_tensor)
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
+        # the last call writes the final values: the kernel checks them
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse, scale=s32)
+                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse, scale=s32,
+                                   scale_tensor=scale_tensor, found_inf=found_inf)
         statuses.append(st)
+    else:
+        _flag_non_finite(found_inf, out)  # the last rank ends on torch's add of its own chunk
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
     return out
@@ -677,7 +714,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
                           check: bool = True, reduce_dtype: Optional[torch.dtype] = None,
                           sparse: bool = False, scale: Optional[float] = None,
-                          average: bool = False) -> torch.Tensor:
+                          average: bool = False, scale_tensor: Optional[torch.Tensor] = None,
+                          found_inf: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
@@ -686,8 +724,10 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     all-gathers the fp32 shards: the float32 result is the fp32 fold on every rank.  sparse=True sends sparse
     archives in both phases (see reduce_scatter_compressed); the result is the same.  scale=s or average=True
     (s = np.float32(1 / world); not both) pre-multiplies every rank's term as in reduce_scatter_compressed: the
-    result is the rank-order fold of (t_r.float() * s32).to(acc) on every rank, bit for bit."""
-    s32 = _check_scale("all_reduce_compressed", scale, average)
+    result is the rank-order fold of (t_r.float() * s32).to(acc) on every rank, bit for bit.  scale_tensor and
+    found_inf are reduce_scatter_compressed's, except that found_inf covers the whole result on every rank: the
+    shards' flags meet in one MAX all-reduce of a one-element tensor."""
+    s32 = _check_scale("all_reduce_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sparse_wire(t.dtype, "all_reduce_compressed", sparse)
     acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
     world = _world(group)
@@ -696,10 +736,21 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     flat = t.reshape(-1)
     n = flat.numel()
     if world == 1 or n == 0:
-        return t.to(acc_dtype, copy=True) if s32 is None else _term(t, acc_dtype, s32)
+        if s32 is None and scale_tensor is None:
+            return t.to(acc_dtype, copy=True)
+        res = _term(t, acc_dtype, s32 if scale_tensor is None else scale_tensor)
+        _flag_non_finite(found_inf, res)
+        return res
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
+    # (a padding zero's term is non-finite only for an inf or NaN scale, which makes every element's term so too)
+    shard_inf = None if found_inf is None else torch.zeros(1, dtype=torch.float32, device=t.device)
     shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse,
-                                      scale=s32)
+                                      scale=s32, scale_tensor=scale_tensor, found_inf=shard_inf)
+    if found_inf is not None:
+        on_device = _device_collectives(group)
+        flag = shard_inf if on_device else shard_inf.cpu()
+        dist.all_reduce(flag, op=dist.ReduceOp.MAX, group=group)
+        torch.maximum(found_inf, flag.to(t.device), out=found_inf)
     full = all_gather_compressed(shard, group, members, temp_mem=temp_mem, check=check, sparse=sparse)
     return full[:n].view(t.shape)

@@ -535,21 +535,21 @@ int dgb_float_decompress_reduce(void* temp, size_t tempBytes, int ft, int pb, ui
                                 uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                 const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, ft, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, false, nullptr, (cudaStream_t)stream);
+                      outSuccess_dev, false, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int dgb_float_decompress_reduce_to(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
                                    uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                    const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, false, nullptr, (cudaStream_t)stream);
+                      outSuccess_dev, false, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int dgb_float_decompress_reduce_sparse(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
                                        uint32_t archivesPerGroup, const void* const* in, void* const* out,
                                        const uint32_t* outSize, int accumulate, uint8_t* outSuccess_dev, void* stream) {
   return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, true, nullptr, (cudaStream_t)stream);
+                      outSuccess_dev, true, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int dgb_float_decompress_reduce_scaled(void* temp, size_t tempBytes, int ft, int outFt, int pb, uint32_t numGroups,
@@ -558,7 +558,19 @@ int dgb_float_decompress_reduce_scaled(void* temp, size_t tempBytes, int ft, int
                                        void* stream) {
   // the dense pairs of dgb_float_decompress_reduce_to and the sparse pairs of dgb_float_decompress_reduce_sparse
   return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
-                      outSuccess_dev, isSparseKind(ft), &scale, (cudaStream_t)stream);
+                      outSuccess_dev, isSparseKind(ft), &scale, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int dgb_float_decompress_reduce_scaled_dev(void* temp, size_t tempBytes, int ft, int outFt, int pb,
+                                           uint32_t numGroups, uint32_t archivesPerGroup, const void* const* in,
+                                           void* const* out, const uint32_t* outSize, int accumulate,
+                                           const float* scale_dev, float* foundInf_dev, uint8_t* outSuccess_dev,
+                                           void* stream) {
+  // the pairs of dgb_float_decompress_reduce_scaled; the scale is read by the kernels, never on the host
+  if (!scale_dev || (reinterpret_cast<uintptr_t>(scale_dev) & 3u)) return DGB_ERR_INVALID_ARG;
+  if (reinterpret_cast<uintptr_t>(foundInf_dev) & 3u) return DGB_ERR_INVALID_ARG;
+  return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
+                      outSuccess_dev, isSparseKind(ft), nullptr, scale_dev, foundInf_dev, (cudaStream_t)stream);
 }
 
 // ---- info ------------------------------------------------------------------

@@ -208,7 +208,8 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
                 uint8_t* mismatchHost, cudaStream_t stream);
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
-                 uint8_t* outSuccess_dev, bool sparse, const float* scale, cudaStream_t stream);
+                 uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
+                 cudaStream_t stream);
 size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize);
 size_t decodeTempBytes(int kind, uint32_t n);
 int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool inIsDevice,

@@ -151,12 +151,18 @@ constexpr uint32_t kRingSlots = 3;              // groups resident per warp: cur
 
 // writer kinds of the decode-and-sum (further down): the archive kind | kAddWriter adds the decoded word to the
 // output's word; | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives (dense or sparse);
-// | kScaled multiplies every decoded word by the call's scale first (0x40 is the encoder's narrowing bit)
+// | kScaled multiplies every decoded word by the call's scale first (0x40 is the encoder's narrowing bit);
+// | kDevScale (kernels only, with kScaled) reads that scale from device memory when the kernel runs;
+// | kCheckFinite (writers only) also reports whether a word it stores is inf or NaN
 constexpr int kAddWriter = 0x10;
 constexpr int kWidenF32 = 0x20;
 constexpr int kScaled = 0x80;
+constexpr int kDevScale = 0x100;
+constexpr int kCheckFinite = 0x200;
 // the archive kind of a decode-and-sum kernel or writer kind
-__host__ __device__ constexpr int reduceArchiveKind(int k) { return k & ~(kAddWriter | kWidenF32 | kScaled); }
+__host__ __device__ constexpr int reduceArchiveKind(int k) {
+  return k & ~(kAddWriter | kWidenF32 | kScaled | kDevScale | kCheckFinite);
+}
 
 template <int KIND>
 struct RowWriter;
@@ -1290,6 +1296,23 @@ __device__ __forceinline__ uint32_t scaleWiden(uint32_t w, float s) {
   return __float_as_uint(__fmul_rn(__uint_as_float(widenWord<KIND>(w)), s));
 }
 
+// The non-finite check of the device-scale sums (| kCheckFinite): the writer of a call's last archive passes every
+// word it stores through note(), which ORs into the lane's `bad` whether the word's exponent field is all ones (inf
+// or NaN) in SK, the stored type; decodeReduceBlock votes over the warp once per block.  Lanes that store nothing
+// (past the end of a partial row, or every lane of a group left unwritten) never call note().
+template <int SK>
+__device__ __forceinline__ bool nonFiniteWord(uint32_t w) {
+  constexpr uint32_t e = SK == kKindF32 ? 0x7f800000u : SK == kKindF16 ? 0x7c00u : 0x7f80u;
+  return (w & e) == e;
+}
+template <int SK>
+struct FiniteCheck {
+  mutable uint32_t bad = 0u;
+  __device__ __forceinline__ uint32_t note(uint32_t w) const {
+    bad |= nonFiniteWord<SK>(w) ? 1u : 0u;
+    return w;
+  }
+};
 // Widening writers: the 16-bit kind's ring, copies and join; each lane stores one u32 per row, so a row is one
 // 128 B store.  The store writer takes archive 0 of a non-accumulating call, the add writer every later archive.
 template <int KIND>
@@ -1535,6 +1558,126 @@ template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled> : SparseScaled<kK
 template <> struct RowWriter<kKindF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindF16S, kWidenF32 | kAddWriter> {};
 template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindBF16S, kWidenF32 | kAddWriter> {};
 
+// Checking writers (| kCheckFinite; the device-scale sums' last archive): the scaled writer of the same kind with
+// every stored word passed through FiniteCheck::note.
+template <int KIND>
+struct RowWriterScale16Check : RowWriterScale16<KIND>, FiniteCheck<KIND> {
+  typedef RowWriter16<KIND> B;
+  template <int J>
+  __device__ __forceinline__ void write(const typename B::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)this->note(scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    B::out[row * 32u] = (uint16_t)this->note(scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale));
+  }
+};
+template <int KIND>
+struct RowWriterScaleAdd16Check : RowWriterScaleAdd16<KIND>, FiniteCheck<KIND> {
+  typedef RowWriterAdd16<KIND> A;
+  typedef RowWriter16<KIND> B;
+  template <int J>
+  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = (uint16_t)this->note(
+        addWord<KIND>(c.prev[J], scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint16_t* o = B::out + row * 32u;
+    *o = (uint16_t)this->note(addWord<KIND>(*o, scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale)));
+  }
+};
+struct RowWriterScale32Check : RowWriterScale32, FiniteCheck<kKindF32> {
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = note(scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    out[row * 32u] = note(scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale));
+  }
+};
+struct RowWriterScaleAdd32Check : RowWriterScaleAdd32, FiniteCheck<kKindF32> {
+  template <int J>
+  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = note(addWord<kKindF32>(
+        c.prev[J], scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = out + row * 32u;
+    *o = note(addWord<kKindF32>(*o, scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)),
+                                                        scale)));
+  }
+};
+template <int KIND>
+struct RowWriterScaleWiden16Check : RowWriterScaleWiden16<KIND>, FiniteCheck<kKindF32> {
+  typedef RowWriterWiden16<KIND> W;
+  typedef RowWriter16<KIND> B;
+  template <int J>
+  __device__ __forceinline__ void write(const typename W::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = this->note(scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    W::out32[row * 32u] = this->note(scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale));
+  }
+};
+template <int KIND>
+struct RowWriterScaleWidenAdd16Check : RowWriterScaleWidenAdd16<KIND>, FiniteCheck<kKindF32> {
+  typedef RowWriterWidenAdd16<KIND> A;
+  typedef RowWriter16<KIND> B;
+  template <int J>
+  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
+    c.o[J * 32] = this->note(addWord<kKindF32>(c.prev[J], scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale)));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    uint32_t* o = A::out32 + row * 32u;
+    *o = this->note(addWord<kKindF32>(*o, scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale)));
+  }
+};
+// sparse: RowWriterSparseScaled's word and term, noted before it is stored
+template <int WK>
+struct RowWriterSparseScaledCheck : RowWriterSparseScaled<WK & ~kCheckFinite>,
+                                    FiniteCheck<RowWriterSparseScaled<WK & ~kCheckFinite>::R::kSumKind> {
+  typedef RowWriterSparseScaled<WK & ~kCheckFinite> S;
+  typedef typename S::R R;
+  typedef typename S::B B;
+  typedef typename S::T T;
+  template <int J>
+  __device__ __forceinline__ void write(const typename R::Cursor& c, uint32_t entry) const {
+    const uint32_t w = B::word(entry, true);
+    if constexpr (R::kAdd) c.o[J * 32] = (T)this->note(S::combine(c.prev[J], w));
+    else c.o[J * 32] = (T)this->note(S::combine(0u, w));
+  }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
+  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
+    const uint32_t w = B::word(entry, valid);
+    if (valid) {
+      T* o = R::sum + row * 32u;
+      *o = (T)this->note(S::combine(R::kAdd ? (uint32_t)*o : 0u, w));
+    }
+  }
+};
+constexpr int kScaledCheck = kScaled | kCheckFinite;
+template <> struct RowWriter<kKindF16 | kScaledCheck> : RowWriterScale16Check<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kScaledCheck> : RowWriterScale16Check<kKindBF16> {};
+template <> struct RowWriter<kKindF16 | kScaledCheck | kAddWriter> : RowWriterScaleAdd16Check<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kScaledCheck | kAddWriter> : RowWriterScaleAdd16Check<kKindBF16> {};
+template <> struct RowWriter<kKindF32 | kScaledCheck> : RowWriterScale32Check {};
+template <> struct RowWriter<kKindF32 | kScaledCheck | kAddWriter> : RowWriterScaleAdd32Check {};
+template <> struct RowWriter<kKindF16 | kWidenF32 | kScaledCheck> : RowWriterScaleWiden16Check<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaledCheck> : RowWriterScaleWiden16Check<kKindBF16> {};
+template <> struct RowWriter<kKindF16 | kWidenF32 | kScaledCheck | kAddWriter> : RowWriterScaleWidenAdd16Check<kKindF16> {};
+template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaledCheck | kAddWriter> : RowWriterScaleWidenAdd16Check<kKindBF16> {};
+template <int SK, int EXTRA>
+using SparseScaledCheck = RowWriterSparseScaledCheck<SK | kScaledCheck | EXTRA>;
+template <> struct RowWriter<kKindF16S | kScaledCheck> : SparseScaledCheck<kKindF16S, 0> {};
+template <> struct RowWriter<kKindBF16S | kScaledCheck> : SparseScaledCheck<kKindBF16S, 0> {};
+template <> struct RowWriter<kKindF32S | kScaledCheck> : SparseScaledCheck<kKindF32S, 0> {};
+template <> struct RowWriter<kKindF16S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF16S, kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindBF16S, kAddWriter> {};
+template <> struct RowWriter<kKindF32S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF32S, kAddWriter> {};
+template <> struct RowWriter<kKindF16S | kWidenF32 | kScaledCheck> : SparseScaledCheck<kKindF16S, kWidenF32> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaledCheck> : SparseScaledCheck<kKindBF16S, kWidenF32> {};
+template <> struct RowWriter<kKindF16S | kWidenF32 | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF16S, kWidenF32 | kAddWriter> {};
+template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindBF16S, kWidenF32 | kAddWriter> {};
+
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
 // consistent with its word count, and that word count is the group's output size.
 template <int KIND, int PB>
@@ -1551,7 +1694,8 @@ template <int WK, int PB>
 __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, uint32_t block, uint32_t nb,
                                                   const typename Lut<PB, false>::Entry* __restrict__ lut,
                                                   uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
-                                                  uint32_t slotWords, uint32_t lane, float scale) {
+                                                  uint32_t slotWords, uint32_t lane, float scale,
+                                                  float* foundInf) {
   const ArchiveView av = openArchive<reduceArchiveKind(WK)>(in);
   const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
   const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
@@ -1589,18 +1733,27 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
     GmemStream st{stream + words};
     decodeBlockWarp<WK, PB, false>(state, st, blockLen, lut, wr, lane);
   }
+  if constexpr ((WK & kCheckFinite) != 0) {
+    // one vote per block; every lane that saw a non-finite word would store the same 1.0f
+    if (__any_sync(0xffffffffu, wr.bad != 0u) && lane == 0 && foundInf) *foundInf = 1.0f;
+  }
 }
 
 // One pass: archives [a0, a1) of every group.  Member table entry g * width + j = {archive (g, j), out[g],
 // out_size[g], block cap of group g}.  addFirst: archive a0 adds too (accumulate, or a later pass).  Only the
 // first pass (a0 == 0) reports outSuccess.  KIND is the archive kind, | kWidenF32 for fp32 outputs, | kScaled for
-// scaled sums (the scale is im.scale, in every pass).
+// scaled sums (the scale is im.scale, in every pass), | kScaled | kDevScale for device-scale sums
+// (decodeReduceDevScaleKernel: the scale is *scaleDev, read once per CTA in every pass; the writer of archive
+// width - 1, the last pass's last, checks the words it stores and sets *foundInf, when not null, to 1.0f on inf or
+// NaN).  The writers of a device-scale kind are the host-scaled ones: only where s comes from differs.
 template <int KIND, int PB>
-__global__ void __launch_bounds__(kReduceWarps * 32, 4)
-decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
-                   uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
+__device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
+                                                 uint32_t width, uint32_t a0, uint32_t a1, bool addFirst,
+                                                 uint32_t slotWords, uint8_t* __restrict__ outSuccess,
+                                                 const float* scaleDev, float* foundInf) {
   constexpr int AK = reduceArchiveKind(KIND);
-  const float scale = (KIND & kScaled) != 0 ? im.scale : 1.0f;  // the unscaled kinds never read it
+  constexpr bool DEV = (KIND & kDevScale) != 0;
+  constexpr int WK = KIND & ~kDevScale;  // the writer kind of archive 0; | kAddWriter for the others
   constexpr int WARPS = kReduceWarps;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t K = 1u << PB;
@@ -1614,8 +1767,8 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
   unsigned long long* sBar = reinterpret_cast<unsigned long long*>(sMisc + 32);
   uint8_t* sRing = reinterpret_cast<uint8_t*>(sBar + ((WARPS + 1) & ~1));
   constexpr uint32_t ringBytes = kRingSlots * RowWriter<AK>::kRingSlotBytes;
-  static_assert(RowWriter<KIND | kAddWriter>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
-  static_assert(RowWriter<KIND>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
+  static_assert(RowWriter<WK | kAddWriter>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
+  static_assert(RowWriter<WK>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
   uint8_t* sSlots = sRing + WARPS * ringBytes;
   const uint32_t slotBytes = 128u + slotWords * 2u;
 
@@ -1626,8 +1779,13 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
   const uint32_t ring = smemAddr(sRing + warp * ringBytes);
   uint32_t phase = 0;
   if (lane == 0) mbarInit(myBar, 1);
+  if constexpr (DEV) {
+    if (t == 0) sMisc[3] = __float_as_uint(*scaleDev);  // the CTA's one load of the scale
+  }
   fenceBarrierInit();
   __syncthreads();
+  // the unscaled kinds never read it
+  const float scale = DEV ? __uint_as_float(sMisc[3]) : (KIND & kScaled) != 0 ? im.scale : 1.0f;
 
   uint32_t cursor = (uint32_t)((uint64_t)blockIdx.x * groups / gridDim.x);
   for (;;) {
@@ -1701,12 +1859,24 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
       if (work && block < nb) {
         for (uint32_t a = a0; a < a1; ++a) {
           const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
+          if constexpr (DEV) {
+            if (a + 1 == width) {  // the final value of every element: checked
+              if (a == a0 && !addFirst)
+                decodeReduceBlock<WK | kCheckFinite, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase,
+                                                         slotWords, lane, scale, foundInf);
+              else
+                decodeReduceBlock<WK | kCheckFinite | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring,
+                                                                      mySlot, myBar, phase, slotWords, lane, scale,
+                                                                      foundInf);
+              continue;
+            }
+          }
           if (a == a0 && !addFirst)
-            decodeReduceBlock<KIND, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane,
-                                        scale);
+            decodeReduceBlock<WK, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane,
+                                      scale, nullptr);
           else
-            decodeReduceBlock<KIND | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring, mySlot, myBar, phase,
-                                                     slotWords, lane, scale);
+            decodeReduceBlock<WK | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring, mySlot, myBar, phase,
+                                                   slotWords, lane, scale, nullptr);
         }
       }
       block = __shfl_sync(0xffffffffu, nextBlock, 0);
@@ -1716,13 +1886,35 @@ decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, u
 }
 
 template <int KIND, int PB>
+__global__ void __launch_bounds__(kReduceWarps * 32, 4)
+decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
+                   uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
+  static_assert((KIND & kDevScale) == 0, "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, nullptr, nullptr);
+}
+// the device-scale sums (KIND | kScaled | kDevScale): the same body with the scale's and the flag's pointers
+template <int KIND, int PB>
+__global__ void __launch_bounds__(kReduceWarps * 32, 4)
+decodeReduceDevScaleKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups,
+                           uint32_t width, uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords,
+                           uint8_t* __restrict__ outSuccess, const float* __restrict__ scaleDev,
+                           float* __restrict__ foundInf) {
+  static_assert((KIND & (kScaled | kDevScale)) == (kScaled | kDevScale), "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf);
+}
+
+template <int KIND, int PB>
 int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
-                       uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream) {
-  auto kern = decodeReduceKernel<KIND, PB>;
+                       uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream,
+                       const float* scaleDev = nullptr, float* foundInf = nullptr) {
+  constexpr bool DEV = (KIND & kDevScale) != 0;
+  const void* kern;
+  if constexpr (DEV) kern = (const void*)decodeReduceDevScaleKernel<KIND, PB>;
+  else kern = (const void*)decodeReduceKernel<KIND, PB>;
   uint32_t slotWords;
   const size_t smemBytes = decoderSmem<reduceArchiveKind(KIND), PB>(kReduceWarps, opt, &slotWords);
   int perSm = 1;
-  const int rc = residentCtasPerSm((const void*)kern, kReduceWarps * 32, smemBytes, 160 * 1024, &perSm);
+  const int rc = residentCtasPerSm(kern, kReduceWarps * 32, smemBytes, 160 * 1024, &perSm);
   if (rc != DGB_OK) return rc;
   const uint64_t resident = (uint64_t)perSm * smCount();
   const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(resident, totalChunks));
@@ -1730,8 +1922,13 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
     // claim counters and `seen` start at zero in every pass
     DGB_CUDA_TRY(cudaMemsetAsync(sc.next, 0, 8 * (size_t)groups * width, stream));
     timerBegin(opt, kSlotDecode, stream);
-    kern<<<grid, kReduceWarps * 32, smemBytes, stream>>>(sc, im, groups, width, a0, std::min(width, a0 + kReducePass),
-                                                         accumulate || a0 > 0, slotWords, outSuccess);
+    const uint32_t a1 = std::min(width, a0 + kReducePass);
+    if constexpr (DEV)
+      decodeReduceDevScaleKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
+          sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess, scaleDev, foundInf);
+    else
+      decodeReduceKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
+          sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess);
     DGB_CUDA_TRY(cudaGetLastError());
     timerEnd(opt, kSlotDecode, stream);
   }
@@ -1877,9 +2074,11 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
-                 uint8_t* outSuccess_dev, bool sparse, const float* scale, cudaStream_t stream) {
+                 uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
+                 cudaStream_t stream) {
   // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8; scale: null for a plain sum, else
-  // the multiplier of the scaled kinds
+  // the multiplier of the scaled kinds; scaleDev (device memory, read by the kernels) in place of scale for the
+  // device-scale kinds, with the non-finite flag foundInf (may be null)
   if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
   // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
   const int dk = denseKind(kind);
@@ -1930,13 +2129,18 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
     constexpr int KIND = decltype(K)::value;
     constexpr int DK = denseKind(KIND);
-    // the kernel of writer kind WK, or of WK | kScaled
+    // the kernel of writer kind WK, or of WK | kScaled (| kDevScale)
+    // (the device-scale kernels are named last, so that every other kernel is instantiated, and compiled, in the
+    // order it had before they existed)
     auto launch = [&](auto WK) {
       if (scale)
         return launchDecodeReduce<decltype(WK)::value | kScaled, decltype(P)::value>(
             opt, sc, im, groups, width, totalChunks, accumulate, outSuccess_dev, stream);
-      return launchDecodeReduce<decltype(WK)::value, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
-                                                                        accumulate, outSuccess_dev, stream);
+      if (!scaleDev)
+        return launchDecodeReduce<decltype(WK)::value, decltype(P)::value>(opt, sc, im, groups, width, totalChunks,
+                                                                          accumulate, outSuccess_dev, stream);
+      return launchDecodeReduce<decltype(WK)::value | kScaled | kDevScale, decltype(P)::value>(
+          opt, sc, im, groups, width, totalChunks, accumulate, outSuccess_dev, stream, scaleDev, foundInf);
     };
     if constexpr (DK == kKindF16 || DK == kKindBF16) {
       if (widen) return launch(std::integral_constant<int, KIND | kWidenF32>());

@@ -407,12 +407,36 @@ def _scale32(scale) -> Optional[np.float32]:
     return np.float32(scale)
 
 
+def _check_flag_tensor(what: str, t, dev) -> None:
+    """A one-element contiguous float32 CUDA tensor on dev (a device-resident scale, or a non-finite flag)."""
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{what} is a one-element float32 CUDA tensor, not {type(t).__name__}")
+    if t.dtype != torch.float32 or t.numel() != 1 or not t.is_contiguous():
+        raise ValueError(f"{what} is a one-element contiguous float32 tensor, not {t.dtype} with {t.numel()} "
+                         f"element(s){'' if t.is_contiguous() else ', non-contiguous'}")
+    if not t.is_cuda or t.device != dev:
+        raise ValueError(f"{what} must be on the outputs' device {dev}, not {t.device}")
+
+
+def _check_dev_scale(scale32, scale_tensor, found_inf, dev) -> None:
+    """The device-scale keywords of decompress_data_reduce: scale_tensor replaces scale, found_inf needs it."""
+    if scale_tensor is not None and scale32 is not None:
+        raise ValueError("decompress_data_reduce: pass scale or scale_tensor, not both")
+    if found_inf is not None and scale_tensor is None:
+        raise ValueError("decompress_data_reduce: found_inf needs scale_tensor (torch.ones(1) for the unscaled sum)")
+    if scale_tensor is not None:
+        _check_flag_tensor("scale_tensor", scale_tensor, dev)
+    if found_inf is not None:
+        _check_flag_tensor("found_inf", found_inf, dev)
+
+
 def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequence[torch.Tensor],
                            accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
                            out_status: Optional[torch.Tensor] = None, *,
                            prob_bits: int = K_DEFAULT_PRECISION,
                            archive_dtype: Optional[torch.dtype] = None, sparse: bool = False,
-                           scale: Optional[float] = None) -> int:
+                           scale: Optional[float] = None, scale_tensor: Optional[torch.Tensor] = None,
+                           found_inf: Optional[torch.Tensor] = None) -> int:
     """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
@@ -435,8 +459,18 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     while float32 and widening sums keep it in float32.  The result is torch's fold acc = term(x(g, 0)) (or
     ts_out[g] unscaled when accumulating); acc = acc + term(x(g, 1)); ... bit for bit, with archive_dtype and sparse
     too (an elided zero is scaled like any other word, so s < 0 turns +0 into -0).  scale=1.0 gives the unscaled
-    result; None (the default) calls the unscaled entries.  A scale is a host value: a tensor raises TypeError."""
+    result; None (the default) calls the unscaled entries.  A scale is a host value: a tensor raises TypeError.
+
+    scale_tensor (dgb_float_decompress_reduce_scaled_dev): the scale as a one-element float32 CUDA tensor on the
+    outputs' device, e.g. a GradScaler's inverse scale or 1 / the token count of an all-reduce.  The kernels read it
+    when they run, so the host never reads it (no synchronisation) and a CUDA graph replays with its current value.
+    The result is bit for bit this call with scale=float(scale_tensor).  Not with scale.
+    found_inf (with scale_tensor only): a one-element float32 CUDA tensor on the same device, set to 1.0 when any
+    element this call writes ends up inf or NaN, and never cleared (torch.amp's found_inf); with
+    scale_tensor=torch.ones(1) it flags the unscaled sum.  Elements of a group left untouched never count.
+    These keywords raise ValueError before any archive is read."""
     scale32 = _scale32(scale)
+    _check_dev_scale(scale32, scale_tensor, found_inf, ts_out[0].device if len(ts_out) else None)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
@@ -467,6 +501,9 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     extra = ()
     if scale32 is not None:
         entry, extra = L.dgb_float_decompress_reduce_scaled, (float(scale32),)
+    elif scale_tensor is not None:
+        entry = L.dgb_float_decompress_reduce_scaled_dev
+        extra = (scale_tensor.data_ptr(), found_inf.data_ptr() if found_inf is not None else None)
     with torch.cuda.device(dev):
         need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
         tmp = _Temp(temp_mem, need, dev)

@@ -289,6 +289,29 @@ int dgb_float_decompress_reduce_scaled(void* temp_dev, size_t temp_bytes, int fl
                                        const void* const* in, void* const* out, const uint32_t* out_size,
                                        int accumulate, float scale, uint8_t* out_success_dev, void* stream);
 
+/* Device-scale decode-and-sum (new; no reference counterpart): dgb_float_decompress_reduce_scaled with the scale
+ * read from device memory, *scale_dev, by the kernels when they run, and an optional non-finite flag.  For mixed-
+ * precision loss scaling (an inverse loss scale that lives on the device), a per-token normalisation whose token
+ * count comes out of an all-reduce, or a CUDA graph whose scale changes between replays: the host never reads the
+ * scale, the call never synchronises and may be captured, and a replay reads the value *scale_dev holds then.
+ * Everything else is dgb_float_decompress_reduce_scaled's contract with s = *scale_dev: the ten type pairs, the
+ * terms, the fold, the validity rule, statuses, groups with an invalid archive left unwritten, num_groups = 0
+ * returning DGB_OK with nothing written, and the scratch size; the result is bit-identical to that entry called
+ * with the same float.  Every launch of a call (one per 4 archives of a group) reads *scale_dev.
+ * found_inf_dev (may be NULL): set to 1.0f when any output word this call writes ends up inf or NaN (exponent field
+ * all ones).  Only final values are checked: the words the writer of archive W - 1 stores.  Output words this call
+ * leaves alone (past out_size[g], or in a group with an invalid archive) never count.  The flag is never cleared,
+ * as torch.amp's found_inf is not; a non-finite input word, a finite word times an infinite or NaN scale, inf * 0, a
+ * sum that overflows and a non-finite running value taken in by accumulate all set it, since no later term turns
+ * inf or NaN finite.
+ * DGB_ERR_INVALID_ARG before any CUDA call: scale_dev NULL or not 4 B aligned, found_inf_dev not 4 B aligned, and
+ * every argument dgb_float_decompress_reduce_scaled refuses. */
+int dgb_float_decompress_reduce_scaled_dev(void* temp_dev, size_t temp_bytes, int float_type, int out_float_type,
+                                           int prob_bits, uint32_t num_groups, uint32_t archives_per_group,
+                                           const void* const* in, void* const* out, const uint32_t* out_size,
+                                           int accumulate, const float* scale_dev, float* found_inf_dev,
+                                           uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

@@ -15,6 +15,8 @@ the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_AR
 
 --sparse: sparse against dense decode-and-sum (bench_sparse) at zero fractions 0 %, ReLU (about 50 %), 90 % and 99 %.
 --scale: the scaled decode-and-sum against the unscaled one and against scaling the inputs with torch (bench_scale).
+--scale-tensor: the device-scale decode-and-sum with its non-finite flag against the host-scaled one and against
+an unscaled sum followed by torch.amp's unscale-and-check (bench_scale_tensor).
 """
 import argparse
 import json
@@ -305,6 +307,68 @@ def bench_scale(dtype, groups, width, n, iters, out_dtype, sparse):
     return r
 
 
+def bench_scale_tensor(dtype, groups, width, n, iters, out_dtype, sparse):
+    """--scale-tensor, s = fp32(1 / W) held in a one-element CUDA tensor, on the same archives, alternated:
+    (1) the device-scale decode-and-sum with found_inf; (2) the host-scaled one with s = float(s32) (bit-identical to
+    (1), checked); (3) what a GradScaler user does today: the unscaled sum, then
+    torch._amp_foreach_non_finite_check_and_unscale_(outs, found, s32) (bf16 outputs, which it does not take: a
+    torch multiply and isfinite check per output), which multiplies after the sum and so rounds
+    differently (timed only).  Reported: call time of all three; kernel time (timing=1) of (1), (2) and of (3)'s
+    decode-and-sum."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [sparse_data(dtype, n, "relu" if sparse else "0", g) for _ in range(groups * width)]
+    s32 = torch.tensor([1.0 / width], dtype=torch.float32, device="cuda")
+    s = float(s32)
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    comp, sizes, _ = ops.compress_data(True, xs, sparse=sparse)
+    hs = sizes.cpu().tolist()
+    gi = [[comp[k * width + j, :hs[k * width + j]] for j in range(width)] for k in range(groups)]
+    del xs
+    outs = {k: [torch.empty(n, dtype=out_dtype, device="cuda") for _ in range(groups)] for k in ("1", "2", "3")}
+    found = {k: torch.zeros(1, dtype=torch.float32, device="cuda") for k in ("1", "3")}
+
+    def one():
+        ops.decompress_data_reduce(gi, outs["1"], False, temp, archive_dtype=dtype, sparse=sparse, scale_tensor=s32,
+                                   found_inf=found["1"])
+
+    def two():
+        ops.decompress_data_reduce(gi, outs["2"], False, temp, archive_dtype=dtype, sparse=sparse, scale=s)
+
+    def three_sum():
+        ops.decompress_data_reduce(gi, outs["3"], False, temp, archive_dtype=dtype, sparse=sparse)
+
+    def three():
+        three_sum()
+        if out_dtype != torch.bfloat16:
+            torch._amp_foreach_non_finite_check_and_unscale_(outs["3"], found["3"], s32)
+        else:  # torch.amp's fused unscale has no bf16 kernel: the same multiply and check, per output
+            for o in outs["3"]:
+                o.mul_(s32)
+                torch.maximum(found["3"], (~o.isfinite()).any().float(), out=found["3"])
+
+    fns = {"1": one, "2": two, "3": three}
+    for f in fns.values():  # warm-up
+        f()
+    torch.cuda.synchronize()
+    it = torch.int32 if out_dtype == torch.float32 else torch.int16
+    for k in range(groups):
+        assert torch.equal(outs["1"][k].view(it), outs["2"][k].view(it)), k
+    assert float(found["1"].item()) == 0.0 and float(found["3"].item()) == 0.0
+    t = {k: [] for k in fns}
+    for _ in range(3):  # alternate
+        for k, f in fns.items():
+            t[k].append(timed(f, iters))
+    kt = {"1": kernel_us(one, iters), "2": kernel_us(two, iters), "3_sum": kernel_us(three_sum, iters)}
+    r = {"shape": f"{'sparse relu ' if sparse else ''}{str(dtype).split('.')[-1]}->{str(out_dtype).split('.')[-1]} "
+                  f"{groups}x{width}x{n}", "scale": s,
+         "call_us": {k: min(v) for k, v in t.items()}, "call_us_max": {k: max(v) for k, v in t.items()},
+         "kernel_us": kt}
+    r["kernel_dev_over_host"] = kt["1"] / kt["2"]
+    r["call_dev_over_host"] = r["call_us"]["1"] / r["call_us"]["2"]
+    r["call_dev_over_amp"] = r["call_us"]["1"] / r["call_us"]["3"]
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -313,10 +377,19 @@ def main():
                     help="float32: sum the 16-bit shapes' archives into fp32 outputs (bench32)")
     ap.add_argument("--sparse", action="store_true", help="sparse against dense archives (bench_sparse)")
     ap.add_argument("--scale", action="store_true", help="scaled against unscaled sums and torch's scaling (bench_scale)")
+    ap.add_argument("--scale-tensor", action="store_true",
+                    help="device-scale sums with the non-finite flag against host-scaled sums and torch.amp's "
+                         "unscale (bench_scale_tensor)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    if args.scale:
+    if args.scale_tensor:
+        for shape in SCALE_SHAPES:
+            r = bench_scale_tensor(*shape[:4], args.iters, *shape[4:])
+            info["results"].append(r)
+            print(json.dumps(r), flush=True)
+        shapes = []
+    elif args.scale:
         for shape in SCALE_SHAPES:
             r = bench_scale(*shape[:4], args.iters, *shape[4:])
             info["results"].append(r)
