@@ -222,12 +222,20 @@ struct RowWriter16 {
     // low 16 bits (higher bits are dropped by the 16-bit store)
     return __funnelshift_r(__byte_perm(entry, nc, 0x0444), nc, 17);
   }
+  // the joined word of row J of the cursor's group (from the ring), or of any row (from global memory)
+  template <int J>
+  __device__ __forceinline__ uint32_t word(const Cursor& c, uint32_t entry) const {
+    return join(entry, ldsU8<J * 32>(c.s));
+  }
+  __device__ __forceinline__ uint32_t wordSlow(uint32_t row, uint32_t entry) const {
+    return join(entry, __ldg(non + row * 32u));
+  }
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)join(entry, ldsU8<J * 32>(c.s));
+    c.o[J * 32] = (uint16_t)word<J>(c, entry);
   }
   __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    out[row * 32u] = (uint16_t)join(entry, __ldg(non + row * 32u));
+    out[row * 32u] = (uint16_t)wordSlow(row, entry);
   }
 };
 template <> struct RowWriter<kKindF16> : RowWriter16<kKindF16> {};
@@ -298,6 +306,8 @@ struct RowWriterSparse {
     if (keep) asm volatile("ld.shared.u8 %0, [%1];" : "=r"(nc) : "r"(cur + __popc(b & ltMask)));
     return keep ? RowWriter16<BT>::join(entry, nc) : (s == ep ? 0u : 0x8000u);
   }
+  template <int J>
+  __device__ __forceinline__ uint32_t word(const Cursor&, uint32_t entry) const { return word(entry, true); }
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
     c.o[J * 32] = (uint16_t)word(entry, true);
@@ -418,11 +428,18 @@ struct RowWriter<kKindF32> {
     return __funnelshift_r(v, v, 1);
   }
   template <int J>
+  __device__ __forceinline__ uint32_t word(const Cursor& c, uint32_t entry) const {
+    return join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1));
+  }
+  __device__ __forceinline__ uint32_t wordSlow(uint32_t row, uint32_t entry) const {
+    return join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u));
+  }
+  template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1));
+    c.o[J * 32] = word<J>(c, entry);
   }
   __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    out[row * 32u] = join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u));
+    out[row * 32u] = wordSlow(row, entry);
   }
 };
 
@@ -559,6 +576,8 @@ struct RowWriter<kKindF32S> {
     }
     return keep ? RowWriter<kKindF32>::join(entry, lo, hi) : (s == ep ? 0u : 0x80000000u);
   }
+  template <int J>
+  __device__ __forceinline__ uint32_t word(const Cursor&, uint32_t entry) const { return word(entry, true); }
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
     c.o[J * 32] = word(entry, true);
@@ -1164,18 +1183,18 @@ int launchDecodeFused(const Options& opt, const DecodeScratch& sc, const InlineM
 // every archive of the pass in archive order.  Lane l owns the same elements of block k in every archive, so
 // its running sums are its own earlier stores (program order, no atomics, no cross-lane traffic), and the sum
 // order per element is fixed whatever the grid, the claims or the passes: the result is bit-reproducible.
-// The first archive of an accumulate=0 call is stored verbatim (the ordinary writer); every later one goes
-// through an add writer that loads the 16 running sums of a row group when the group starts (once per group
-// instead of once per row on the decode loop), adds, and stores.
+// The first archive of an accumulate=0 call is stored verbatim (the archive kind's own writer); every later one
+// goes through an add writer (RowWriterSum, below: one writer built from the kind's flags for every decode-and-sum
+// writer kind), which loads the 16 running sums of a row group when the group starts (once per group instead of
+// once per row on the decode loop), adds, and stores.
 // LUTs cost shared memory, so at most kReducePass archives are decoded per launch; the host issues
 // ceil(W / kReducePass) launches in order and every launch after the first accumulates (DESIGN.md section 3).
 // Widening sums (dgb_float_decompress_reduce_to): fp16 / bf16 archives summed into fp32 outputs.  The kernel's
 // kind is then the archive kind | kWidenF32; every decoded word is converted exactly to fp32 and each add is one
 // fp32 round-to-nearest-even add, which is torch's acc.float() + x.float() fold.
 // Sparse sums (dgb_float_decompress_reduce_sparse): archives of type 5, 6 or 8 into outputs of the dense type, or
-// types 5 and 6 into fp32.  The kernel's kind is then the sparse kind (| kWidenF32); its writers take each word
-// from the sparse decoder's writer and add it as the dense writers do, so the result is the dense sum of the same
-// words bit for bit.
+// types 5 and 6 into fp32.  The kernel's kind is then the sparse kind (| kWidenF32); each word comes from the sparse
+// decoder's writer and is added as a dense word is, so the result is the dense sum of the same words bit for bit.
 // Scaled sums (dgb_float_decompress_reduce_scaled): any of the ten kinds above | kScaled.  Every writer, the store
 // of archive 0 included, replaces the decoded word x by its term s(x) (scaleWord / scaleWiden) before it stores or
 // adds it; the running sum an add writer loads is not scaled.  The scale is a kernel parameter (InlineMembers::scale)
@@ -1211,54 +1230,6 @@ __device__ __forceinline__ uint32_t ldGlobalU32(const uint32_t* p) {
   asm volatile("ld.global.u32 %0, [%1];" : "=r"(v) : "l"(__cvta_generic_to_global(p)));
   return v;
 }
-
-template <int KIND>
-struct RowWriterAdd16 : RowWriter16<KIND> {
-  typedef RowWriter16<KIND> B;
-  struct Cursor { uint16_t* o; uint32_t s; uint32_t prev[kGroupRows]; };
-  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
-    Cursor c;
-    c.o = B::out + row * 32u;
-    c.s = B::ring + slot * B::kRingSlotBytes + B::lane;
-#pragma unroll
-    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU16(c.o + j * 32);
-    return c;
-  }
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)addWord<KIND>(c.prev[J], B::join(entry, ldsU8<J * 32>(c.s)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint16_t* o = B::out + row * 32u;
-    *o = (uint16_t)addWord<KIND>(*o, B::join(entry, __ldg(B::non + row * 32u)));
-  }
-};
-template <> struct RowWriter<kKindF16 | kAddWriter> : RowWriterAdd16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kAddWriter> : RowWriterAdd16<kKindBF16> {};
-
-template <>
-struct RowWriter<kKindF32 | kAddWriter> : RowWriter<kKindF32> {
-  typedef RowWriter<kKindF32> B;
-  struct Cursor { uint32_t* o; uint32_t s2, s1; uint32_t prev[kGroupRows]; };
-  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
-    const typename B::Cursor b = B::at(row, slot);
-    Cursor c;
-    c.o = b.o;
-    c.s2 = b.s2;
-    c.s1 = b.s1;
-#pragma unroll
-    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU32(c.o + j * 32);
-    return c;
-  }
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = addWord<kKindF32>(c.prev[J], join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = out + row * 32u;
-    *o = addWord<kKindF32>(*o, join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)));
-  }
-};
 
 // The exact fp32 value of a joined fp16 / bf16 word.  join leaves garbage above bit 15 (the 16-bit store drops
 // it), so the widening takes the low half only.
@@ -1313,370 +1284,99 @@ struct FiniteCheck {
     return w;
   }
 };
-// Widening writers: the 16-bit kind's ring, copies and join; each lane stores one u32 per row, so a row is one
-// 128 B store.  The store writer takes archive 0 of a non-accumulating call, the add writer every later archive.
-template <int KIND>
-struct RowWriterWiden16 : RowWriter16<KIND> {
-  typedef RowWriter16<KIND> B;
-  uint32_t* out32;
-  struct Cursor { uint32_t* o; uint32_t s; };
-  __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
-    B::setBlock(av, outBase, block, l);
-    out32 = static_cast<uint32_t*>(outBase) + (size_t)block * kBlockBytes + l;
-    __builtin_assume(__isGlobal(out32));
-  }
-  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
-    return Cursor{out32 + row * 32u, B::ring + slot * B::kRingSlotBytes + B::lane};
-  }
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = widenWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    out32[row * 32u] = widenWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)));
-  }
-};
+struct NoFiniteCheck { static __device__ __forceinline__ uint32_t note(uint32_t w) { return w; } };
+template <bool SCALED>
+struct SumScale { static constexpr float scale = 1.0f; };  // unscaled sums: combine ignores it
+template <>
+struct SumScale<true> { float scale; };  // the call's scale; decodeReduceBlock sets it
 
-template <int KIND>
-struct RowWriterWidenAdd16 : RowWriterWiden16<KIND> {
-  typedef RowWriterWiden16<KIND> W;
-  typedef RowWriter16<KIND> B;
-  struct Cursor { uint32_t* o; uint32_t s; uint32_t prev[kGroupRows]; };
-  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
-    Cursor c;
-    c.o = W::out32 + row * 32u;
-    c.s = B::ring + slot * B::kRingSlotBytes + B::lane;
-#pragma unroll
-    for (int j = 0; j < kGroupRows; ++j) c.prev[j] = ldGlobalU32(c.o + j * 32);
-    return c;
-  }
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = addWord<kKindF32>(c.prev[J], widenWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s))));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = W::out32 + row * 32u;
-    *o = addWord<kKindF32>(*o, widenWord<KIND>(B::join(entry, __ldg(B::non + row * 32u))));
-  }
-};
-template <> struct RowWriter<kKindF16 | kWidenF32> : RowWriterWiden16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32> : RowWriterWiden16<kKindBF16> {};
-template <> struct RowWriter<kKindF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32 | kAddWriter> : RowWriterWidenAdd16<kKindBF16> {};
+// the kind in which a decode-and-sum writer kind adds, which is also the type it stores
+__host__ __device__ constexpr int reduceSumKind(int wk) {
+  return (wk & kWidenF32) != 0 ? kKindF32 : denseKind(reduceArchiveKind(wk));
+}
 
-// Sparse decode-and-sum writers (dgb_float_decompress_reduce_sparse): the sparse kind's word (its ring, segment copy
-// or windows, and kept-word cursor), then the dense kind's add, widening or widening add.  An elided word is the +0
-// or -0 it stands for and goes through the add like any other (-0 + -0 = -0, -0 + +0 = +0).  word() votes across
-// the warp, so every row, the partial one too, runs on the whole warp.  WK = the sparse kind | kAddWriter and / or
-// | kWidenF32 (fp32 outputs of types 5 and 6); the plain store of archive 0 is the sparse decoder's own writer.
+// The decode-and-sum writer of writer kind WK: the archive kind's writer B (its ring, copies and join; a sparse
+// kind's segment copy or windows and kept-word cursor) and four steps on every word it decodes:
+//   1. the word w from B: word<J> from the ring, wordSlow from global memory (a sparse kind's elided word is the
+//      +0 or -0 it stands for and goes through the steps below like any other: -0 + -0 = -0, -0 + +0 = +0);
+//   2. the term: w, or w widened exactly to fp32 (| kWidenF32: widenWord), or w times the call's scale
+//      (| kScaled: scaleWord in the archive's dense type, scaleWiden when widening);
+//   3. (| kAddWriter) the term added to the element's running sum with one addWord in the sum kind;
+//   4. (| kCheckFinite) the result noted by FiniteCheck before it is stored.
+// It stores one u16 (same-type fp16 / bf16 sums) or one u32 (fp32 and widening sums: a row is one 128 B store)
+// per element.  Add writers load a row group's running sums when the group starts (volatile loads in at(), so they
+// are issued there), writeSlow and writePartial the one sum they add to.  A sparse word votes across the warp, so
+// sparse rows, the partial one too (writePartial), run on the whole warp, and the vote comes before the running
+// sum is read.  The unscaled store of archive 0 (WK = the bare archive kind) is the archive kind's own writer.
 template <int WK>
-struct RowWriterSparseReduce : RowWriter<reduceArchiveKind(WK)> {
+struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
+                      SumScale<(WK & kScaled) != 0>,
+                      std::conditional<(WK & kCheckFinite) != 0, FiniteCheck<reduceSumKind(WK)>, NoFiniteCheck>::type {
   typedef RowWriter<reduceArchiveKind(WK)> B;
-  static constexpr int BT = denseKind(reduceArchiveKind(WK));
+  static constexpr int AK = reduceArchiveKind(WK), kSumKind = reduceSumKind(WK);
   static constexpr bool kAdd = (WK & kAddWriter) != 0, kWiden = (WK & kWidenF32) != 0;
-  static constexpr int kSumKind = kWiden ? kKindF32 : BT;  // the output words' type, in which the adds are taken
+  static constexpr bool kScale = (WK & kScaled) != 0;
   typedef typename std::conditional<kSumKind == kKindF32, uint32_t, uint16_t>::type T;
   T* sum;
-  struct Cursor { T* o; uint32_t prev[kGroupRows]; };
+  struct Cursor {
+    T* o;
+    typename B::Cursor in;      // B's cursor of the group: its ring addresses (its output pointer goes unused)
+    uint32_t prev[kGroupRows];  // add writers: the running sums of the group's rows
+  };
   __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
     B::setBlock(av, outBase, block, l);
     sum = static_cast<T*>(outBase) + (size_t)block * kBlockBytes + l;
     __builtin_assume(__isGlobal(sum));
   }
-  static __device__ __forceinline__ uint32_t value(uint32_t w) {
-    if constexpr (kWiden) return widenWord<BT>(w);
-    else return w;
-  }
-  // the output word from the running sum `prev` (ignored by the store writer) and the decoded word `w`
-  static __device__ __forceinline__ T combine(uint32_t prev, uint32_t w) {
-    if constexpr (kAdd) return (T)addWord<kSumKind>(prev, value(w));
-    else return (T)value(w);
-  }
-  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t) const {
-    Cursor c;
-    c.o = sum + row * 32u;
+  __device__ __forceinline__ Cursor at(uint32_t row, uint32_t slot) const {
+    Cursor c{sum + row * 32u, B::at(row, slot)};
     if constexpr (kAdd) {
 #pragma unroll
-      for (int j = 0; j < kGroupRows; ++j)
-        c.prev[j] = sizeof(T) == 4 ? ldGlobalU32(reinterpret_cast<const uint32_t*>(c.o + j * 32))
-                                   : ldGlobalU16(reinterpret_cast<const uint16_t*>(c.o + j * 32));
+      for (int j = 0; j < kGroupRows; ++j) {
+        if constexpr (sizeof(T) == 4) c.prev[j] = ldGlobalU32(c.o + j * 32);
+        else c.prev[j] = ldGlobalU16(c.o + j * 32);
+      }
     }
     return c;
   }
+  // steps 2 and 3 (prev: add writers only); this->note() around it is step 4.  Static, as are the unscaled scale and
+  // the unchecked note: passing the writer into the store path makes the sparse fp32 add writer spill more
+  static __device__ __forceinline__ uint32_t combine(uint32_t prev, uint32_t w, float s) {
+    uint32_t v = w;
+    if constexpr (kScale && kWiden) v = scaleWiden<denseKind(AK)>(w, s);
+    else if constexpr (kScale) v = scaleWord<denseKind(AK)>(w, s);
+    else if constexpr (kWiden) v = widenWord<denseKind(AK)>(w);
+    if constexpr (kAdd) v = addWord<kSumKind>(prev, v);
+    return v;
+  }
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    const uint32_t w = B::word(entry, true);
-    if constexpr (kAdd) c.o[J * 32] = combine(c.prev[J], w);
-    else c.o[J * 32] = combine(0u, w);
+    c.o[J * 32] = (T)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
   }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
+  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
+    if constexpr (isSparseKind(AK)) {
+      writePartial(row, entry, true);
+    } else if constexpr (kAdd) {
+      T* o = sum + row * 32u;
+      *o = (T)this->note(combine(*o, B::wordSlow(row, entry), this->scale));
+    } else {
+      sum[row * 32u] = (T)this->note(combine(0u, B::wordSlow(row, entry), this->scale));
+    }
+  }
+  // sparse kinds: every lane takes part in the word's vote; lanes with valid = false store nothing
   __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
     const uint32_t w = B::word(entry, valid);
     if (valid) {
       T* o = sum + row * 32u;
-      *o = combine(kAdd ? (uint32_t)*o : 0u, w);
+      *o = (T)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
     }
   }
 };
-template <> struct RowWriter<kKindF16S | kAddWriter> : RowWriterSparseReduce<kKindF16S | kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kAddWriter> : RowWriterSparseReduce<kKindBF16S | kAddWriter> {};
-template <> struct RowWriter<kKindF32S | kAddWriter> : RowWriterSparseReduce<kKindF32S | kAddWriter> {};
-template <> struct RowWriter<kKindF16S | kWidenF32> : RowWriterSparseReduce<kKindF16S | kWidenF32> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32> : RowWriterSparseReduce<kKindBF16S | kWidenF32> {};
-template <> struct RowWriter<kKindF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindF16S | kWidenF32 | kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32 | kAddWriter> : RowWriterSparseReduce<kKindBF16S | kWidenF32 | kAddWriter> {};
-
-// Scaled writers (| kScaled): the unscaled writer of the same kind with the term s(x) in place of the decoded word
-// x.  Each keeps its base's ring, copies, cursor and running-sum loads, and has its own `scale` (decodeReduceBlock
-// sets it).
+// every writer kind other than the bare archive kinds, whose own writers are above
 template <int KIND>
-struct RowWriterScale16 : RowWriter16<KIND> {
-  typedef RowWriter16<KIND> B;
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const typename B::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale);
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    B::out[row * 32u] = (uint16_t)scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale);
-  }
+struct RowWriter : RowWriterSum<KIND> {
+  static_assert((KIND & (kAddWriter | kWidenF32 | kScaled | kCheckFinite)) != 0, "not a decode-and-sum writer kind");
 };
-template <int KIND>
-struct RowWriterScaleAdd16 : RowWriterAdd16<KIND> {
-  typedef RowWriterAdd16<KIND> A;
-  typedef RowWriter16<KIND> B;
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)addWord<KIND>(c.prev[J], scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint16_t* o = B::out + row * 32u;
-    *o = (uint16_t)addWord<KIND>(*o, scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale));
-  }
-};
-struct RowWriterScale32 : RowWriter<kKindF32> {
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale);
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    out[row * 32u] = scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale);
-  }
-};
-struct RowWriterScaleAdd32 : RowWriter<kKindF32 | kAddWriter> {
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = addWord<kKindF32>(c.prev[J], scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)),
-                                                                   scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = out + row * 32u;
-    *o = addWord<kKindF32>(*o, scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale));
-  }
-};
-template <int KIND>
-struct RowWriterScaleWiden16 : RowWriterWiden16<KIND> {
-  typedef RowWriterWiden16<KIND> W;
-  typedef RowWriter16<KIND> B;
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const typename W::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale);
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    W::out32[row * 32u] = scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale);
-  }
-};
-template <int KIND>
-struct RowWriterScaleWidenAdd16 : RowWriterWidenAdd16<KIND> {
-  typedef RowWriterWidenAdd16<KIND> A;
-  typedef RowWriter16<KIND> B;
-  float scale;
-  template <int J>
-  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = addWord<kKindF32>(c.prev[J], scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = A::out32 + row * 32u;
-    *o = addWord<kKindF32>(*o, scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), scale));
-  }
-};
-template <> struct RowWriter<kKindF16 | kScaled> : RowWriterScale16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kScaled> : RowWriterScale16<kKindBF16> {};
-template <> struct RowWriter<kKindF16 | kScaled | kAddWriter> : RowWriterScaleAdd16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kScaled | kAddWriter> : RowWriterScaleAdd16<kKindBF16> {};
-template <> struct RowWriter<kKindF32 | kScaled> : RowWriterScale32 {};
-template <> struct RowWriter<kKindF32 | kScaled | kAddWriter> : RowWriterScaleAdd32 {};
-template <> struct RowWriter<kKindF16 | kWidenF32 | kScaled> : RowWriterScaleWiden16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaled> : RowWriterScaleWiden16<kKindBF16> {};
-template <> struct RowWriter<kKindF16 | kWidenF32 | kScaled | kAddWriter> : RowWriterScaleWidenAdd16<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaled | kAddWriter> : RowWriterScaleWidenAdd16<kKindBF16> {};
-// Sparse: RowWriterSparseReduce's word, cursor and running sums with the term in place of the word, for archive 0
-// as well (the sparse decoder's own writer stores unscaled words).  WK = the sparse kind | kScaled, | kAddWriter
-// and / or | kWidenF32.
-template <int WK>
-struct RowWriterSparseScaled : RowWriterSparseReduce<WK & ~kScaled> {
-  typedef RowWriterSparseReduce<WK & ~kScaled> R;
-  typedef typename R::B B;
-  typedef typename R::T T;
-  float scale;
-  __device__ __forceinline__ T combine(uint32_t prev, uint32_t w) const {
-    uint32_t v;
-    if constexpr (R::kWiden) v = scaleWiden<R::BT>(w, scale);
-    else v = scaleWord<R::BT>(w, scale);
-    if constexpr (R::kAdd) return (T)addWord<R::kSumKind>(prev, v);
-    else return (T)v;
-  }
-  template <int J>
-  __device__ __forceinline__ void write(const typename R::Cursor& c, uint32_t entry) const {
-    const uint32_t w = B::word(entry, true);
-    if constexpr (R::kAdd) c.o[J * 32] = combine(c.prev[J], w);
-    else c.o[J * 32] = combine(0u, w);
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
-  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
-    const uint32_t w = B::word(entry, valid);
-    if (valid) {
-      T* o = R::sum + row * 32u;
-      *o = combine(R::kAdd ? (uint32_t)*o : 0u, w);
-    }
-  }
-};
-template <int SK, int EXTRA>
-using SparseScaled = RowWriterSparseScaled<SK | kScaled | EXTRA>;
-template <> struct RowWriter<kKindF16S | kScaled> : SparseScaled<kKindF16S, 0> {};
-template <> struct RowWriter<kKindBF16S | kScaled> : SparseScaled<kKindBF16S, 0> {};
-template <> struct RowWriter<kKindF32S | kScaled> : SparseScaled<kKindF32S, 0> {};
-template <> struct RowWriter<kKindF16S | kScaled | kAddWriter> : SparseScaled<kKindF16S, kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kScaled | kAddWriter> : SparseScaled<kKindBF16S, kAddWriter> {};
-template <> struct RowWriter<kKindF32S | kScaled | kAddWriter> : SparseScaled<kKindF32S, kAddWriter> {};
-template <> struct RowWriter<kKindF16S | kWidenF32 | kScaled> : SparseScaled<kKindF16S, kWidenF32> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled> : SparseScaled<kKindBF16S, kWidenF32> {};
-template <> struct RowWriter<kKindF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindF16S, kWidenF32 | kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaled | kAddWriter> : SparseScaled<kKindBF16S, kWidenF32 | kAddWriter> {};
-
-// Checking writers (| kCheckFinite; the device-scale sums' last archive): the scaled writer of the same kind with
-// every stored word passed through FiniteCheck::note.
-template <int KIND>
-struct RowWriterScale16Check : RowWriterScale16<KIND>, FiniteCheck<KIND> {
-  typedef RowWriter16<KIND> B;
-  template <int J>
-  __device__ __forceinline__ void write(const typename B::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)this->note(scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    B::out[row * 32u] = (uint16_t)this->note(scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale));
-  }
-};
-template <int KIND>
-struct RowWriterScaleAdd16Check : RowWriterScaleAdd16<KIND>, FiniteCheck<KIND> {
-  typedef RowWriterAdd16<KIND> A;
-  typedef RowWriter16<KIND> B;
-  template <int J>
-  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (uint16_t)this->note(
-        addWord<KIND>(c.prev[J], scaleWord<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint16_t* o = B::out + row * 32u;
-    *o = (uint16_t)this->note(addWord<KIND>(*o, scaleWord<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale)));
-  }
-};
-struct RowWriterScale32Check : RowWriterScale32, FiniteCheck<kKindF32> {
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = note(scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    out[row * 32u] = note(scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)), scale));
-  }
-};
-struct RowWriterScaleAdd32Check : RowWriterScaleAdd32, FiniteCheck<kKindF32> {
-  template <int J>
-  __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = note(addWord<kKindF32>(
-        c.prev[J], scaleWord<kKindF32>(join(entry, ldsU16<J * 64>(c.s2), ldsU8<J * 32>(c.s1)), scale)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = out + row * 32u;
-    *o = note(addWord<kKindF32>(*o, scaleWord<kKindF32>(join(entry, __ldg(non2 + row * 32u), __ldg(non1 + row * 32u)),
-                                                        scale)));
-  }
-};
-template <int KIND>
-struct RowWriterScaleWiden16Check : RowWriterScaleWiden16<KIND>, FiniteCheck<kKindF32> {
-  typedef RowWriterWiden16<KIND> W;
-  typedef RowWriter16<KIND> B;
-  template <int J>
-  __device__ __forceinline__ void write(const typename W::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = this->note(scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    W::out32[row * 32u] = this->note(scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale));
-  }
-};
-template <int KIND>
-struct RowWriterScaleWidenAdd16Check : RowWriterScaleWidenAdd16<KIND>, FiniteCheck<kKindF32> {
-  typedef RowWriterWidenAdd16<KIND> A;
-  typedef RowWriter16<KIND> B;
-  template <int J>
-  __device__ __forceinline__ void write(const typename A::Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = this->note(addWord<kKindF32>(c.prev[J], scaleWiden<KIND>(B::join(entry, ldsU8<J * 32>(c.s)), this->scale)));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
-    uint32_t* o = A::out32 + row * 32u;
-    *o = this->note(addWord<kKindF32>(*o, scaleWiden<KIND>(B::join(entry, __ldg(B::non + row * 32u)), this->scale)));
-  }
-};
-// sparse: RowWriterSparseScaled's word and term, noted before it is stored
-template <int WK>
-struct RowWriterSparseScaledCheck : RowWriterSparseScaled<WK & ~kCheckFinite>,
-                                    FiniteCheck<RowWriterSparseScaled<WK & ~kCheckFinite>::R::kSumKind> {
-  typedef RowWriterSparseScaled<WK & ~kCheckFinite> S;
-  typedef typename S::R R;
-  typedef typename S::B B;
-  typedef typename S::T T;
-  template <int J>
-  __device__ __forceinline__ void write(const typename R::Cursor& c, uint32_t entry) const {
-    const uint32_t w = B::word(entry, true);
-    if constexpr (R::kAdd) c.o[J * 32] = (T)this->note(S::combine(c.prev[J], w));
-    else c.o[J * 32] = (T)this->note(S::combine(0u, w));
-  }
-  __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const { writePartial(row, entry, true); }
-  __device__ __forceinline__ void writePartial(uint32_t row, uint32_t entry, bool valid) const {
-    const uint32_t w = B::word(entry, valid);
-    if (valid) {
-      T* o = R::sum + row * 32u;
-      *o = (T)this->note(S::combine(R::kAdd ? (uint32_t)*o : 0u, w));
-    }
-  }
-};
-constexpr int kScaledCheck = kScaled | kCheckFinite;
-template <> struct RowWriter<kKindF16 | kScaledCheck> : RowWriterScale16Check<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kScaledCheck> : RowWriterScale16Check<kKindBF16> {};
-template <> struct RowWriter<kKindF16 | kScaledCheck | kAddWriter> : RowWriterScaleAdd16Check<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kScaledCheck | kAddWriter> : RowWriterScaleAdd16Check<kKindBF16> {};
-template <> struct RowWriter<kKindF32 | kScaledCheck> : RowWriterScale32Check {};
-template <> struct RowWriter<kKindF32 | kScaledCheck | kAddWriter> : RowWriterScaleAdd32Check {};
-template <> struct RowWriter<kKindF16 | kWidenF32 | kScaledCheck> : RowWriterScaleWiden16Check<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaledCheck> : RowWriterScaleWiden16Check<kKindBF16> {};
-template <> struct RowWriter<kKindF16 | kWidenF32 | kScaledCheck | kAddWriter> : RowWriterScaleWidenAdd16Check<kKindF16> {};
-template <> struct RowWriter<kKindBF16 | kWidenF32 | kScaledCheck | kAddWriter> : RowWriterScaleWidenAdd16Check<kKindBF16> {};
-template <int SK, int EXTRA>
-using SparseScaledCheck = RowWriterSparseScaledCheck<SK | kScaledCheck | EXTRA>;
-template <> struct RowWriter<kKindF16S | kScaledCheck> : SparseScaledCheck<kKindF16S, 0> {};
-template <> struct RowWriter<kKindBF16S | kScaledCheck> : SparseScaledCheck<kKindBF16S, 0> {};
-template <> struct RowWriter<kKindF32S | kScaledCheck> : SparseScaledCheck<kKindF32S, 0> {};
-template <> struct RowWriter<kKindF16S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF16S, kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindBF16S, kAddWriter> {};
-template <> struct RowWriter<kKindF32S | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF32S, kAddWriter> {};
-template <> struct RowWriter<kKindF16S | kWidenF32 | kScaledCheck> : SparseScaledCheck<kKindF16S, kWidenF32> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaledCheck> : SparseScaledCheck<kKindBF16S, kWidenF32> {};
-template <> struct RowWriter<kKindF16S | kWidenF32 | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindF16S, kWidenF32 | kAddWriter> {};
-template <> struct RowWriter<kKindBF16S | kWidenF32 | kScaledCheck | kAddWriter> : SparseScaledCheck<kKindBF16S, kWidenF32 | kAddWriter> {};
 
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
 // consistent with its word count, and that word count is the group's output size.
@@ -1739,6 +1439,18 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
   }
 }
 
+// f(std::integral_constant<int, K>()) with K the writer kind of one archive: WK when it is stored (archive a0 of a
+// pass that does not add), WK | kAddWriter when it is added; | kCheckFinite as well when it is checked (CHECK kinds
+// only, so the others instantiate no checking writer)
+template <int WK, bool CHECK, typename F>
+__device__ __forceinline__ void withWriterKind(bool store, bool check, F&& f) {
+  if constexpr (CHECK) {
+    if (check) return withWriterKind<WK | kCheckFinite, false>(store, false, f);
+  }
+  if (store) f(std::integral_constant<int, WK>());
+  else f(std::integral_constant<int, WK | kAddWriter>());
+}
+
 // One pass: archives [a0, a1) of every group.  Member table entry g * width + j = {archive (g, j), out[g],
 // out_size[g], block cap of group g}.  addFirst: archive a0 adds too (accumulate, or a later pass).  Only the
 // first pass (a0 == 0) reports outSuccess.  KIND is the archive kind, | kWidenF32 for fp32 outputs, | kScaled for
@@ -1766,9 +1478,7 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
   uint32_t* sMisc = sWarp + 32;
   unsigned long long* sBar = reinterpret_cast<unsigned long long*>(sMisc + 32);
   uint8_t* sRing = reinterpret_cast<uint8_t*>(sBar + ((WARPS + 1) & ~1));
-  constexpr uint32_t ringBytes = kRingSlots * RowWriter<AK>::kRingSlotBytes;
-  static_assert(RowWriter<WK | kAddWriter>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
-  static_assert(RowWriter<WK>::kRingSlotBytes == RowWriter<AK>::kRingSlotBytes, "");
+  constexpr uint32_t ringBytes = kRingSlots * RowWriter<AK>::kRingSlotBytes;  // every writer kind's: RowWriterSum's base
   uint8_t* sSlots = sRing + WARPS * ringBytes;
   const uint32_t slotBytes = 128u + slotWords * 2u;
 
@@ -1859,24 +1569,12 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
       if (work && block < nb) {
         for (uint32_t a = a0; a < a1; ++a) {
           const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
-          if constexpr (DEV) {
-            if (a + 1 == width) {  // the final value of every element: checked
-              if (a == a0 && !addFirst)
-                decodeReduceBlock<WK | kCheckFinite, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase,
-                                                         slotWords, lane, scale, foundInf);
-              else
-                decodeReduceBlock<WK | kCheckFinite | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring,
-                                                                      mySlot, myBar, phase, slotWords, lane, scale,
-                                                                      foundInf);
-              continue;
-            }
-          }
-          if (a == a0 && !addFirst)
-            decodeReduceBlock<WK, PB>(in, gd.out, block, nb, lut[0], ring, mySlot, myBar, phase, slotWords, lane,
-                                      scale, nullptr);
-          else
-            decodeReduceBlock<WK | kAddWriter, PB>(in, gd.out, block, nb, lut[a - a0], ring, mySlot, myBar, phase,
-                                                   slotWords, lane, scale, nullptr);
+          // the device-scale sums check archive width - 1: the final value of every element
+          withWriterKind<WK, DEV>(a == a0 && !addFirst, a + 1 == width, [&](auto wk) {
+            constexpr int W = decltype(wk)::value;
+            decodeReduceBlock<W, PB>(in, gd.out, block, nb, lut[(W & kAddWriter) != 0 ? a - a0 : 0u], ring, mySlot,
+                                     myBar, phase, slotWords, lane, scale, foundInf);
+          });
         }
       }
       block = __shfl_sync(0xffffffffu, nextBlock, 0);
