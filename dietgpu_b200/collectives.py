@@ -71,6 +71,12 @@ def pack_offsets(sizes: Sequence[int]) -> Tuple[List[int], int]:
     return offs, o
 
 
+def _pieces(members: int, stages: int) -> List[Tuple[int, int]]:
+    """The non-empty member ranges [a, b) of a cut of `members` into `stages` nearly equal pipeline pieces."""
+    cuts = [round(k * members / stages) for k in range(stages + 1)]
+    return [(a, b) for a, b in zip(cuts[:-1], cuts[1:]) if b > a]
+
+
 class _Exchange:
     """One in-flight archive exchange (all-gather of every rank's packed archives)."""
 
@@ -251,9 +257,7 @@ def _all_gather_push(flat: torch.Tensor, as_float: bool, bounds: List[int], ws: 
     off = ws.begin((world + 1) * region)  # [own archives | inbox of source 0 | ... | inbox of source world-1]
     out = torch.empty(world * n, dtype=flat.dtype, device=dev)
     mine = ws.view(rank, off, region).view(members, cols)
-    stages = max(1, min(int(stages), members, 7))
-    cuts = [round(k * members / stages) for k in range(stages + 1)]
-    groups = [(a, b) for a, b in zip(cuts[:-1], cuts[1:]) if b > a]
+    groups = _pieces(members, max(1, min(int(stages), members, 7)))  # one flag channel per group
     cur = torch.cuda.current_stream(dev)
     peers = [(rank + k) % world for k in range(1, world)]
     sizes = torch.empty(members, dtype=torch.int32, device=dev)
@@ -297,15 +301,13 @@ def _all_gather_peer(flat: torch.Tensor, as_float: bool, bounds: List[int], ws: 
     ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(members)], checksum, temp_mem, mine, sizes)
     ws.barrier()  # every rank's archives are complete (and every rank is done with the previous call's other half)
     out[rank * n:(rank + 1) * n].copy_(flat)  # own shard: a local copy, no codec
-    stages = max(1, min(int(stages), members))
-    cuts = [round(k * members / stages) for k in range(stages + 1)]
+    pieces = _pieces(members, max(1, min(int(stages), members)))
     units = []
     for k in range(1, world):
         w = (rank + k) % world  # start with a different peer on every rank: spreads the pulls over the links
         rows = ws.view(w, off, members * cols).view(members, cols)
-        for a, b in zip(cuts[:-1], cuts[1:]):
-            if b > a:
-                units.append((rows[a:b], [out[w * n + bounds[i]: w * n + bounds[i + 1]] for i in range(a, b)]))
+        for a, b in pieces:
+            units.append((rows[a:b], [out[w * n + bounds[i]: w * n + bounds[i + 1]] for i in range(a, b)]))
     if units:
         _pull_and_decode(ws, as_float, flat.dtype, units, cols, checksum, temp_mem, check, direct)
     return out
@@ -393,9 +395,7 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
         return out if as_float else out.view(t.dtype)
     world = _world(group)
     out = torch.empty(world * n, dtype=wire_dtype or flat.dtype, device=t.device)
-    stages = max(1, min(int(stages), members))
-    cuts = [round(k * members / stages) for k in range(stages + 1)]
-    pieces = [(cuts[k], cuts[k + 1]) for k in range(stages) if cuts[k + 1] > cuts[k]]
+    pieces = _pieces(members, max(1, min(int(stages), members)))
 
     def compress(a, b):
         comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem,
@@ -472,6 +472,36 @@ def _all_to_all_bytes(send: torch.Tensor, send_sizes: List[int], recv_sizes: Lis
     return host.to(send.device)
 
 
+def _send_to_each(per_dest: List[List[torch.Tensor]], group,
+                  extra: Optional[List[int]] = None) -> Tuple[List[List[torch.Tensor]], Optional[List[int]]]:
+    """Send the archives per_dest[d] (m exact-length uint8 tensors on one device for every d; an empty tensor sends
+    nothing) to rank d.  Returns (per_src, extra_in): per_src[s] = the m archives rank s sent here, views into one
+    receive buffer on the same device, and extra_in[s] = extra[this rank] of rank s (None without extra).
+    Two all_to_all_single calls: the int64 table of archive sizes (and extras), then the archives packed 16 B
+    aligned, so each link carries only its own bytes.  The one host synchronisation is the read of the received
+    table."""
+    m = len(per_dest[0])
+    dev = per_dest[0][0].device
+    on_device = _device_collectives(group)
+    table = [[a.numel() for a in row] + ([] if extra is None else [int(extra[d])]) for d, row in enumerate(per_dest)]
+    table_out = torch.tensor(table, dtype=torch.int64).to(dev if on_device else torch.device("cpu"))
+    table_in = torch.empty_like(table_out)
+    dist.all_to_all_single(table_in, table_out, group=group)
+    recv_table = table_in.tolist()
+    sent = [a for row in per_dest for a in row]
+    offs, total = pack_offsets([a.numel() for a in sent])
+    send = torch.zeros(total, dtype=torch.uint8, device=dev)
+    for a, o in zip(sent, offs):
+        send[o:o + a.numel()].copy_(a)
+    recv = _all_to_all_bytes(send, [pack_offsets(row[:m])[1] for row in table],
+                             [pack_offsets(row[:m])[1] for row in recv_table], group, on_device)
+    lens = [k for row in recv_table for k in row[:m]]
+    offs, _ = pack_offsets(lens)
+    views = [recv[o:o + k] for o, k in zip(offs, lens)]
+    per_src = [views[s * m:(s + 1) * m] for s in range(len(recv_table))]
+    return per_src, None if extra is None else [row[m] for row in recv_table]
+
+
 def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, peer: Optional[PeerWorkspace] = None,
                           check: bool = True, peer_mode: str = "pull", sparse: bool = False) -> List[torch.Tensor]:
@@ -498,28 +528,10 @@ def all_to_all_compressed(chunks: Sequence[torch.Tensor], group=None, checksum: 
         out = torch.empty_like(flats[0])
         ops.decompress_data(as_float, [comp[0, :int(sizes[0])]], [out], checksum, temp_mem, sparse=sparse)
         return [out.view(chunks[0].shape) if as_float else out.view(dt).view(chunks[0].shape)]
-    on_device = _device_collectives(group)
-    cdev = dev if on_device else torch.device("cpu")
-    # (archive bytes, element count) per destination -> per source
-    meta_out = torch.stack([sizes.to(torch.int64), torch.tensor([f.numel() for f in flats], device=dev)], dim=1).to(cdev)
-    meta_in = torch.empty_like(meta_out)
-    dist.all_to_all_single(meta_in, meta_out, group=group)
-    send_sizes = [_round_up(int(v), _ALIGN) for v in meta_out[:, 0].tolist()]  # host sync
-    recv_meta = meta_in.tolist()
-    recv_sizes = [_round_up(int(v[0]), _ALIGN) for v in recv_meta]
-    send = torch.zeros(sum(send_sizes), dtype=torch.uint8, device=dev)
-    o = 0
-    for d in range(world):
-        k = int(meta_out[d, 0])
-        send[o:o + k].copy_(comp[d, :k])
-        o += send_sizes[d]
-    recv = _all_to_all_bytes(send, send_sizes, recv_sizes, group, on_device)
-    ins, outs, o = [], [], 0
-    for s in range(world):
-        k, elems = int(recv_meta[s][0]), int(recv_meta[s][1])
-        ins.append(recv[o:o + k])
-        outs.append(torch.empty(elems, dtype=flats[0].dtype, device=dev))
-        o += recv_sizes[s]
+    hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
+    per_src, elems = _send_to_each([[comp[d, :hs[d]]] for d in range(world)], group, [f.numel() for f in flats])
+    ins = [a for (a,) in per_src]
+    outs = [torch.empty(k, dtype=flats[0].dtype, device=dev) for k in elems]
     status = torch.zeros(world, dtype=torch.uint8, device=dev)
     ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status, sparse=sparse)
     if not bool(status.all()):
@@ -579,6 +591,14 @@ def _flag_non_finite(found_inf: Optional[torch.Tensor], x: torch.Tensor) -> None
     """found_inf = max(found_inf, 1 if x has an inf or NaN else 0), on the device (no host sync, never cleared)."""
     if found_inf is not None:
         torch.maximum(found_inf, (~x.isfinite()).any().float(), out=found_inf)
+
+
+def _local_sum(x: torch.Tensor, acc_dtype: torch.dtype, s32, found_inf: Optional[torch.Tensor]) -> torch.Tensor:
+    """A reducing collective's result when this rank's words are the only terms (a world of one, or no elements):
+    each word's _term in acc_dtype, always a new tensor, with found_inf raised when one is non-finite."""
+    res = x.to(acc_dtype, copy=True) if s32 is None else _term(x, acc_dtype, s32)
+    _flag_non_finite(found_inf, res)
+    return res
 
 
 def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
@@ -641,11 +661,7 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
     arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     if world == 1 or n == 0:
-        if sd is None:
-            return flat[: n // world].to(arch_dtype).to(acc_dtype, copy=True)
-        res = _term(flat[: n // world].to(arch_dtype), acc_dtype, sd)
-        _flag_non_finite(found_inf, res)
-        return res
+        return _local_sum(flat[: n // world].to(arch_dtype), acc_dtype, sd, found_inf)
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
@@ -654,33 +670,11 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
                                               for d in dests for i in range(m)], False, temp_mem,
                                        archive_dtype=arch_dtype, sparse=sparse)
-    on_device = _device_collectives(group)
-    cdev = dev if on_device else torch.device("cpu")
     hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
-    meta_out = torch.zeros(world, m, dtype=torch.int64)
+    per_dest = [[comp.new_empty(0)] * m for _ in range(world)]  # nothing for this rank's own chunk
     for k, d in enumerate(dests):
-        meta_out[d] = torch.tensor(hs[k * m:(k + 1) * m], dtype=torch.int64)
-    meta_in = torch.empty_like(meta_out, device=cdev)
-    dist.all_to_all_single(meta_in, meta_out.to(cdev), group=group)
-    recv_meta = meta_in.cpu().tolist()
-    send_sizes = [sum(_round_up(int(v), _ALIGN) for v in row) for row in meta_out.tolist()]
-    recv_sizes = [sum(_round_up(int(v), _ALIGN) for v in row) for row in recv_meta]
-    send = torch.zeros(sum(send_sizes), dtype=torch.uint8, device=dev)
-    o = 0
-    for k, d in enumerate(dests):
-        for i in range(m):
-            a = hs[k * m + i]
-            send[o:o + a].copy_(comp[k * m + i, :a])
-            o += _round_up(a, _ALIGN)
-    recv = _all_to_all_bytes(send, send_sizes, recv_sizes, group, on_device)
-    archives = []  # archives[s][i]: member i of the chunk source s sent here
-    o = 0
-    for s in range(world):
-        row = []
-        for a in recv_meta[s]:
-            row.append(recv[o:o + int(a)])
-            o += _round_up(int(a), _ALIGN)
-        archives.append(row)
+        per_dest[d] = [comp[k * m + i, :hs[k * m + i]] for i in range(m)]
+    archives, _ = _send_to_each(per_dest, group)  # archives[s][i]: member i of the chunk source s sent here
     out = torch.empty(shard, dtype=acc_dtype, device=dev)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
     own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
@@ -736,11 +730,7 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     flat = t.reshape(-1)
     n = flat.numel()
     if world == 1 or n == 0:
-        if s32 is None and scale_tensor is None:
-            return t.to(acc_dtype, copy=True)
-        res = _term(t, acc_dtype, s32 if scale_tensor is None else scale_tensor)
-        _flag_non_finite(found_inf, res)
-        return res
+        return _local_sum(t, acc_dtype, s32 if scale_tensor is None else scale_tensor, found_inf)
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
     # (a padding zero's term is non-finite only for an inf or NaN scale, which makes every element's term so too)

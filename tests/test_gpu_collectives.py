@@ -2,88 +2,62 @@
 the GPU, real exchange between two processes.  On a box with >= 2 GPUs the ranks use NCCL, one GPU each; on a
 single-GPU box both ranks share cuda:0 and talk over gloo (the packed archives are staged through host memory),
 so the multi-rank path is exercised wherever the GPU tests run."""
-import os
-
 import pytest
 import torch
+
+from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu
 
 
-def _worker(rank, world, port, backend, q):
+def _worker(rank, world, dev):
     import torch.distributed as dist
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    local = rank if backend == "nccl" else 0
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group(backend, rank=rank, world_size=world)
-    try:
-        import dietgpu_b200 as dg
+    import dietgpu_b200 as dg
 
-        ok = True
-        # peer-memory transport (NVLink pull by the decode kernel): needs one GPU per rank
-        ws = dg.PeerWorkspace(32 << 20) if backend == "nccl" else None
-        for dt, n in ((torch.bfloat16, 300001), (torch.float16, 70000), (torch.uint8, 123457)):
-            def make(r):
-                g = torch.Generator(device="cpu").manual_seed(1000 + r)
+    # peer-memory transport (NVLink pull by the decode kernel): needs one GPU per rank
+    ws = dg.PeerWorkspace(32 << 20) if dist.get_backend() == "nccl" else None
+    for dt, n in ((torch.bfloat16, 300001), (torch.float16, 70000), (torch.uint8, 123457)):
+        def make(r):
+            g = torch.Generator(device="cpu").manual_seed(1000 + r)
+            if dt.is_floating_point:
+                return torch.randn(n, generator=g).to(dt)
+            return torch.randint(0, 40, (n,), generator=g, dtype=torch.int32).to(dt)
+
+        mine = make(rank).to(dev)
+        want = torch.cat([make(r) for r in range(world)]).to(dev)
+        for stages in (1, 2, 3):
+            got = dg.all_gather_compressed(mine, members=6, stages=stages)
+            assert torch.equal(got.view(torch.uint8), want.view(torch.uint8)), f"all_gather {dt} stages {stages}"
+        # all-to-all: rank r sends a different chunk (and a different LENGTH) to every destination
+        def chunk(src, dst):
+            g = torch.Generator(device="cpu").manual_seed(77 + 10 * src + dst)
+            m = 50000 + 3001 * src + 17 * dst
+            if dt.is_floating_point:
+                return torch.randn(m, generator=g).to(dt)
+            return torch.randint(0, 9, (m,), generator=g, dtype=torch.int32).to(dt)
+
+        recv = dg.all_to_all_compressed([chunk(rank, d).to(dev) for d in range(world)])
+        for s in range(world):
+            assert torch.equal(recv[s].view(torch.uint8), chunk(s, rank).to(dev).view(torch.uint8)), \
+                f"all_to_all {dt} from {s}"
+        if ws is not None:
+            for mode, stages in (("push", 1), ("push", 2), ("push", 3), ("pull", 2), ("direct", 1), ("auto", 2)):
+                got = dg.all_gather_compressed(mine, members=6, peer=ws, peer_mode=mode, stages=stages)
+                assert torch.equal(got.view(torch.uint8), want.view(torch.uint8)), f"{mode} {dt} stages {stages}"
+
+            def reg(src, dst):  # regular all-to-all: one length
+                g = torch.Generator(device="cpu").manual_seed(99 + 10 * src + dst)
                 if dt.is_floating_point:
-                    return torch.randn(n, generator=g).to(dt)
-                return torch.randint(0, 40, (n,), generator=g, dtype=torch.int32).to(dt)
+                    return torch.randn(40001, generator=g).to(dt)
+                return torch.randint(0, 9, (40001,), generator=g, dtype=torch.int32).to(dt)
 
-            mine = make(rank).to(dev)
-            want = torch.cat([make(r) for r in range(world)]).to(dev)
-            for stages in (1, 2, 3):
-                got = dg.all_gather_compressed(mine, members=6, stages=stages)
-                ok = ok and torch.equal(got.view(torch.uint8), want.view(torch.uint8))
-            # all-to-all: rank r sends a different chunk (and a different LENGTH) to every destination
-            def chunk(src, dst):
-                g = torch.Generator(device="cpu").manual_seed(77 + 10 * src + dst)
-                m = 50000 + 3001 * src + 17 * dst
-                if dt.is_floating_point:
-                    return torch.randn(m, generator=g).to(dt)
-                return torch.randint(0, 9, (m,), generator=g, dtype=torch.int32).to(dt)
-
-            recv = dg.all_to_all_compressed([chunk(rank, d).to(dev) for d in range(world)])
-            for s in range(world):
-                ok = ok and torch.equal(recv[s].view(torch.uint8), chunk(s, rank).to(dev).view(torch.uint8))
-            if ws is not None:
-                for mode, stages in (("push", 1), ("push", 2), ("push", 3), ("pull", 2), ("direct", 1), ("auto", 2)):
-                    got = dg.all_gather_compressed(mine, members=6, peer=ws, peer_mode=mode, stages=stages)
-                    ok = ok and torch.equal(got.view(torch.uint8), want.view(torch.uint8))
-
-                def reg(src, dst):  # regular all-to-all: one length
-                    g = torch.Generator(device="cpu").manual_seed(99 + 10 * src + dst)
-                    if dt.is_floating_point:
-                        return torch.randn(40001, generator=g).to(dt)
-                    return torch.randint(0, 9, (40001,), generator=g, dtype=torch.int32).to(dt)
-
-                for mode in ("pull", "direct"):
-                    recv = dg.all_to_all_compressed([reg(rank, d).to(dev) for d in range(world)], peer=ws, peer_mode=mode)
-                    for s in range(world):
-                        ok = ok and torch.equal(recv[s].view(torch.uint8), reg(s, rank).to(dev).view(torch.uint8))
-        q.put((rank, bool(ok)))
-    except Exception as ex:  # noqa: BLE001  (report instead of leaving the parent to time out)
-        q.put((rank, f"{type(ex).__name__}: {ex}"))
-        raise
-    finally:
-        dist.destroy_process_group()
+            for mode in ("pull", "direct"):
+                recv = dg.all_to_all_compressed([reg(rank, d).to(dev) for d in range(world)], peer=ws, peer_mode=mode)
+                for s in range(world):
+                    assert torch.equal(recv[s].view(torch.uint8), reg(s, rank).to(dev).view(torch.uint8)), \
+                        f"{mode} all_to_all {dt} from {s}"
 
 
 def test_two_rank_compressed_collectives():
-    import torch.multiprocessing as mp
-
-    world = 2
-    backend = "nccl" if torch.cuda.device_count() >= world else "gloo"
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29800 + (os.getpid() % 150)
-    procs = [ctx.Process(target=_worker, args=(r, world, port, backend, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=150) for _ in range(world))
-    assert res == {0: True, 1: True}, (backend, res)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    run_ranks(_worker, 2, timeout=150)

@@ -5,7 +5,6 @@ the existing path applied to the cast x.to(T) made by torch ON THE DEVICE (torch
 oracle's archive of the cast words and the library's own compress of the cast.  Default archives are compared
 field by field (their streams are in completion order), canonical ones byte for byte."""
 import inspect
-import os
 import re
 
 import numpy as np
@@ -14,6 +13,7 @@ import torch
 
 from codec_helpers import (GUARD, KINDS, SENTINEL, assert_pdf_matches, codec_options, guarded_decode, oracle_archive,
                            placed_inputs)
+from multirank import run_ranks
 from oracle import oracle as O
 from test_gpu_variants import VARIANTS
 
@@ -405,69 +405,36 @@ def test_refusals_single_process():
     assert _refusals(dg, "cuda") == "ok"
 
 
-def _worker(rank, world, port, backend, q):
-    import torch.distributed as dist
+def _worker(rank, world, dev):
+    import dietgpu_b200 as dg
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    local = rank if backend == "nccl" else 0
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group(backend, rank=rank, world_size=world)
-    msg = "ok"
-    try:
-        import dietgpu_b200 as dg
+    def same(a, b):  # NaN compared as "both NaN" (a sum's NaN payload is not part of the formula)
+        nan = torch.isnan(a) & torch.isnan(b)
+        return a.dtype == b.dtype and a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
 
-        def same(a, b):  # NaN compared as "both NaN" (a sum's NaN payload is not part of the formula)
-            nan = torch.isnan(a) & torch.isnan(b)
-            return a.dtype == b.dtype and a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
-
-        for w in TYPES:
-            for n in (2 * 40000, 300002):
-                ts = []
-                for r in range(world):
-                    g = torch.Generator(device="cpu").manual_seed(900 + r + n)
-                    x = torch.randn(n, generator=g) * (1 + r)
-                    x[::97] = float("nan") if r == 1 else 0.0
-                    x[5::89] = -0.0
-                    x[7::211] = float("inf") if r == 0 else float("-inf")
-                    x[9::301] = 70000.0  # above fp16's range: +Inf in fp16, finite in bf16
-                    ts.append(x.to(dev))
-                for members in (1, 6):
-                    got = dg.all_gather_compressed(ts[rank], members=members, wire_dtype=w)
-                    if not torch.equal(_bits(got), _bits(torch.cat([t.to(w) for t in ts]))):
-                        msg = f"all_gather {w} {n} {members}"
-                    shard = n // world
-                    want = ts[0].to(w).float()
-                    for t in ts[1:]:
-                        want = want + t.to(w).float()
-                    got = dg.reduce_scatter_compressed(ts[rank], members=members, wire_dtype=w)
-                    if not same(got, want[rank * shard:(rank + 1) * shard]):
-                        msg = f"reduce_scatter {w} {n} {members}"
-        refused = _refusals(dg, dev)
-        if refused != "ok":
-            msg = refused
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg))
-        dist.destroy_process_group()
+    for w in TYPES:
+        for n in (2 * 40000, 300002):
+            ts = []
+            for r in range(world):
+                g = torch.Generator(device="cpu").manual_seed(900 + r + n)
+                x = torch.randn(n, generator=g) * (1 + r)
+                x[::97] = float("nan") if r == 1 else 0.0
+                x[5::89] = -0.0
+                x[7::211] = float("inf") if r == 0 else float("-inf")
+                x[9::301] = 70000.0  # above fp16's range: +Inf in fp16, finite in bf16
+                ts.append(x.to(dev))
+            for members in (1, 6):
+                got = dg.all_gather_compressed(ts[rank], members=members, wire_dtype=w)
+                assert torch.equal(_bits(got), _bits(torch.cat([t.to(w) for t in ts]))), f"all_gather {w} {n} {members}"
+                shard = n // world
+                want = ts[0].to(w).float()
+                for t in ts[1:]:
+                    want = want + t.to(w).float()
+                got = dg.reduce_scatter_compressed(ts[rank], members=members, wire_dtype=w)
+                assert same(got, want[rank * shard:(rank + 1) * shard]), f"reduce_scatter {w} {n} {members}"
+    refused = _refusals(dg, dev)
+    assert refused == "ok", refused
 
 
 def test_two_rank_collectives_with_a_16_bit_wire():
-    import torch.multiprocessing as mp
-
-    world = 2
-    backend = "nccl" if torch.cuda.device_count() >= world else "gloo"
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29600 + (os.getpid() % 140)
-    procs = [ctx.Process(target=_worker, args=(r, world, port, backend, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for p in procs:
-        p.join(timeout=120)
-    assert res == {0: "ok", 1: "ok"}, (backend, res)
-    for p in procs:
-        assert p.exitcode == 0
+    run_ranks(_worker, 2, timeout=300)

@@ -1,7 +1,6 @@
 """Decode-and-sum (dgb_float_decompress_reduce / ops.decompress_data_reduce) and the reducing collectives built on
 it.  Decoding is lossless, so the reference of every group is the torch left fold of the ORIGINAL tensors in
 archive order; results must match it bit for bit, with NaN compared as "both NaN"."""
-import os
 import re
 
 import numpy as np
@@ -9,6 +8,7 @@ import pytest
 import torch
 
 from codec_helpers import assert_guard_intact, codec_options, guarded_out
+from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -294,76 +294,38 @@ def test_argument_errors():
 
 # ---- two ranks ------------------------------------------------------------------------------------------------
 
-def _worker(rank, world, port, backend, q):
-    import torch.distributed as dist
+def _worker(rank, world, dev):
+    import dietgpu_b200 as dg
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    local = rank if backend == "nccl" else 0
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group(backend, rank=rank, world_size=world)
-    msg = "ok"
-    try:
-        import dietgpu_b200 as dg
+    def same(a, b):
+        nan = torch.isnan(a) & torch.isnan(b)
+        return a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
 
-        def same(a, b):
-            nan = torch.isnan(a) & torch.isnan(b)
-            return a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
-
-        for dt in DTYPES:
-            for n in (2 * 40000, 300001):
-                ts = []
-                for r in range(world):
-                    g = torch.Generator(device="cpu").manual_seed(500 + r + n)
-                    x = torch.randn(n, generator=g) * (1 + r)
-                    x[::97] = float("nan") if r == 1 else 0.0
-                    x[5::89] = -0.0
-                    ts.append(x.to(dt).to(dev))
-                want = fold(ts)
-                for members in (1, 6):
-                    if n % world == 0:
-                        got = dg.reduce_scatter_compressed(ts[rank], members=members)
-                        shard = n // world
-                        if not same(got, want[rank * shard:(rank + 1) * shard]):
-                            msg = f"reduce_scatter {dt} {n} {members}"
-                    got = dg.all_reduce_compressed(ts[rank].view(-1, 1) if n % 2 else ts[rank], members=members)
-                    if not same(got.reshape(-1), want):
-                        msg = f"all_reduce {dt} {n} {members}"
-        for bad in (torch.zeros(16, dtype=torch.uint8, device=dev), torch.zeros(16, dtype=torch.float64, device=dev),
-                    torch.zeros(15, dtype=torch.bfloat16, device=dev)):
-            try:
-                dg.reduce_scatter_compressed(bad)
-                msg = f"no ValueError for {bad.dtype} {bad.numel()}"
-            except ValueError:
-                pass
-        for bad in (torch.zeros(16, dtype=torch.uint8, device=dev), torch.zeros(16, dtype=torch.float64, device=dev)):
-            try:
-                dg.all_reduce_compressed(bad)
-                msg = f"no ValueError for all_reduce {bad.dtype}"
-            except ValueError:
-                pass
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg))
-        dist.destroy_process_group()
+    for dt in DTYPES:
+        for n in (2 * 40000, 300001):
+            ts = []
+            for r in range(world):
+                g = torch.Generator(device="cpu").manual_seed(500 + r + n)
+                x = torch.randn(n, generator=g) * (1 + r)
+                x[::97] = float("nan") if r == 1 else 0.0
+                x[5::89] = -0.0
+                ts.append(x.to(dt).to(dev))
+            want = fold(ts)
+            for members in (1, 6):
+                if n % world == 0:
+                    got = dg.reduce_scatter_compressed(ts[rank], members=members)
+                    shard = n // world
+                    assert same(got, want[rank * shard:(rank + 1) * shard]), f"reduce_scatter {dt} {n} {members}"
+                got = dg.all_reduce_compressed(ts[rank].view(-1, 1) if n % 2 else ts[rank], members=members)
+                assert same(got.reshape(-1), want), f"all_reduce {dt} {n} {members}"
+    for bad in (torch.zeros(16, dtype=torch.uint8, device=dev), torch.zeros(16, dtype=torch.float64, device=dev),
+                torch.zeros(15, dtype=torch.bfloat16, device=dev)):
+        with pytest.raises(ValueError):
+            dg.reduce_scatter_compressed(bad)
+    for bad in (torch.zeros(16, dtype=torch.uint8, device=dev), torch.zeros(16, dtype=torch.float64, device=dev)):
+        with pytest.raises(ValueError):
+            dg.all_reduce_compressed(bad)
 
 
 def test_two_rank_reduce_collectives():
-    import torch.multiprocessing as mp
-
-    world = 2
-    backend = "nccl" if torch.cuda.device_count() >= world else "gloo"
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29650 + (os.getpid() % 140)
-    procs = [ctx.Process(target=_worker, args=(r, world, port, backend, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for p in procs:
-        p.join(timeout=120)
-    assert res == {0: "ok", 1: "ok"}, (backend, res)
-    for p in procs:
-        assert p.exitcode == 0
+    run_ranks(_worker, 2, timeout=300)

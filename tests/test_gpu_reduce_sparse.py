@@ -11,8 +11,6 @@ The corpus mixes, inside every group, archives whose words are ReLU outputs, all
 two symbols are free, so nothing is elided and +-0 words are stored) and NaN / +-inf / subnormals among zeros.
 Every call parses its archives' block tables and fails unless blocks were decoded through both stream branches of
 decodeReduceBlock (staged in the warp's slot, or read from global memory)."""
-import os
-import queue
 import re
 
 import numpy as np
@@ -20,6 +18,7 @@ import pytest
 import torch
 
 from codec_helpers import assert_guard_intact, codec_options, guarded_out, to_dev_bytes
+from multirank import NAME, host_words, rank_data, run_ranks
 from oracle import oracle as O
 from reduce_reference import WORD, assert_same_words, fold_ref
 import sparse32_oracle as SP32
@@ -458,17 +457,9 @@ def test_profiler_sees_every_instantiation():
 
 # ---- collectives ------------------------------------------------------------------------------------------------
 
-def _host_words(x):
-    x = x.detach().contiguous().cpu()
-    return x.view(torch.int32 if x.element_size() == 4 else torch.int16).numpy().view(
-        np.uint32 if x.element_size() == 4 else np.uint16)
-
-
 def sparse_rank_data(dt, n, world, seed, pruned, widened=False):
-    """tests/test_gpu_reduce_ranks.rank_data (order-dependent elements, +-0, NaN, +-inf in elements 0..7 of every
-    16) with the other elements ReLU'd, or 90 % of them pruned to +-0."""
-    from test_gpu_reduce_ranks import rank_data
-
+    """tests/multirank.rank_data (order-dependent elements, +-0, NaN, +-inf in elements 0..7 of every 16) with the
+    other elements ReLU'd, or 90 % of them pruned to +-0."""
     xs = rank_data(dt, n, world, seed, widened=widened)
     pos = torch.arange(n)
     out = []
@@ -486,134 +477,100 @@ def sparse_rank_data(dt, n, world, seed, pruned, widened=False):
     return out
 
 
-def _worker(rank, world, port, q):
+def _worker(rank, world, dev):
     import torch.distributed as dist
 
-    from dietgpu_b200 import collectives as C
+    import dietgpu_b200 as dg
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(0)
-    dev = torch.device("cuda", 0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    msg = "ok"
     done = []
     sent = [0]
-    try:
-        import dietgpu_b200 as dg
+    a2a_calls = []
 
-        # count the payload bytes this rank sends (the size exchanges are int tensors and not counted)
-        real_gather, real_a2a = dist.all_gather_into_tensor, dist.all_to_all_single
+    # count the payload bytes this rank sends (the size exchanges are int tensors and not counted), and the
+    # all_to_all_single calls by the dtype they send
+    real_gather, real_a2a = dist.all_gather_into_tensor, dist.all_to_all_single
 
-        def gather(out, inp, *a, **k):
-            if inp.dtype == torch.uint8:
-                sent[0] += inp.numel()
-            return real_gather(out, inp, *a, **k)
+    def gather(out, inp, *a, **k):
+        if inp.dtype == torch.uint8:
+            sent[0] += inp.numel()
+        return real_gather(out, inp, *a, **k)
 
-        def a2a(out, inp, *a, **k):
-            if inp.dtype == torch.uint8:
-                sent[0] += inp.numel()
-            return real_a2a(out, inp, *a, **k)
+    def a2a(out, inp, *a, **k):
+        a2a_calls.append(inp.dtype)
+        if inp.dtype == torch.uint8:
+            sent[0] += inp.numel()
+        return real_a2a(out, inp, *a, **k)
 
-        C.dist.all_gather_into_tensor, C.dist.all_to_all_single = gather, a2a
+    dist.all_gather_into_tensor, dist.all_to_all_single = gather, a2a
 
-        def run(f):
-            sent[0] = 0
-            r = f()
-            return r, sent[0]
+    def run(f):
+        sent[0] = 0
+        r = f()
+        return r, sent[0]
 
-        def same(a, b, what):
-            assert np.array_equal(_host_words(a), _host_words(b)), what
-            done.append(what)
+    def exchange(f, what):
+        """f() makes one per-destination exchange: the int64 size table, then the uint8 payload."""
+        a2a_calls.clear()
+        r = f()
+        assert a2a_calls == [torch.int64, torch.uint8], f"{what}: all_to_all_single sent {a2a_calls}"
+        return r
 
-        for dt in (torch.float16, torch.bfloat16, torch.float32):
-            for pruned in (False, True):
-                for members in (1, 6):
-                    tag = f"{dt} pruned {pruned} members {members}"
-                    n = world * 12289
-                    ts = sparse_rank_data(dt, n, world, 100 + members, pruned)
+    def same(a, b, what):
+        assert np.array_equal(host_words(a), host_words(b)), what
+        done.append(what)
+
+    for dt in (torch.float16, torch.bfloat16, torch.float32):
+        for pruned in (False, True):
+            for members in (1, 6):
+                tag = f"{dt} pruned {pruned} members {members}"
+                n = world * 12289
+                ts = sparse_rank_data(dt, n, world, 100 + members, pruned)
+                x = ts[rank].to(dev)
+                got, b_s = run(lambda: dg.all_gather_compressed(x, members=members, sparse=True))
+                want, b_d = run(lambda: dg.all_gather_compressed(x, members=members))
+                same(got, want, f"all_gather {tag}")
+                same(got, torch.cat(ts), f"all_gather {tag} (inputs)")
+                assert b_s < b_d, f"all_gather {tag}: {b_s} sparse bytes sent, {b_d} dense"
+                chunks = [x[d * 12289:(d + 1) * 12289 - d] for d in range(world)]
+                got = exchange(lambda: dg.all_to_all_compressed(chunks, sparse=True), f"all_to_all {tag}")
+                want = exchange(lambda: dg.all_to_all_compressed(chunks), f"all_to_all {tag}")
+                for s in range(world):
+                    same(got[s], want[s], f"all_to_all {tag} from {s}")
+                for reduce_dtype in ([None] if dt == torch.float32 else [None, torch.float32]):
+                    widened = reduce_dtype is not None
+                    ts = sparse_rank_data(dt, n, world, 200 + members, pruned, widened)
                     x = ts[rank].to(dev)
-                    got, b_s = run(lambda: dg.all_gather_compressed(x, members=members, sparse=True))
-                    want, b_d = run(lambda: dg.all_gather_compressed(x, members=members))
-                    same(got, want, f"all_gather {tag}")
-                    same(got, torch.cat(ts), f"all_gather {tag} (inputs)")
-                    assert b_s < b_d, f"all_gather {tag}: {b_s} sparse bytes sent, {b_d} dense"
-                    chunks = [x[d * 12289:(d + 1) * 12289 - d] for d in range(world)]
-                    got = dg.all_to_all_compressed(chunks, sparse=True)
-                    want = dg.all_to_all_compressed(chunks)
-                    for s in range(world):
-                        same(got[s], want[s], f"all_to_all {tag} from {s}")
-                    for reduce_dtype in ([None] if dt == torch.float32 else [None, torch.float32]):
-                        widened = reduce_dtype is not None
-                        ts = sparse_rank_data(dt, n, world, 200 + members, pruned, widened)
-                        x = ts[rank].to(dev)
-                        ot = "f32" if widened or dt == torch.float32 else {torch.float16: "f16",
-                                                                            torch.bfloat16: "bf16"}[dt]
-                        at = {torch.float16: "f16", torch.bfloat16: "bf16", torch.float32: "f32"}[dt]
-                        got, b_s = run(lambda: dg.reduce_scatter_compressed(x, members=members,
-                                                                            reduce_dtype=reduce_dtype, sparse=True))
-                        want, b_d = run(lambda: dg.reduce_scatter_compressed(x, members=members,
-                                                                             reduce_dtype=reduce_dtype))
-                        what = f"reduce_scatter {tag} reduce {reduce_dtype}"
+                    at = NAME[dt]
+                    ot = "f32" if widened else at
+                    what = f"reduce_scatter {tag} reduce {reduce_dtype}"
+                    got, b_s = run(lambda: exchange(lambda: dg.reduce_scatter_compressed(
+                        x, members=members, reduce_dtype=reduce_dtype, sparse=True), what))
+                    want, b_d = run(lambda: exchange(lambda: dg.reduce_scatter_compressed(
+                        x, members=members, reduce_dtype=reduce_dtype), what))
+                    same(got, want, what)
+                    lo, hi = rank * (n // world), (rank + 1) * (n // world)
+                    assert_same_words(host_words(got), fold_ref([host_words(t[lo:hi]) for t in ts], at, ot),
+                                      ot, f"{what} (rank-order fold)")
+                    assert b_s < b_d, f"{what}: {b_s} sparse bytes sent, {b_d} dense"
+                    for m in (1, 300001):
+                        tm = sparse_rank_data(dt, m, world, 300 + m, pruned, widened)
+                        xm = tm[rank].to(dev)
+                        got = dg.all_reduce_compressed(xm, members=members, reduce_dtype=reduce_dtype,
+                                                       sparse=True)
+                        want = dg.all_reduce_compressed(xm, members=members, reduce_dtype=reduce_dtype)
+                        what = f"all_reduce {tag} n {m} reduce {reduce_dtype}"
                         same(got, want, what)
-                        lo, hi = rank * (n // world), (rank + 1) * (n // world)
-                        assert_same_words(_host_words(got), fold_ref([_host_words(t[lo:hi]) for t in ts], at, ot),
-                                          ot, f"{what} (rank-order fold)")
-                        assert b_s < b_d, f"{what}: {b_s} sparse bytes sent, {b_d} dense"
-                        for m in (1, 300001):
-                            tm = sparse_rank_data(dt, m, world, 300 + m, pruned, widened)
-                            xm = tm[rank].to(dev)
-                            got = dg.all_reduce_compressed(xm, members=members, reduce_dtype=reduce_dtype,
-                                                           sparse=True)
-                            want = dg.all_reduce_compressed(xm, members=members, reduce_dtype=reduce_dtype)
-                            what = f"all_reduce {tag} n {m} reduce {reduce_dtype}"
-                            same(got, want, what)
-                            assert_same_words(_host_words(got), fold_ref([_host_words(t) for t in tm], at, ot), ot,
-                                              f"{what} (rank-order fold)")
-                            zero = np.all(np.stack([(_host_words(t) & ~np.array(
-                                0x80000000 if t.element_size() == 4 else 0x8000, _host_words(t).dtype)) == 0
-                                for t in tm]), axis=0)
-                            gw = _host_words(got)
-                            assert np.all((gw[zero] & ~np.array(0x80000000 if got.element_size() == 4 else 0x8000,
-                                                                gw.dtype)) == 0), f"{what}: zeros"
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg, len(done)))
-        dist.destroy_process_group()
+                        assert_same_words(host_words(got), fold_ref([host_words(t) for t in tm], at, ot), ot,
+                                          f"{what} (rank-order fold)")
+                        zero = np.all(np.stack([(host_words(t) & ~np.array(
+                            0x80000000 if t.element_size() == 4 else 0x8000, host_words(t).dtype)) == 0
+                            for t in tm]), axis=0)
+                        gw = host_words(got)
+                        assert np.all((gw[zero] & ~np.array(0x80000000 if got.element_size() == 4 else 0x8000,
+                                                            gw.dtype)) == 0), f"{what}: zeros"
+    return len(done)
 
 
 @pytest.mark.parametrize("world", [2, 3, 4])
 def test_sparse_collectives(world):
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 31600 + 3 * (os.getpid() % 100) + (world - 2)  # no other test uses 31600..31899
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    res = {}
-    try:
-        for p in procs:
-            p.start()
-        for _ in range(world):
-            try:
-                r, msg, cnt = q.get(timeout=600)
-            except queue.Empty:
-                break
-            res[r] = (msg, cnt)
-        for p in procs:
-            p.join(timeout=120)
-    finally:
-        started = [p for p in procs if p.pid is not None]
-        for p in started:
-            if p.is_alive():
-                p.terminate()
-        for p in started:
-            p.join(timeout=30)
-            if p.is_alive():
-                p.kill()
-                p.join()
-    print(f"world {world}: checks per rank {[res.get(r, (None, 0))[1] for r in range(world)]}")
-    assert sorted(res) == list(range(world)), res
-    assert all(m == "ok" for m, _ in res.values()), res
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    run_ranks(_worker, world, backend="gloo", timeout=600)

@@ -3,13 +3,13 @@ reducing collectives' reduce_dtype=torch.float32.  fp16 / bf16 archives are summ
 lossless, so the reference of every group is torch's fp32 left fold of the ORIGINAL 16-bit tensors in archive order,
 acc = x0.float(); acc = acc + x1.float(); ...  Results must match it bit for bit, with NaN compared as "both NaN"."""
 import itertools
-import os
 import re
 
 import pytest
 import torch
 
 from codec_helpers import assert_guard_intact, codec_options, guarded_out
+from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -359,83 +359,46 @@ def test_argument_errors():
 
 # ---- two ranks ------------------------------------------------------------------------------------------------
 
-def _worker(rank, world, port, backend, q):
-    import torch.distributed as dist
+def _worker(rank, world, dev):
+    import dietgpu_b200 as dg
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    local = rank if backend == "nccl" else 0
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group(backend, rank=rank, world_size=world)
-    msg = "ok"
-    try:
-        import dietgpu_b200 as dg
+    def same(a, b):
+        nan = torch.isnan(a) & torch.isnan(b)
+        return a.dtype == b.dtype and a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
 
-        def same(a, b):
-            nan = torch.isnan(a) & torch.isnan(b)
-            return a.dtype == b.dtype and a.shape == b.shape and not bool(((_bits(a) != _bits(b)) & ~nan).any())
-
-        for dt in DTYPES:
-            for n in (2 * 40000, 300001):
-                ts = []
-                for r in range(world):
-                    g = torch.Generator(device="cpu").manual_seed(700 + r + n)
-                    x = torch.randn(n, generator=g) * (1 + r)
-                    x[::97] = float("nan") if r == 1 else 0.0
-                    x[5::89] = -0.0
-                    ts.append(x.to(dt).to(dev))
-                want = fold32(ts)
-                for members in (1, 6):
-                    if n % world == 0:
-                        shard = n // world
-                        got = dg.reduce_scatter_compressed(ts[rank], members=members, reduce_dtype=torch.float32)
-                        if not same(got, want[rank * shard:(rank + 1) * shard]):
-                            msg = f"reduce_scatter {dt} {n} {members}"
-                        a = dg.reduce_scatter_compressed(ts[rank], members=members, reduce_dtype=dt)
-                        b = dg.reduce_scatter_compressed(ts[rank], members=members)
-                        if not same(a, b):
-                            msg = f"reduce_scatter reduce_dtype={dt} {n} {members}"
-                    t = ts[rank].view(-1, 1) if n % 2 else ts[rank]
-                    got = dg.all_reduce_compressed(t, members=members, reduce_dtype=torch.float32)
-                    if got.shape != t.shape or not same(got.reshape(-1), want):
-                        msg = f"all_reduce {dt} {n} {members}"
-                    a = dg.all_reduce_compressed(t, members=members, reduce_dtype=dt)
-                    b = dg.all_reduce_compressed(t, members=members)
-                    if not same(a, b):
-                        msg = f"all_reduce reduce_dtype={dt} {n} {members}"
-        for t, rdt in ((torch.zeros(16, dtype=torch.float32, device=dev), torch.float16),
-                       (torch.zeros(16, dtype=torch.float32, device=dev), torch.bfloat16),
-                       (torch.zeros(16, dtype=torch.bfloat16, device=dev), torch.float64),
-                       (torch.zeros(16, dtype=torch.float16, device=dev), torch.bfloat16),
-                       (torch.zeros(16, dtype=torch.bfloat16, device=dev), torch.float16)):
-            for fn in (dg.reduce_scatter_compressed, dg.all_reduce_compressed):
-                try:
-                    fn(t, reduce_dtype=rdt)
-                    msg = f"no ValueError for {fn.__name__} {t.dtype} reduce_dtype={rdt}"
-                except ValueError:
-                    pass
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg))
-        dist.destroy_process_group()
+    for dt in DTYPES:
+        for n in (2 * 40000, 300001):
+            ts = []
+            for r in range(world):
+                g = torch.Generator(device="cpu").manual_seed(700 + r + n)
+                x = torch.randn(n, generator=g) * (1 + r)
+                x[::97] = float("nan") if r == 1 else 0.0
+                x[5::89] = -0.0
+                ts.append(x.to(dt).to(dev))
+            want = fold32(ts)
+            for members in (1, 6):
+                if n % world == 0:
+                    shard = n // world
+                    got = dg.reduce_scatter_compressed(ts[rank], members=members, reduce_dtype=torch.float32)
+                    assert same(got, want[rank * shard:(rank + 1) * shard]), f"reduce_scatter {dt} {n} {members}"
+                    a = dg.reduce_scatter_compressed(ts[rank], members=members, reduce_dtype=dt)
+                    b = dg.reduce_scatter_compressed(ts[rank], members=members)
+                    assert same(a, b), f"reduce_scatter reduce_dtype={dt} {n} {members}"
+                t = ts[rank].view(-1, 1) if n % 2 else ts[rank]
+                got = dg.all_reduce_compressed(t, members=members, reduce_dtype=torch.float32)
+                assert got.shape == t.shape and same(got.reshape(-1), want), f"all_reduce {dt} {n} {members}"
+                a = dg.all_reduce_compressed(t, members=members, reduce_dtype=dt)
+                b = dg.all_reduce_compressed(t, members=members)
+                assert same(a, b), f"all_reduce reduce_dtype={dt} {n} {members}"
+    for t, rdt in ((torch.zeros(16, dtype=torch.float32, device=dev), torch.float16),
+                   (torch.zeros(16, dtype=torch.float32, device=dev), torch.bfloat16),
+                   (torch.zeros(16, dtype=torch.bfloat16, device=dev), torch.float64),
+                   (torch.zeros(16, dtype=torch.float16, device=dev), torch.bfloat16),
+                   (torch.zeros(16, dtype=torch.bfloat16, device=dev), torch.float16)):
+        for fn in (dg.reduce_scatter_compressed, dg.all_reduce_compressed):
+            with pytest.raises(ValueError):
+                fn(t, reduce_dtype=rdt)
 
 
 def test_two_rank_reduce_collectives_fp32():
-    import torch.multiprocessing as mp
-
-    world = 2
-    backend = "nccl" if torch.cuda.device_count() >= world else "gloo"
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29800 + (os.getpid() % 140)
-    procs = [ctx.Process(target=_worker, args=(r, world, port, backend, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for p in procs:
-        p.join(timeout=120)
-    assert res == {0: "ok", 1: "ok"}, (backend, res)
-    for p in procs:
-        assert p.exitcode == 0
+    run_ranks(_worker, 2, timeout=300)

@@ -15,8 +15,6 @@ torch.profiler's trace, and the profiler drops GPU records whose timestamps have
 that drift grows with the age of the process, and after minutes of GPU work it drops the first records of a
 session.  A module of this length run ahead of them would shift their sessions minutes later and make them miss
 launches."""
-import os
-import queue
 import re
 import time
 
@@ -25,6 +23,7 @@ import pytest
 import torch
 
 from codec_helpers import assert_guard_intact, codec_options, guarded_out
+from multirank import NAME, host_words, rank_data, run_ranks
 from reduce_reference import assert_same_words
 from scaled_reference import SCALES, scaled_fold_ref
 import test_gpu_reduce_edges as E
@@ -312,115 +311,61 @@ def test_graph_capture_replays_the_captured_scale(at, ot, sparse):
 
 # ---- collectives ----------------------------------------------------------------------------------------------------
 
-def _host_words(x):
-    x = x.detach().contiguous().cpu()
-    return x.view(torch.int32 if x.element_size() == 4 else torch.int16).numpy().view(
-        np.uint32 if x.element_size() == 4 else np.uint16)
-
-
-NAME = {torch.float16: "f16", torch.bfloat16: "bf16", torch.float32: "f32"}
-
-
 def _term(x, acc, s):
     return (x.float() * torch.tensor(s, dtype=torch.float32, device=x.device)).to(acc)
 
 
-def _worker(rank, world, port, q):
-    import torch.distributed as dist
+def _worker(rank, world, dev):
+    import dietgpu_b200 as dg
 
-    from test_gpu_reduce_ranks import rank_data
-
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(0)
-    dev = torch.device("cuda", 0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    msg = "ok"
     done = []
-    try:
-        import dietgpu_b200 as dg
 
-        def check(got, ts_arch, acc, s, what):
-            """got == the rank-order fold of term(t_r) (torch on the GPU and float64), t_r in the archive dtype."""
-            want = _term(ts_arch[0].to(dev), acc, s)
-            for x in ts_arch[1:]:
-                want = want + _term(x.to(dev), acc, s)
-            assert bool(same_dev(got, want).all()), f"{what}: differs from torch's fold"
-            assert_same_words(_host_words(got), scaled_fold_ref([_host_words(x) for x in ts_arch],
-                                                                NAME[ts_arch[0].dtype], NAME[acc], s),
-                              NAME[acc], f"{what} (float64)")
-            done.append(what)
+    def check(got, ts_arch, acc, s, what):
+        """got == the rank-order fold of term(t_r) (torch on the GPU and float64), t_r in the archive dtype."""
+        want = _term(ts_arch[0].to(dev), acc, s)
+        for x in ts_arch[1:]:
+            want = want + _term(x.to(dev), acc, s)
+        assert bool(same_dev(got, want).all()), f"{what}: differs from torch's fold"
+        assert_same_words(host_words(got), scaled_fold_ref([host_words(x) for x in ts_arch],
+                                                            NAME[ts_arch[0].dtype], NAME[acc], s),
+                          NAME[acc], f"{what} (float64)")
+        done.append(what)
 
-        avg = float(np.float32(1 / world))
-        for dt in (torch.float16, torch.bfloat16, torch.float32):
-            variants = [(None, None)] + ([(torch.float32, None)] if dt != torch.float32 else
-                                         [(None, torch.bfloat16), (None, torch.float16)])
-            for reduce_dtype, wire in variants:
-                for sparse in ((False, True) if wire is None else (False,)):
-                    for how in ("average", "scale"):
-                        kw = dict(average=True) if how == "average" else dict(scale=-0.3)
-                        s = avg if how == "average" else -0.3
-                        tag = f"{dt} reduce {reduce_dtype} wire {wire} sparse {sparse} {how}"
-                        widened = reduce_dtype is not None
-                        n = world * 12289 if world > 1 else 12289
-                        ts = rank_data(dt, n, world, 500 + len(done), widened=widened)
-                        acc = torch.float32 if (widened or wire is not None) else dt
-                        arch_dt = wire or dt
-                        got = dg.reduce_scatter_compressed(ts[rank].to(dev), members=3, reduce_dtype=reduce_dtype,
-                                                           wire_dtype=wire, sparse=sparse, **kw)
-                        lo, hi = rank * (n // world), (rank + 1) * (n // world)
-                        check(got, [t[lo:hi].to(arch_dt) for t in ts], acc, s, f"reduce_scatter {tag}")
-                        if wire is None:
-                            for m in (1, 30001):
-                                tm = rank_data(dt, m, world, 900 + m, widened=widened)
-                                got = dg.all_reduce_compressed(tm[rank].to(dev), members=3, reduce_dtype=reduce_dtype,
-                                                               sparse=sparse, **kw)
-                                check(got, tm, acc, s, f"all_reduce {tag} n {m}")
-                                if dt == torch.float16 and how == "average" and world > 1 and not widened:
-                                    # element 5 of every 16 is max, max, -max, ...: the rank-order fp16 sum
-                                    # overflows to inf, the average does not
-                                    k5 = got.view(-1)[5::16]
-                                    assert bool(torch.isfinite(k5).all()), f"{tag}: the average overflowed"
-                                    plain = dg.all_reduce_compressed(tm[rank].to(dev), members=3)
-                                    assert bool(torch.isinf(plain.view(-1)[5::16]).all()), f"{tag}: plain sum"
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg, len(done)))
-        dist.destroy_process_group()
+    avg = float(np.float32(1 / world))
+    for dt in (torch.float16, torch.bfloat16, torch.float32):
+        variants = [(None, None)] + ([(torch.float32, None)] if dt != torch.float32 else
+                                     [(None, torch.bfloat16), (None, torch.float16)])
+        for reduce_dtype, wire in variants:
+            for sparse in ((False, True) if wire is None else (False,)):
+                for how in ("average", "scale"):
+                    kw = dict(average=True) if how == "average" else dict(scale=-0.3)
+                    s = avg if how == "average" else -0.3
+                    tag = f"{dt} reduce {reduce_dtype} wire {wire} sparse {sparse} {how}"
+                    widened = reduce_dtype is not None
+                    n = world * 12289 if world > 1 else 12289
+                    ts = rank_data(dt, n, world, 500 + len(done), widened=widened)
+                    acc = torch.float32 if (widened or wire is not None) else dt
+                    arch_dt = wire or dt
+                    got = dg.reduce_scatter_compressed(ts[rank].to(dev), members=3, reduce_dtype=reduce_dtype,
+                                                       wire_dtype=wire, sparse=sparse, **kw)
+                    lo, hi = rank * (n // world), (rank + 1) * (n // world)
+                    check(got, [t[lo:hi].to(arch_dt) for t in ts], acc, s, f"reduce_scatter {tag}")
+                    if wire is None:
+                        for m in (1, 30001):
+                            tm = rank_data(dt, m, world, 900 + m, widened=widened)
+                            got = dg.all_reduce_compressed(tm[rank].to(dev), members=3, reduce_dtype=reduce_dtype,
+                                                           sparse=sparse, **kw)
+                            check(got, tm, acc, s, f"all_reduce {tag} n {m}")
+                            if dt == torch.float16 and how == "average" and world > 1 and not widened:
+                                # element 5 of every 16 is max, max, -max, ...: the rank-order fp16 sum
+                                # overflows to inf, the average does not
+                                k5 = got.view(-1)[5::16]
+                                assert bool(torch.isfinite(k5).all()), f"{tag}: the average overflowed"
+                                plain = dg.all_reduce_compressed(tm[rank].to(dev), members=3)
+                                assert bool(torch.isinf(plain.view(-1)[5::16]).all()), f"{tag}: plain sum"
+    return len(done)
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 4])
 def test_scaled_collectives(world):
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 31900 + 4 * (os.getpid() % 100) + (world - 1)  # no other test uses 31900..32299
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    res = {}
-    try:
-        for p in procs:
-            p.start()
-        for _ in range(world):
-            try:
-                r, msg, cnt = q.get(timeout=600)
-            except queue.Empty:
-                break
-            res[r] = (msg, cnt)
-        for p in procs:
-            p.join(timeout=120)
-    finally:
-        started = [p for p in procs if p.pid is not None]
-        for p in started:
-            if p.is_alive():
-                p.terminate()
-        for p in started:
-            p.join(timeout=30)
-            if p.is_alive():
-                p.kill()
-                p.join()
-    print(f"world {world}: checks per rank {[res.get(r, (None, 0))[1] for r in range(world)]}")
-    assert sorted(res) == list(range(world)), res
-    assert all(m == "ok" for m, _ in res.values()), res
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    run_ranks(_worker, world, backend="gloo", timeout=600)

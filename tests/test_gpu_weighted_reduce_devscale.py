@@ -15,8 +15,6 @@ other GPU module that reads torch.profiler's trace; its own profiler check comes
 drops GPU records whose timestamps have drifted outside its capture window, the drift grows with the age of the
 process, and this module's minutes of GPU work run ahead of a check without wide margins around its window would
 make that check miss launches (test_gpu_weighted_reduce.py)."""
-import os
-import queue
 import re
 import time
 
@@ -25,6 +23,7 @@ import pytest
 import torch
 
 from codec_helpers import assert_guard_intact, codec_options, guarded_out
+from multirank import rank_data, run_ranks
 from reduce_reference import assert_same_words
 from scaled_reference import SCALES, scaled_fold_ref
 import test_gpu_reduce_edges as E
@@ -362,120 +361,74 @@ def _bits_equal(a, b):
     return torch.equal(a.view(W._it_of(a)), b.view(W._it_of(b)))
 
 
-def _worker(rank, world, port, q):
-    import torch.distributed as dist
+def _worker(rank, world, dev):
+    import dietgpu_b200 as dg
 
-    from test_gpu_reduce_ranks import rank_data
-
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(0)
-    dev = torch.device("cuda", 0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    msg = "ok"
     done = []
-    try:
-        import dietgpu_b200 as dg
-
-        s = float(np.float32(-0.3) / np.float32(world))
-        for dt in (torch.float16, torch.bfloat16, torch.float32):
-            variants = [(None, None)] + ([(torch.float32, None)] if dt != torch.float32 else
-                                         [(None, torch.bfloat16), (None, torch.float16)])
-            for reduce_dtype, wire in variants:
-                for sparse in ((False, True) if wire is None else (False,)):
-                    tag = f"{dt} reduce {reduce_dtype} wire {wire} sparse {sparse}"
-                    kw2 = dict(members=3, reduce_dtype=reduce_dtype, sparse=sparse)  # all_reduce_compressed's
-                    kw = dict(kw2, wire_dtype=wire)
-                    n = world * 12289 if world > 1 else 12289
-                    ts = rank_data(dt, n, world, 700 + len(done), widened=reduce_dtype is not None)
-                    x = ts[rank].to(dev)
-                    # equivalence: == scale=float(s), with the flag set exactly where the shard is non-finite
-                    fi = torch.zeros(1, device=dev)
-                    got = dg.reduce_scatter_compressed(x, scale_tensor=torch.tensor([s], device=dev), found_inf=fi,
-                                                       **kw)
-                    want = dg.reduce_scatter_compressed(x, scale=s, **kw)
-                    assert _bits_equal(got, want), f"reduce_scatter {tag}"
-                    assert float(fi.item()) == float(bool((~torch.isfinite(got)).any())), f"reduce_scatter {tag} flag"
-                    done.append(tag)
+    s = float(np.float32(-0.3) / np.float32(world))
+    for dt in (torch.float16, torch.bfloat16, torch.float32):
+        variants = [(None, None)] + ([(torch.float32, None)] if dt != torch.float32 else
+                                     [(None, torch.bfloat16), (None, torch.float16)])
+        for reduce_dtype, wire in variants:
+            for sparse in ((False, True) if wire is None else (False,)):
+                tag = f"{dt} reduce {reduce_dtype} wire {wire} sparse {sparse}"
+                kw2 = dict(members=3, reduce_dtype=reduce_dtype, sparse=sparse)  # all_reduce_compressed's
+                kw = dict(kw2, wire_dtype=wire)
+                n = world * 12289 if world > 1 else 12289
+                ts = rank_data(dt, n, world, 700 + len(done), widened=reduce_dtype is not None)
+                x = ts[rank].to(dev)
+                # equivalence: == scale=float(s), with the flag set exactly where the shard is non-finite
+                fi = torch.zeros(1, device=dev)
+                got = dg.reduce_scatter_compressed(x, scale_tensor=torch.tensor([s], device=dev), found_inf=fi,
+                                                   **kw)
+                want = dg.reduce_scatter_compressed(x, scale=s, **kw)
+                assert _bits_equal(got, want), f"reduce_scatter {tag}"
+                assert float(fi.item()) == float(bool((~torch.isfinite(got)).any())), f"reduce_scatter {tag} flag"
+                done.append(tag)
+                if wire is None:
+                    for m in (1, 30001):
+                        tm = rank_data(dt, m, world, 900 + m, widened=reduce_dtype is not None)
+                        fi = torch.zeros(1, device=dev)
+                        got = dg.all_reduce_compressed(tm[rank].to(dev), scale_tensor=torch.tensor([s], device=dev),
+                                                       found_inf=fi, **kw2)
+                        want = dg.all_reduce_compressed(tm[rank].to(dev), scale=s, **kw2)
+                        assert _bits_equal(got, want), f"all_reduce {tag} n {m}"
+                        assert float(fi.item()) == float(bool((~torch.isfinite(got)).any())), \
+                            f"all_reduce {tag} n {m} flag"
+                        done.append(tag)
+                # the flag: one non-finite word in rank r's chunk for destination d
+                n = world * 4104
+                shard = n // world
+                base = _randn(dt, n, 31 * rank + 5)
+                for flag0 in (0.0, 1.0):  # a finite run leaves the flag as it was
+                    fi = torch.full((1,), flag0, device=dev)
+                    dg.reduce_scatter_compressed(base.to(dev), scale_tensor=torch.tensor([s], device=dev),
+                                                 found_inf=fi, **kw)
+                    assert float(fi.item()) == flag0, f"{tag}: finite reduce_scatter, flag {flag0}"
                     if wire is None:
-                        for m in (1, 30001):
-                            tm = rank_data(dt, m, world, 900 + m, widened=reduce_dtype is not None)
-                            fi = torch.zeros(1, device=dev)
-                            got = dg.all_reduce_compressed(tm[rank].to(dev), scale_tensor=torch.tensor([s], device=dev),
-                                                           found_inf=fi, **kw2)
-                            want = dg.all_reduce_compressed(tm[rank].to(dev), scale=s, **kw2)
-                            assert _bits_equal(got, want), f"all_reduce {tag} n {m}"
-                            assert float(fi.item()) == float(bool((~torch.isfinite(got)).any())), \
-                                f"all_reduce {tag} n {m} flag"
-                            done.append(tag)
-                    # the flag: one non-finite word in rank r's chunk for destination d
-                    n = world * 4104
-                    shard = n // world
-                    base = _randn(dt, n, 31 * rank + 5)
-                    for flag0 in (0.0, 1.0):  # a finite run leaves the flag as it was
                         fi = torch.full((1,), flag0, device=dev)
-                        dg.reduce_scatter_compressed(base.to(dev), scale_tensor=torch.tensor([s], device=dev),
+                        dg.all_reduce_compressed(base.to(dev), scale_tensor=torch.tensor([s], device=dev),
+                                                 found_inf=fi, **kw2)
+                        assert float(fi.item()) == flag0, f"{tag}: finite all_reduce, flag {flag0}"
+                for d in range(world):
+                    for r in sorted({d, (d + 1) % world}):
+                        x = base.clone()
+                        if rank == r:
+                            x[d * shard + 4097] = float("inf") if d % 2 == 0 else float("nan")
+                        fi = torch.zeros(1, device=dev)
+                        dg.reduce_scatter_compressed(x.to(dev), scale_tensor=torch.tensor([s], device=dev),
                                                      found_inf=fi, **kw)
-                        assert float(fi.item()) == flag0, f"{tag}: finite reduce_scatter, flag {flag0}"
+                        assert float(fi.item()) == (1.0 if rank == d else 0.0), \
+                            f"{tag}: reduce_scatter, bad word from {r} for {d}, flag on {rank}"
                         if wire is None:
-                            fi = torch.full((1,), flag0, device=dev)
-                            dg.all_reduce_compressed(base.to(dev), scale_tensor=torch.tensor([s], device=dev),
-                                                     found_inf=fi, **kw2)
-                            assert float(fi.item()) == flag0, f"{tag}: finite all_reduce, flag {flag0}"
-                    for d in range(world):
-                        for r in sorted({d, (d + 1) % world}):
-                            x = base.clone()
-                            if rank == r:
-                                x[d * shard + 4097] = float("inf") if d % 2 == 0 else float("nan")
                             fi = torch.zeros(1, device=dev)
-                            dg.reduce_scatter_compressed(x.to(dev), scale_tensor=torch.tensor([s], device=dev),
-                                                         found_inf=fi, **kw)
-                            assert float(fi.item()) == (1.0 if rank == d else 0.0), \
-                                f"{tag}: reduce_scatter, bad word from {r} for {d}, flag on {rank}"
-                            if wire is None:
-                                fi = torch.zeros(1, device=dev)
-                                dg.all_reduce_compressed(x.to(dev), scale_tensor=torch.tensor([s], device=dev),
-                                                         found_inf=fi, **kw2)
-                                assert float(fi.item()) == 1.0, f"{tag}: all_reduce, bad word from {r} for {d}"
-                            done.append(tag)
-    except Exception as e:  # reported to the parent, which fails the test with it
-        msg = f"{type(e).__name__}: {e}"
-    finally:
-        q.put((rank, msg, len(done)))
-        dist.destroy_process_group()
+                            dg.all_reduce_compressed(x.to(dev), scale_tensor=torch.tensor([s], device=dev),
+                                                     found_inf=fi, **kw2)
+                            assert float(fi.item()) == 1.0, f"{tag}: all_reduce, bad word from {r} for {d}"
+                        done.append(tag)
+    return len(done)
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 4])
 def test_devscale_collectives(world):
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 32300 + 4 * (os.getpid() % 100) + (world - 1)  # no other test uses 32300..32699
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    res = {}
-    try:
-        for p in procs:
-            p.start()
-        for _ in range(world):
-            try:
-                r, msg, cnt = q.get(timeout=600)
-            except queue.Empty:
-                break
-            res[r] = (msg, cnt)
-        for p in procs:
-            p.join(timeout=120)
-    finally:
-        started = [p for p in procs if p.pid is not None]
-        for p in started:
-            if p.is_alive():
-                p.terminate()
-        for p in started:
-            p.join(timeout=30)
-            if p.is_alive():
-                p.kill()
-                p.join()
-    print(f"world {world}: checks per rank {[res.get(r, (None, 0))[1] for r in range(world)]}")
-    assert sorted(res) == list(range(world)), res
-    assert all(m == "ok" for m, _ in res.values()), res
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    run_ranks(_worker, world, backend="gloo", timeout=600)

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from dietgpu_b200 import capi
+from multirank import Untouchable, no_communication  # noqa: F401  (no_communication is a fixture)
 
 FAKE = 1 << 20  # never dereferenced: every call below fails (or returns) before it touches memory
 ALLOWED = {(1, 1), (2, 2), (3, 3), (1, 3), (2, 3), (5, 1), (6, 2), (8, 3), (5, 3), (6, 3)}
@@ -84,13 +85,6 @@ def test_signature_is_declared():
 
 # ---- ops.decompress_data_reduce(scale_tensor=, found_inf=) ----------------------------------------------------------
 
-class _Untouchable:
-    """Stands for an archive tensor: any use of it fails the test."""
-
-    def __getattr__(self, name):
-        raise AssertionError(f"the archive was touched ({name}) before the call was refused")
-
-
 def _one(dtype=torch.float32, n=1):
     return torch.ones(n, dtype=dtype)  # on the CPU: never the outputs' CUDA device
 
@@ -113,7 +107,7 @@ def test_ops_refuses_before_touching_archives(kw, match, out_dtype):
 
     out = torch.empty(4, dtype=out_dtype)  # a CPU tensor: any device work would fail differently
     with pytest.raises(ValueError, match=match):
-        ops.decompress_data_reduce([[_Untouchable()]], [out], **kw)
+        ops.decompress_data_reduce([[Untouchable()]], [out], **kw)
 
 
 def test_ops_checks_the_flag_too():
@@ -124,30 +118,17 @@ def test_ops_checks_the_flag_too():
         with pytest.raises(ValueError, match="found_inf"):
             ops._check_flag_tensor("found_inf", bad, torch.device("cpu"))  # a CPU tensor is never accepted
     with pytest.raises(ValueError):
-        ops.decompress_data_reduce([[_Untouchable()]], [out], scale_tensor=_one(), found_inf=_one(n=2))
+        ops.decompress_data_reduce([[Untouchable()]], [out], scale_tensor=_one(), found_inf=_one(n=2))
 
 
 def test_ops_keeps_refusing_tensor_scales():
     from dietgpu_b200 import ops
 
     with pytest.raises(TypeError, match="scale"):
-        ops.decompress_data_reduce([[_Untouchable()]], [torch.empty(4)], scale=torch.tensor(0.5))
+        ops.decompress_data_reduce([[Untouchable()]], [torch.empty(4)], scale=torch.tensor(0.5))
 
 
 # ---- the collectives' refusals --------------------------------------------------------------------------------------
-
-@pytest.fixture
-def no_communication(monkeypatch):
-    """Every torch.distributed call fails the test."""
-    import torch.distributed as dist
-
-    def boom(*a, **k):
-        raise AssertionError("communication before the refusal")
-
-    for name in ("all_gather_into_tensor", "all_to_all_single", "all_gather", "all_reduce", "broadcast", "barrier",
-                 "get_rank", "get_world_size", "get_backend", "is_initialized"):
-        monkeypatch.setattr(dist, name, boom)
-
 
 @pytest.mark.parametrize("kw,match", [
     (dict(scale=0.5, scale_tensor=_one()), "scale_tensor replaces"),

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from dietgpu_b200 import capi
+from multirank import Untouchable, no_communication  # noqa: F401  (no_communication is a fixture)
 from reduce_reference import assert_same_words, f32_to_bf16_words, fold_ref, to_f64
 from scaled_reference import SCALE_IDS, SCALES, scaled_fold_ref, term_ref
 
@@ -84,20 +85,13 @@ def test_signature_is_declared():
 
 # ---- ops.decompress_data_reduce(scale=) -----------------------------------------------------------------------------
 
-class _Untouchable:
-    """Stands for an archive tensor: any use of it fails the test."""
-
-    def __getattr__(self, name):
-        raise AssertionError(f"the archive was touched ({name}) before the call was refused")
-
-
 @pytest.mark.parametrize("scale", [torch.tensor(0.5), "0.5", True, 1j, [0.5]])
 def test_ops_refuses_non_real_scales_first(scale):
     from dietgpu_b200 import ops
 
     out = torch.empty(4, dtype=torch.bfloat16)  # a CPU tensor: any device work would fail differently
     with pytest.raises(TypeError, match="scale"):
-        ops.decompress_data_reduce([[_Untouchable()]], [out], scale=scale)
+        ops.decompress_data_reduce([[Untouchable()]], [out], scale=scale)
 
 
 @pytest.mark.parametrize("sparse", [False, True])
@@ -109,23 +103,10 @@ def test_ops_refuses_bad_pairs_first(archive_dtype, out_dtype, sparse):
 
     out = torch.empty(4, dtype=out_dtype)
     with pytest.raises(ValueError):
-        ops.decompress_data_reduce([[_Untouchable()]], [out], archive_dtype=archive_dtype, sparse=sparse, scale=0.5)
+        ops.decompress_data_reduce([[Untouchable()]], [out], archive_dtype=archive_dtype, sparse=sparse, scale=0.5)
 
 
 # ---- the collectives' refusals --------------------------------------------------------------------------------------
-
-@pytest.fixture
-def no_communication(monkeypatch):
-    """Every torch.distributed call fails the test."""
-    import torch.distributed as dist
-
-    def boom(*a, **k):
-        raise AssertionError("communication before the refusal")
-
-    for name in ("all_gather_into_tensor", "all_to_all_single", "all_gather", "broadcast", "barrier",
-                 "get_rank", "get_world_size", "get_backend", "is_initialized"):
-        monkeypatch.setattr(dist, name, boom)
-
 
 @pytest.mark.parametrize("scale", [0.5, 1.0, float("nan")])
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16, torch.float32])

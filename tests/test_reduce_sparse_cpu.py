@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from dietgpu_b200 import capi
+from multirank import Untouchable, no_communication  # noqa: F401  (no_communication is a fixture)
 
 FAKE = 1 << 20  # never dereferenced: every call below fails (or returns) before it touches memory
 ALLOWED = {(5, 1), (6, 2), (8, 3), (5, 3), (6, 3)}
@@ -81,13 +82,6 @@ def test_signature_is_declared():
 
 # ---- ops.decompress_data_reduce(sparse=True) ------------------------------------------------------------------------
 
-class _Untouchable:
-    """Stands for an archive tensor: any use of it fails the test."""
-
-    def __getattr__(self, name):
-        raise AssertionError(f"the archive was touched ({name}) before the dtype pair was refused")
-
-
 @pytest.mark.parametrize("archive_dtype,out_dtype", [
     (torch.float32, torch.float16), (torch.float32, torch.bfloat16), (torch.float16, torch.bfloat16),
     (torch.bfloat16, torch.float16), (torch.float64, torch.float64), (torch.float64, torch.float32),
@@ -97,22 +91,17 @@ def test_ops_refuses_bad_pairs_first(archive_dtype, out_dtype):
 
     out = torch.empty(4, dtype=out_dtype)  # a CPU tensor: any device work would fail differently
     with pytest.raises(ValueError):
-        ops.decompress_data_reduce([[_Untouchable()]], [out], archive_dtype=archive_dtype, sparse=True)
+        ops.decompress_data_reduce([[Untouchable()]], [out], archive_dtype=archive_dtype, sparse=True)
 
 
 # ---- the collectives' refusals --------------------------------------------------------------------------------------
 
-@pytest.fixture
-def no_communication(monkeypatch):
-    """Every torch.distributed call fails the test."""
+def _allow_world_size_query(monkeypatch):
+    """all_to_all_compressed checks its chunk count against the world size before its other arguments; outside a
+    process group that is 1 and asks nothing of another process."""
     import torch.distributed as dist
 
-    def boom(*a, **k):
-        raise AssertionError("communication before the refusal")
-
-    for name in ("all_gather_into_tensor", "all_to_all_single", "all_gather", "broadcast", "barrier",
-                 "get_rank", "get_world_size", "get_backend"):
-        monkeypatch.setattr(dist, name, boom)
+    monkeypatch.setattr(dist, "is_initialized", lambda: False)
 
 
 @pytest.mark.parametrize("dtype", [torch.float64, torch.int32, torch.uint8, torch.int16])
@@ -123,11 +112,12 @@ def test_collectives_refuse_other_dtypes(dtype, no_communication):
     with pytest.raises(ValueError, match="sparse"):
         dg.all_gather_compressed(t, sparse=True)
     with pytest.raises(ValueError, match="sparse"):
-        dg.all_to_all_compressed([t], sparse=True)
-    with pytest.raises(ValueError, match="sparse"):
         dg.reduce_scatter_compressed(t, sparse=True)
     with pytest.raises(ValueError, match="sparse"):
         dg.all_reduce_compressed(t, sparse=True)
+    _allow_world_size_query(no_communication)
+    with pytest.raises(ValueError, match="sparse"):
+        dg.all_to_all_compressed([t], sparse=True)
 
 
 @pytest.mark.parametrize("wire", [torch.float16, torch.bfloat16])
@@ -149,5 +139,6 @@ def test_collectives_refuse_peer_transports(dtype, no_communication):
     ws = object()  # never used: the refusal comes first
     with pytest.raises(ValueError, match="peer"):
         dg.all_gather_compressed(t, peer=ws, sparse=True)
+    _allow_world_size_query(no_communication)
     with pytest.raises(ValueError, match="peer"):
         dg.all_to_all_compressed([t], peer=ws, sparse=True)

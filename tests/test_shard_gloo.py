@@ -1,14 +1,11 @@
 """world_size-2 gloo test of the multi-GPU plumbing (host logic only): the batch shards by member with
 no data-path collective; ranks only exchange the archive sizes."""
-import os
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from dietgpu_b200.collectives import exchange_archives, pack_offsets
 from dietgpu_b200.shard import gather_sizes, shard_members, shard_range
+from multirank import run_ranks
 
 
 def test_shard_range_partitions():
@@ -25,34 +22,17 @@ def test_shard_range_partitions():
     assert shard_members(list("abcde"), 1, 2) == ["d", "e"]
 
 
-def _worker(rank, world, port, n, q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        mine = shard_range(n, rank, world)
-        # each rank "compresses" its members: fake sizes that encode the member index
-        local = torch.tensor([1000 + 16 * i for i in mine], dtype=torch.int32)
-        allsz = gather_sizes(local, n)
-        q.put((rank, allsz.tolist()))
-    finally:
-        dist.destroy_process_group()
+def _worker(rank, world, dev, n):
+    mine = shard_range(n, rank, world)
+    # each rank "compresses" its members: fake sizes that encode the member index
+    local = torch.tensor([1000 + 16 * i for i in mine], dtype=torch.int32)
+    allsz = gather_sizes(local, n)
+    assert allsz.tolist() == [1000 + 16 * i for i in range(n)], allsz.tolist()
 
 
 @pytest.mark.parametrize("n", [7, 64])
 def test_gather_sizes_world2(n):
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29500 + (os.getpid() % 500) + n
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, n, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=120) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    want = [1000 + 16 * i for i in range(n)]
-    assert res[0] == want and res[1] == want
+    run_ranks(_worker, 2, n, backend=None, timeout=120, join_timeout=60)
 
 
 def test_pack_offsets():
@@ -65,37 +45,20 @@ def _archive(rank, i, size):
     return torch.randint(0, 256, (size,), dtype=torch.uint8, generator=g)
 
 
-def _exchange_worker(rank, world, port, sizes, q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        rows = [_archive(rank, i, s) for i, s in enumerate(sizes[rank])]
-        got = exchange_archives(rows)
-        ok = len(got) == world
-        for w in range(world):
-            ok = ok and len(got[w]) == len(sizes[w])
-            for i, s in enumerate(sizes[w]):
-                ok = ok and got[w][i].numel() == s and torch.equal(got[w][i], _archive(w, i, s))
-        q.put((rank, bool(ok)))
-    finally:
-        dist.destroy_process_group()
+def _exchange_worker(rank, world, dev, sizes):
+    rows = [_archive(rank, i, s) for i, s in enumerate(sizes[rank])]
+    got = exchange_archives(rows)
+    assert len(got) == world
+    for w in range(world):
+        assert len(got[w]) == len(sizes[w])
+        for i, s in enumerate(sizes[w]):
+            assert got[w][i].numel() == s and torch.equal(got[w][i], _archive(w, i, s)), (w, i)
 
 
 @pytest.mark.parametrize("sizes", [[[160, 48, 4112], [16, 70000, 32]], [[32], [1616]]])
 def test_exchange_archives_world2(sizes):
     # variable-size archives, different totals per rank: sizes all-gather + padded payload all-gather
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29700 + (os.getpid() % 200) + len(sizes[0])
-    procs = [ctx.Process(target=_exchange_worker, args=(r, 2, port, sizes, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = dict(q.get(timeout=120) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    assert res == {0: True, 1: True}
+    run_ranks(_exchange_worker, 2, sizes, backend=None, timeout=120, join_timeout=60)
 
 
 def test_exchange_archives_single_process():
