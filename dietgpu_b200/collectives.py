@@ -556,6 +556,23 @@ def _check_reducible(t: torch.Tensor, what: str, reduce_dtype: Optional[torch.dt
                      f"not {reduce_dtype} for {t.dtype}")
 
 
+def _check_out_dtype(what: str, out_dtype: Optional[torch.dtype], dtype: torch.dtype,
+                     reduce_dtype: Optional[torch.dtype], wire_dtype: Optional[torch.dtype]) -> Optional[torch.dtype]:
+    """The result's dtype for a tensor of `dtype`: None for the sum's (which _check_reducible checks), or the archives'
+    16-bit dtype for a float32 sum, which the decode-and-sum rounds once from its float32 sums
+    (ops.decompress_data_reduce(reduce_dtype=torch.float32)).  Reads dtypes only, so it refuses before any other
+    check of t."""
+    acc_dtype = torch.float32 if torch.float32 in (dtype, reduce_dtype) else dtype
+    arch_dtype = wire_dtype or dtype
+    if out_dtype is None or out_dtype == acc_dtype:
+        return None
+    if acc_dtype == torch.float32 and out_dtype == arch_dtype and arch_dtype in (torch.float16, torch.bfloat16):
+        return out_dtype
+    raise ValueError(f"{what}: out_dtype is None, the sum's dtype {acc_dtype}, or the archives' dtype for a float32 "
+                     f"sum of float16 / bfloat16 archives; not {out_dtype} for {arch_dtype} archives summed in "
+                     f"{acc_dtype}")
+
+
 def _check_scale(what: str, scale, average: bool, scale_tensor=None, found_inf=None,
                  dev=None) -> Optional[np.float32]:
     """The float32 pre-multiplier a scale argument stands for (None: a plain sum, or a device scale_tensor); average
@@ -607,7 +624,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               wire_dtype: Optional[torch.dtype] = None, sparse: bool = False,
                               scale: Optional[float] = None, average: bool = False,
                               scale_tensor: Optional[torch.Tensor] = None,
-                              found_inf: Optional[torch.Tensor] = None) -> torch.Tensor:
+                              found_inf: Optional[torch.Tensor] = None,
+                              out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -646,11 +664,21 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     is bit-identical to this call with scale=float(scale_tensor).  Not with scale or average=True.  found_inf (with
     scale_tensor; the same kind of tensor) is set to 1.0 when any element of the returned shard is inf or NaN, and
     never cleared (torch.amp's found_inf convention), without a host sync.  These keywords raise ValueError before
-    any communication."""
+    any communication.
+
+    out_dtype: the result's dtype.  None is the sum's dtype.  When the sum is float32 of float16 / bfloat16 archives
+    (reduce_dtype=torch.float32 with a 16-bit t, or a float32 t with wire_dtype), out_dtype may be the archives'
+    dtype: the sum is still taken in float32 and rounded once per element inside the decode-and-sum kernel, so the
+    result is this call without out_dtype followed by .to(out_dtype), bit for bit on every rank, without a float32
+    result (found_inf then sees the rounded elements).  Any other value raises ValueError before any
+    communication."""
     s32 = _check_scale("reduce_scatter_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
+    narrow_dtype = _check_out_dtype("reduce_scatter_compressed", out_dtype, t.dtype, reduce_dtype, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
+    arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
+    res_dtype = narrow_dtype or acc_dtype
     world = _world(group)
     if average:
         s32 = np.float32(1 / world)
@@ -659,9 +687,10 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
-    arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     if world == 1 or n == 0:
-        return _local_sum(flat[: n // world].to(arch_dtype), acc_dtype, sd, found_inf)
+        if res_dtype == acc_dtype:
+            return _local_sum(flat[: n // world].to(arch_dtype), acc_dtype, sd, found_inf)
+        return _local_sum(_term(flat[: n // world].to(arch_dtype), acc_dtype, sd), res_dtype, None, found_inf)
     rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
@@ -675,8 +704,11 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     for k, d in enumerate(dests):
         per_dest[d] = [comp[k * m + i, :hs[k * m + i]] for i in range(m)]
     archives, _ = _send_to_each(per_dest, group)  # archives[s][i]: member i of the chunk source s sent here
-    out = torch.empty(shard, dtype=acc_dtype, device=dev)
+    out = torch.empty(shard, dtype=acc_dtype, device=dev)  # the running sums (all of it, unless narrowing)
     outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
+    # narrowing: the later sources' call rounds the float32 sums once into res, accumulating from out
+    res = out if res_dtype == acc_dtype else torch.empty(shard, dtype=res_dtype, device=dev)
+    narrow = {} if res is out else dict(reduce_dtype=torch.float32, acc=outs)
     own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
     if sd is not None:
         own = _term(own, acc_dtype, sd)  # the kernel's term of the own chunk, already in the result's dtype
@@ -694,22 +726,27 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     if rank + 1 < world:
         # the last call writes the final values: the kernel checks them
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
-        ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
-                                   temp_mem, st, archive_dtype=arch_dtype, sparse=sparse, scale=s32,
-                                   scale_tensor=scale_tensor, found_inf=found_inf)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)],
+                                   [res[bounds[i]:bounds[i + 1]] for i in range(m)], True, temp_mem, st,
+                                   archive_dtype=arch_dtype, sparse=sparse, scale=s32, scale_tensor=scale_tensor,
+                                   found_inf=found_inf, **narrow)
         statuses.append(st)
     else:
-        _flag_non_finite(found_inf, out)  # the last rank ends on torch's add of its own chunk
+        # the last rank ends on torch's add of its own chunk (and torch's rounding of it when narrowing)
+        if res is not out:
+            res.copy_(out)
+        _flag_non_finite(found_inf, res)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
-    return out
+    return res
 
 
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,
                           check: bool = True, reduce_dtype: Optional[torch.dtype] = None,
                           sparse: bool = False, scale: Optional[float] = None,
                           average: bool = False, scale_tensor: Optional[torch.Tensor] = None,
-                          found_inf: Optional[torch.Tensor] = None) -> torch.Tensor:
+                          found_inf: Optional[torch.Tensor] = None,
+                          out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
@@ -720,23 +757,33 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     (s = np.float32(1 / world); not both) pre-multiplies every rank's term as in reduce_scatter_compressed: the
     result is the rank-order fold of (t_r.float() * s32).to(acc) on every rank, bit for bit.  scale_tensor and
     found_inf are reduce_scatter_compressed's, except that found_inf covers the whole result on every rank: the
-    shards' flags meet in one MAX all-reduce of a one-element tensor."""
+    shards' flags meet in one MAX all-reduce of a one-element tensor.
+
+    out_dtype is reduce_scatter_compressed's: t.dtype for a float16 / bfloat16 t summed with
+    reduce_dtype=torch.float32 makes the shards come back rounded once to t.dtype, the second phase all-gathers
+    16-bit archives instead of float32 ones, and the result is this call without out_dtype followed by
+    .to(out_dtype), bit for bit on every rank.  Any other out_dtype raises ValueError before any communication."""
     s32 = _check_scale("all_reduce_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sparse_wire(t.dtype, "all_reduce_compressed", sparse)
+    narrow_dtype = _check_out_dtype("all_reduce_compressed", out_dtype, t.dtype, reduce_dtype, None)
     acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
+    res_dtype = narrow_dtype or acc_dtype
     world = _world(group)
     if average:
         s32 = np.float32(1 / world)
     flat = t.reshape(-1)
     n = flat.numel()
     if world == 1 or n == 0:
-        return _local_sum(t, acc_dtype, s32 if scale_tensor is None else scale_tensor, found_inf)
+        sd = s32 if scale_tensor is None else scale_tensor
+        if res_dtype == acc_dtype:
+            return _local_sum(t, acc_dtype, sd, found_inf)
+        return _local_sum(_term(t, acc_dtype, sd), res_dtype, None, found_inf)
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
     # (a padding zero's term is non-finite only for an inf or NaN scale, which makes every element's term so too)
     shard_inf = None if found_inf is None else torch.zeros(1, dtype=torch.float32, device=t.device)
     shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse,
-                                      scale=s32, scale_tensor=scale_tensor, found_inf=shard_inf)
+                                      scale=s32, scale_tensor=scale_tensor, found_inf=shard_inf, out_dtype=res_dtype)
     if found_inf is not None:
         on_device = _device_collectives(group)
         flag = shard_inf if on_device else shard_inf.cpu()

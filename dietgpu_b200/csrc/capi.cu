@@ -573,6 +573,24 @@ int dgb_float_decompress_reduce_scaled_dev(void* temp, size_t tempBytes, int ft,
                       outSuccess_dev, isSparseKind(ft), nullptr, scale_dev, foundInf_dev, (cudaStream_t)stream);
 }
 
+int dgb_float_decompress_reduce_narrow(void* temp, size_t tempBytes, int ft, int pb, uint32_t numGroups,
+                                       uint32_t archivesPerGroup, const void* const* in, float* const* acc,
+                                       void* const* out, const uint32_t* outSize, int accumulate, const float* scale,
+                                       const float* scale_dev, float* foundInf_dev, uint8_t* outSuccess_dev,
+                                       void* stream) {
+  // fp16 / bf16 archives, dense or sparse, summed in fp32 from the fp32 accumulators acc[g] into outputs of the
+  // archives' 16-bit type; unscaled, host-scaled (scale) or device-scale (scale_dev, with the optional flag)
+  if (ft != kKindF16 && ft != kKindBF16 && ft != kKindF16S && ft != kKindBF16S) return DGB_ERR_INVALID_ARG;
+  if (scale && scale_dev) return DGB_ERR_INVALID_ARG;
+  if (foundInf_dev && !scale_dev) return DGB_ERR_INVALID_ARG;
+  if (scale_dev && (reinterpret_cast<uintptr_t>(scale_dev) & 3u)) return DGB_ERR_INVALID_ARG;
+  if (reinterpret_cast<uintptr_t>(foundInf_dev) & 3u) return DGB_ERR_INVALID_ARG;
+  if (numGroups && !out) return DGB_ERR_INVALID_ARG;
+  return decodeReduce(ft, kKindF32, temp, tempBytes, pb, numGroups, archivesPerGroup, in,
+                      reinterpret_cast<void* const*>(acc), outSize, accumulate != 0, outSuccess_dev, isSparseKind(ft),
+                      scale, scale_dev, foundInf_dev, (cudaStream_t)stream, out);
+}
+
 // ---- info ------------------------------------------------------------------
 
 int dgb_ans_get_compressed_info(void* temp, size_t tempBytes, const void* const* in,

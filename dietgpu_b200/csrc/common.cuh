@@ -209,7 +209,13 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
-                 cudaStream_t stream);
+                 cudaStream_t stream, void* const* narrowOut = nullptr);
+// the narrowing sums' kernels (decode_narrow.cu): decodeReduce's launches of kind | kWidenF32 | kNarrowOut, scaled
+// (host scale) or with scaleDev / foundInf, reading the groups' 16-bit outputs from the device table narrowTable
+int launchDecodeReduceNarrow(int kind, int pb, bool scaled, const Options& opt, MemberDesc* members, uint32_t* next,
+                             const InlineMembers& im, uint32_t groups, uint32_t width, uint64_t totalChunks,
+                             bool accumulate, uint8_t* outSuccess, cudaStream_t stream, const float* scaleDev,
+                             float* foundInf, void* const* narrowTable);
 size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize);
 size_t decodeTempBytes(int kind, uint32_t n);
 int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool inIsDevice,

@@ -153,15 +153,18 @@ constexpr uint32_t kRingSlots = 3;              // groups resident per warp: cur
 // output's word; | kWidenF32 writes (or adds into) fp32 outputs from fp16 / bf16 archives (dense or sparse);
 // | kScaled multiplies every decoded word by the call's scale first (0x40 is the encoder's narrowing bit);
 // | kDevScale (kernels only, with kScaled) reads that scale from device memory when the kernel runs;
-// | kCheckFinite (writers only) also reports whether a word it stores is inf or NaN
+// | kCheckFinite (writers only) also reports whether a word it stores is inf or NaN;
+// | kNarrowOut (with kWidenF32) sums in fp32 from an fp32 accumulator and stores the sum rounded once to the
+// archive's 16-bit type into a second output (the narrowing sums: kernels and the writer of a call's last archive)
 constexpr int kAddWriter = 0x10;
 constexpr int kWidenF32 = 0x20;
 constexpr int kScaled = 0x80;
 constexpr int kDevScale = 0x100;
 constexpr int kCheckFinite = 0x200;
+constexpr int kNarrowOut = 0x400;
 // the archive kind of a decode-and-sum kernel or writer kind
 __host__ __device__ constexpr int reduceArchiveKind(int k) {
-  return k & ~(kAddWriter | kWidenF32 | kScaled | kDevScale | kCheckFinite);
+  return k & ~(kAddWriter | kWidenF32 | kScaled | kDevScale | kCheckFinite | kNarrowOut);
 }
 
 template <int KIND>
@@ -1079,6 +1082,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
 
 // XOR checksum of decoded outputs (ans/GpuChecksum.cuh:26-93 semantics: XOR of
 // all bytes folded to 8 bits).  grid = (n, Y).
+#ifndef DGB_DECODE_NARROW_TU
 __global__ void __launch_bounds__(256)
 checksumKernel(DecodeScratch sc) {
   const uint32_t m = blockIdx.x;
@@ -1091,6 +1095,7 @@ checksumKernel(DecodeScratch sc) {
   for (int d = 16; d >= 1; d >>= 1) x ^= __shfl_xor_sync(0xffffffffu, x, d);
   if ((threadIdx.x & 31) == 0 && x) atomicXor(sc.checksum + m, x & 0xffu);
 }
+#endif
 
 struct DecodePlan {
   size_t members, next, totals, checksum, archiveChecksum, sizes, total;
@@ -1247,19 +1252,23 @@ __device__ __forceinline__ uint32_t widenWord(uint32_t w) {
 // The terms of the scaled sums.  __fmul_rn is one mul.rn.f32 that nvcc never contracts with the add that follows
 // into an FFMA (a fused multiply-add rounds once, the contract twice).  scaleWord: a word of dense kind KIND times s,
 // in that kind: fp32 products as they are, 16-bit words widened exactly and the fp32 product rounded back to the
-// 16-bit type with round-to-nearest-even.  scaleWiden: a 16-bit word's fp32 product, left in fp32.
+// 16-bit type with round-to-nearest-even (narrowWord, which also rounds the narrowing sums' fp32 results).
+// scaleWiden: a 16-bit word's fp32 product, left in fp32.
+template <int KIND>
+__device__ __forceinline__ uint32_t narrowWord(float p) {
+  unsigned short r;
+  if constexpr (KIND == kKindF16)
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(r) : "f"(p));
+  else
+    asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(p));
+  return r;
+}
 template <int KIND>
 __device__ __forceinline__ uint32_t scaleWord(uint32_t w, float s) {
   if constexpr (KIND == kKindF32) {
     return __float_as_uint(__fmul_rn(__uint_as_float(w), s));
   } else {
-    const float p = __fmul_rn(__uint_as_float(widenWord<KIND>(w)), s);
-    unsigned short r;
-    if constexpr (KIND == kKindF16)
-      asm("cvt.rn.f16.f32 %0, %1;" : "=h"(r) : "f"(p));
-    else
-      asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(p));
-    return r;
+    return narrowWord<KIND>(__fmul_rn(__uint_as_float(widenWord<KIND>(w)), s));
   }
 }
 template <int KIND>
@@ -1289,10 +1298,18 @@ template <bool SCALED>
 struct SumScale { static constexpr float scale = 1.0f; };  // unscaled sums: combine ignores it
 template <>
 struct SumScale<true> { float scale; };  // the call's scale; decodeReduceBlock sets it
+template <bool NARROW>
+struct SumNarrowOut {};
+template <>
+struct SumNarrowOut<true> { uint16_t* dst; };  // this lane's element of the block in the 16-bit output
 
-// the kind in which a decode-and-sum writer kind adds, which is also the type it stores
+// the kind in which a decode-and-sum writer kind adds, which is the type it stores except for the narrowing writers
 __host__ __device__ constexpr int reduceSumKind(int wk) {
   return (wk & kWidenF32) != 0 ? kKindF32 : denseKind(reduceArchiveKind(wk));
+}
+// the type a decode-and-sum writer kind stores: the sum kind, or the archive's 16-bit type (| kNarrowOut)
+__host__ __device__ constexpr int reduceStoreKind(int wk) {
+  return (wk & kNarrowOut) != 0 ? denseKind(reduceArchiveKind(wk)) : reduceSumKind(wk);
 }
 
 // The decode-and-sum writer of writer kind WK: the archive kind's writer B (its ring, copies and join; a sparse
@@ -1302,26 +1319,32 @@ __host__ __device__ constexpr int reduceSumKind(int wk) {
 //   2. the term: w, or w widened exactly to fp32 (| kWidenF32: widenWord), or w times the call's scale
 //      (| kScaled: scaleWord in the archive's dense type, scaleWiden when widening);
 //   3. (| kAddWriter) the term added to the element's running sum with one addWord in the sum kind;
-//   4. (| kCheckFinite) the result noted by FiniteCheck before it is stored.
-// It stores one u16 (same-type fp16 / bf16 sums) or one u32 (fp32 and widening sums: a row is one 128 B store)
-// per element.  Add writers load a row group's running sums when the group starts (volatile loads in at(), so they
-// are issued there), writeSlow and writePartial the one sum they add to.  A sparse word votes across the warp, so
-// sparse rows, the partial one too (writePartial), run on the whole warp, and the vote comes before the running
-// sum is read.  The unscaled store of archive 0 (WK = the bare archive kind) is the archive kind's own writer.
+//   4. (| kNarrowOut) the fp32 result rounded once to the archive's 16-bit type (narrowWord);
+//   5. (| kCheckFinite) the result noted by FiniteCheck before it is stored.
+// It stores one u16 (same-type fp16 / bf16 sums, and the narrowing writers) or one u32 (fp32 and widening sums: a
+// row is one 128 B store) per element.  Add writers load a row group's running sums when the group starts (volatile
+// loads in at(), so they are issued there), writeSlow and writePartial the one sum they add to.  A narrowing writer
+// loads its running sums from `sum`, the fp32 accumulator, and stores to `dst`, the 16-bit output; it never reads
+// `dst` and never writes `sum`.  A sparse word votes across the warp, so sparse rows, the partial one too
+// (writePartial), run on the whole warp, and the vote comes before the running sum is read.  The unscaled store of
+// archive 0 (WK = the bare archive kind) is the archive kind's own writer.
 template <int WK>
 struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
                       SumScale<(WK & kScaled) != 0>,
-                      std::conditional<(WK & kCheckFinite) != 0, FiniteCheck<reduceSumKind(WK)>, NoFiniteCheck>::type {
+                      SumNarrowOut<(WK & kNarrowOut) != 0>,
+                      std::conditional<(WK & kCheckFinite) != 0, FiniteCheck<reduceStoreKind(WK)>, NoFiniteCheck>::type {
   typedef RowWriter<reduceArchiveKind(WK)> B;
   static constexpr int AK = reduceArchiveKind(WK), kSumKind = reduceSumKind(WK);
   static constexpr bool kAdd = (WK & kAddWriter) != 0, kWiden = (WK & kWidenF32) != 0;
-  static constexpr bool kScale = (WK & kScaled) != 0;
+  static constexpr bool kScale = (WK & kScaled) != 0, kNarrow = (WK & kNarrowOut) != 0;
+  static_assert(!kNarrow || kWiden, "a narrowing writer sums in fp32");
   typedef typename std::conditional<kSumKind == kKindF32, uint32_t, uint16_t>::type T;
   T* sum;
   struct Cursor {
     T* o;
     typename B::Cursor in;      // B's cursor of the group: its ring addresses (its output pointer goes unused)
     uint32_t prev[kGroupRows];  // add writers: the running sums of the group's rows
+    uint16_t* d;                // narrowing writers: the group's first row in the 16-bit output
   };
   __device__ __forceinline__ void setBlock(const ArchiveView& av, void* outBase, uint32_t block, uint32_t l) {
     B::setBlock(av, outBase, block, l);
@@ -1337,9 +1360,10 @@ struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
         else c.prev[j] = ldGlobalU16(c.o + j * 32);
       }
     }
+    if constexpr (kNarrow) c.d = this->dst + row * 32u;
     return c;
   }
-  // steps 2 and 3 (prev: add writers only); this->note() around it is step 4.  Static, as are the unscaled scale and
+  // steps 2 to 4 (prev: add writers only); this->note() around it is step 5.  Static, as are the unscaled scale and
   // the unchecked note: passing the writer into the store path makes the sparse fp32 add writer spill more
   static __device__ __forceinline__ uint32_t combine(uint32_t prev, uint32_t w, float s) {
     uint32_t v = w;
@@ -1347,15 +1371,21 @@ struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
     else if constexpr (kScale) v = scaleWord<denseKind(AK)>(w, s);
     else if constexpr (kWiden) v = widenWord<denseKind(AK)>(w);
     if constexpr (kAdd) v = addWord<kSumKind>(prev, v);
+    if constexpr (kNarrow) v = narrowWord<denseKind(AK)>(__uint_as_float(v));
     return v;
   }
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
-    c.o[J * 32] = (T)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
+    if constexpr (kNarrow)
+      c.d[J * 32] = (uint16_t)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
+    else
+      c.o[J * 32] = (T)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
   }
   __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
     if constexpr (isSparseKind(AK)) {
       writePartial(row, entry, true);
+    } else if constexpr (kNarrow) {
+      this->dst[row * 32u] = (uint16_t)this->note(combine(kAdd ? sum[row * 32u] : 0u, B::wordSlow(row, entry), this->scale));
     } else if constexpr (kAdd) {
       T* o = sum + row * 32u;
       *o = (T)this->note(combine(*o, B::wordSlow(row, entry), this->scale));
@@ -1368,14 +1398,18 @@ struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
     const uint32_t w = B::word(entry, valid);
     if (valid) {
       T* o = sum + row * 32u;
-      *o = (T)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
+      if constexpr (kNarrow)
+        this->dst[row * 32u] = (uint16_t)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
+      else
+        *o = (T)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
     }
   }
 };
 // every writer kind other than the bare archive kinds, whose own writers are above
 template <int KIND>
 struct RowWriter : RowWriterSum<KIND> {
-  static_assert((KIND & (kAddWriter | kWidenF32 | kScaled | kCheckFinite)) != 0, "not a decode-and-sum writer kind");
+  static_assert((KIND & (kAddWriter | kWidenF32 | kScaled | kCheckFinite | kNarrowOut)) != 0,
+                "not a decode-and-sum writer kind");
 };
 
 // An archive may join group g iff its float header has the magic and KIND, its ANS header has PB and a block count
@@ -1389,13 +1423,14 @@ __device__ __forceinline__ bool reduceArchiveOk(const void* in, uint32_t words) 
   return h0.x == kAnsMagicVersion && (int)(h1.x & 0xfu) == PB && h0.z == words && h0.y == divUp(words, kBlockBytes);
 }
 
-// block `block` of one archive through writer kind WK (the single-launch decoder's block body)
+// block `block` of one archive through writer kind WK (the single-launch decoder's block body); narrowOut: the
+// group's 16-bit output, which only the narrowing writers (| kNarrowOut) store to
 template <int WK, int PB>
 __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, uint32_t block, uint32_t nb,
                                                   const typename Lut<PB, false>::Entry* __restrict__ lut,
                                                   uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
                                                   uint32_t slotWords, uint32_t lane, float scale,
-                                                  float* foundInf) {
+                                                  float* foundInf, void* narrowOut) {
   const ArchiveView av = openArchive<reduceArchiveKind(WK)>(in);
   const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
   const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
@@ -1405,6 +1440,10 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
   wr.setRing(ring, lane);
   wr.setBlock(av, out, block, lane);
   if constexpr ((WK & kScaled) != 0) wr.scale = scale;
+  if constexpr ((WK & kNarrowOut) != 0) {
+    wr.dst = static_cast<uint16_t*>(narrowOut) + (size_t)block * kBlockBytes + lane;
+    __builtin_assume(__isGlobal(wr.dst));
+  }
   const uint2 bw = __ldg(pBlockWords + block);
   const uint32_t blockLen = bw.x >> 16, words = bw.x & 0xffffu;
   const uint16_t* stream = pData + bw.y;
@@ -1440,12 +1479,16 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
 }
 
 // f(std::integral_constant<int, K>()) with K the writer kind of one archive: WK when it is stored (archive a0 of a
-// pass that does not add), WK | kAddWriter when it is added; | kCheckFinite as well when it is checked (CHECK kinds
-// only, so the others instantiate no checking writer)
-template <int WK, bool CHECK, typename F>
-__device__ __forceinline__ void withWriterKind(bool store, bool check, F&& f) {
+// pass that does not add), WK | kAddWriter when it is added; | kNarrowOut as well for the last archive of a
+// narrowing sum (NARROW kinds only), and | kCheckFinite for the last archive of a checked sum (CHECK kinds only, so
+// the others instantiate no checking or narrowing writer)
+template <int WK, bool CHECK, bool NARROW = false, typename F>
+__device__ __forceinline__ void withWriterKind(bool store, bool last, F&& f) {
+  if constexpr (NARROW) {
+    if (last) return withWriterKind<WK | kNarrowOut, CHECK>(store, true, f);
+  }
   if constexpr (CHECK) {
-    if (check) return withWriterKind<WK | kCheckFinite, false>(store, false, f);
+    if (last) return withWriterKind<WK | kCheckFinite, false>(store, false, f);
   }
   if (store) f(std::integral_constant<int, WK>());
   else f(std::integral_constant<int, WK | kAddWriter>());
@@ -1458,14 +1501,19 @@ __device__ __forceinline__ void withWriterKind(bool store, bool check, F&& f) {
 // (decodeReduceDevScaleKernel: the scale is *scaleDev, read once per CTA in every pass; the writer of archive
 // width - 1, the last pass's last, checks the words it stores and sets *foundInf, when not null, to 1.0f on inf or
 // NaN).  The writers of a device-scale kind are the host-scaled ones: only where s comes from differs.
+// | kNarrowOut (decodeReduceNarrowKernel, with kWidenF32): the members' out is the group's fp32 accumulator and
+// narrowOut[g] its 16-bit output; archive width - 1 goes through the narrowing writer, which reads the accumulator
+// and stores the rounded sum to narrowOut[g], and every other archive through the widening writers into the
+// accumulator.
 template <int KIND, int PB>
 __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
                                                  uint32_t width, uint32_t a0, uint32_t a1, bool addFirst,
                                                  uint32_t slotWords, uint8_t* __restrict__ outSuccess,
-                                                 const float* scaleDev, float* foundInf) {
+                                                 const float* scaleDev, float* foundInf, void* const* narrowOut) {
   constexpr int AK = reduceArchiveKind(KIND);
   constexpr bool DEV = (KIND & kDevScale) != 0;
-  constexpr int WK = KIND & ~kDevScale;  // the writer kind of archive 0; | kAddWriter for the others
+  constexpr bool NARROW = (KIND & kNarrowOut) != 0;
+  constexpr int WK = KIND & ~(kDevScale | kNarrowOut);  // the writer kind of archive 0; | kAddWriter for the others
   constexpr int WARPS = kReduceWarps;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t K = 1u << PB;
@@ -1541,6 +1589,8 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
     const bool report = sMisc[2] != 0;
     const MemberDesc gd = memberAt(im, sc.members, g * width);
     const uint32_t blocksCap = gd.work0, nb = divUp(gd.size, kBlockBytes);
+    void* nout = nullptr;
+    if constexpr (NARROW) nout = narrowOut[g];
 
     // ---- every archive of the group is checked before anything is stored to it: the decision depends on the
     //      headers and out_size alone, so every CTA and every pass takes the same one ----
@@ -1569,11 +1619,12 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
       if (work && block < nb) {
         for (uint32_t a = a0; a < a1; ++a) {
           const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
-          // the device-scale sums check archive width - 1: the final value of every element
-          withWriterKind<WK, DEV>(a == a0 && !addFirst, a + 1 == width, [&](auto wk) {
+          // archive width - 1 writes the final value of every element: the device-scale sums check it there, and
+          // the narrowing sums round it there
+          withWriterKind<WK, DEV, NARROW>(a == a0 && !addFirst, a + 1 == width, [&](auto wk) {
             constexpr int W = decltype(wk)::value;
             decodeReduceBlock<W, PB>(in, gd.out, block, nb, lut[(W & kAddWriter) != 0 ? a - a0 : 0u], ring, mySlot,
-                                     myBar, phase, slotWords, lane, scale, foundInf);
+                                     myBar, phase, slotWords, lane, scale, foundInf, nout);
           });
         }
       }
@@ -1587,8 +1638,9 @@ template <int KIND, int PB>
 __global__ void __launch_bounds__(kReduceWarps * 32, 4)
 decodeReduceKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups, uint32_t width,
                    uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords, uint8_t* __restrict__ outSuccess) {
-  static_assert((KIND & kDevScale) == 0, "");
-  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, nullptr, nullptr);
+  static_assert((KIND & (kDevScale | kNarrowOut)) == 0, "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, nullptr, nullptr,
+                             nullptr);
 }
 // the device-scale sums (KIND | kScaled | kDevScale): the same body with the scale's and the flag's pointers
 template <int KIND, int PB>
@@ -1597,17 +1649,33 @@ decodeReduceDevScaleKernel(DecodeScratch sc, const __grid_constant__ InlineMembe
                            uint32_t width, uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords,
                            uint8_t* __restrict__ outSuccess, const float* __restrict__ scaleDev,
                            float* __restrict__ foundInf) {
-  static_assert((KIND & (kScaled | kDevScale)) == (kScaled | kDevScale), "");
-  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf);
+  static_assert((KIND & (kScaled | kDevScale | kNarrowOut)) == (kScaled | kDevScale), "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf,
+                             nullptr);
+}
+// the narrowing sums (archive kind | kWidenF32 | kNarrowOut, | kScaled, | kScaled | kDevScale): the same body with
+// the device table of the groups' 16-bit outputs; scaleDev and foundInf are those of the device-scale kinds (null
+// for the others)
+template <int KIND, int PB>
+__global__ void __launch_bounds__(kReduceWarps * 32, 4)
+decodeReduceNarrowKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups,
+                         uint32_t width, uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords,
+                         uint8_t* __restrict__ outSuccess, const float* __restrict__ scaleDev,
+                         float* __restrict__ foundInf, void* const* __restrict__ narrowOut) {
+  static_assert((KIND & (kWidenF32 | kNarrowOut)) == (kWidenF32 | kNarrowOut), "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf,
+                             narrowOut);
 }
 
 template <int KIND, int PB>
 int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
                        uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream,
-                       const float* scaleDev = nullptr, float* foundInf = nullptr) {
-  constexpr bool DEV = (KIND & kDevScale) != 0;
+                       const float* scaleDev = nullptr, float* foundInf = nullptr,
+                       void* const* narrowOut = nullptr) {
+  constexpr bool DEV = (KIND & kDevScale) != 0, NARROW = (KIND & kNarrowOut) != 0;
   const void* kern;
-  if constexpr (DEV) kern = (const void*)decodeReduceDevScaleKernel<KIND, PB>;
+  if constexpr (NARROW) kern = (const void*)decodeReduceNarrowKernel<KIND, PB>;
+  else if constexpr (DEV) kern = (const void*)decodeReduceDevScaleKernel<KIND, PB>;
   else kern = (const void*)decodeReduceKernel<KIND, PB>;
   uint32_t slotWords;
   const size_t smemBytes = decoderSmem<reduceArchiveKind(KIND), PB>(kReduceWarps, opt, &slotWords);
@@ -1621,7 +1689,10 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
     DGB_CUDA_TRY(cudaMemsetAsync(sc.next, 0, 8 * (size_t)groups * width, stream));
     timerBegin(opt, kSlotDecode, stream);
     const uint32_t a1 = std::min(width, a0 + kReducePass);
-    if constexpr (DEV)
+    if constexpr (NARROW)
+      decodeReduceNarrowKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
+          sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess, scaleDev, foundInf, narrowOut);
+    else if constexpr (DEV)
       decodeReduceDevScaleKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
           sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess, scaleDev, foundInf);
     else
@@ -1634,6 +1705,37 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
 }
 
 }  // namespace
+
+#ifdef DGB_DECODE_NARROW_TU
+// decode_narrow.cu compiles this file once more with DGB_DECODE_NARROW_TU: that module holds the narrowing sums'
+// kernels and this launcher only.  In the main module their 36 kernels changed the code ptxas generated for the
+// sparse fp32 decode-and-sum kernels (the same sources gave a different and longer schedule), so they are kept apart.
+int launchDecodeReduceNarrow(int kind, int pb, bool scaled, const Options& opt, MemberDesc* members, uint32_t* next,
+                             const InlineMembers& im, uint32_t groups, uint32_t width, uint64_t totalChunks,
+                             bool accumulate, uint8_t* outSuccess, cudaStream_t stream, const float* scaleDev,
+                             float* foundInf, void* const* narrowTable) {
+  DecodeScratch sc{};
+  sc.members = members;
+  sc.next = next;
+  sc.seen = next + (size_t)groups * width;
+  return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
+    constexpr int KIND = decltype(K)::value, PB = decltype(P)::value;
+    if constexpr (denseKind(KIND) == kKindF16 || denseKind(KIND) == kKindBF16) {
+      constexpr int NK = KIND | kWidenF32 | kNarrowOut;
+      if (scaled)
+        return launchDecodeReduce<NK | kScaled, PB>(opt, sc, im, groups, width, totalChunks, accumulate, outSuccess,
+                                                    stream, nullptr, nullptr, narrowTable);
+      if (!scaleDev)
+        return launchDecodeReduce<NK, PB>(opt, sc, im, groups, width, totalChunks, accumulate, outSuccess, stream,
+                                          nullptr, nullptr, narrowTable);
+      return launchDecodeReduce<NK | kScaled | kDevScale, PB>(opt, sc, im, groups, width, totalChunks, accumulate,
+                                                              outSuccess, stream, scaleDev, foundInf, narrowTable);
+    } else {
+      return (int)DGB_ERR_INVALID_ARG;  // not reached (decodeReduce checks the kind)
+    }
+  }); });
+}
+#else
 
 size_t decodeTempBytes(int /*kind*/, uint32_t n) { return planDecodeScratch(n).total + 256; }
 
@@ -1773,18 +1875,23 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
-                 cudaStream_t stream) {
+                 cudaStream_t stream, void* const* narrowOut) {
   // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8; scale: null for a plain sum, else
   // the multiplier of the scaled kinds; scaleDev (device memory, read by the kernels) in place of scale for the
-  // device-scale kinds, with the non-finite flag foundInf (may be null)
+  // device-scale kinds, with the non-finite flag foundInf (may be null).  narrowOut (host array of G, or null): a
+  // narrowing sum of fp16 / bf16 archives, whose out[g] (outKind fp32) is the group's accumulator and narrowOut[g]
+  // its output of the archive's 16-bit type; out and out[g] may be null when the call reads no accumulator (W = 1
+  // without accumulate)
   if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
   // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
   const int dk = denseKind(kind);
   const bool widen = outKind != dk;
   if (widen && !(outKind == kKindF32 && (dk == kKindF16 || dk == kKindBF16))) return DGB_ERR_INVALID_ARG;
+  if (narrowOut && !widen) return DGB_ERR_INVALID_ARG;
   if (pb < 9 || pb > 11 || width == 0) return DGB_ERR_INVALID_ARG;
   if (groups == 0) return DGB_OK;
-  if (!in || !out || !outSize) return DGB_ERR_INVALID_ARG;
+  const bool readsAcc = !narrowOut || width > 1 || accumulate;
+  if (!in || (readsAcc && !out) || !outSize) return DGB_ERR_INVALID_ARG;
   const uint64_t n64 = (uint64_t)groups * width;
   if (n64 > 0xffffffffull) return DGB_ERR_INVALID_ARG;
   const uint32_t n = (uint32_t)n64;
@@ -1799,14 +1906,19 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   const uint32_t elemBytes = wordBytes(outKind);
   uint64_t totalChunks = 0;
   for (uint32_t g = 0; g < groups; ++g) {
-    if ((outSize[g] && !out[g]) || (reinterpret_cast<uintptr_t>(out[g]) & (elemBytes - 1u))) return DGB_ERR_INVALID_ARG;
+    if (narrowOut && ((outSize[g] && !narrowOut[g]) || (reinterpret_cast<uintptr_t>(narrowOut[g]) & 1u)))
+      return DGB_ERR_INVALID_ARG;
+    // a narrowing call that reads no accumulator never touches the members' out: the 16-bit output stands in for it
+    // (any global pointer does)
+    void* o = readsAcc ? out[g] : narrowOut[g];
+    if (readsAcc && ((outSize[g] && !o) || (reinterpret_cast<uintptr_t>(o) & (elemBytes - 1u)))) return DGB_ERR_INVALID_ARG;
     // block cap >= 1: every group's headers are visited, so its status is reported
     const uint32_t blocks = std::max(1u, divUp(outSize[g], kBlockBytes));
     totalChunks += divUp(blocks, 8u);
     for (uint32_t j = 0; j < width; ++j) {
       const void* a = in[(size_t)g * width + j];
       if (!a || (reinterpret_cast<uintptr_t>(a) & 15u)) return DGB_ERR_INVALID_ARG;
-      desc[(size_t)g * width + j] = MemberDesc{a, out[g], outSize[g], blocks};
+      desc[(size_t)g * width + j] = MemberDesc{a, o, outSize[g], blocks};
     }
   }
   uint8_t* base = static_cast<uint8_t*>(temp);
@@ -1823,7 +1935,16 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
     const int rc = uploadTable(sc.members, desc, sizeof(MemberDesc) * n, stream);
     if (rc != DGB_OK) return rc;
   }
+  // the narrowing sums' table of 16-bit outputs: G pointers in the scratch the checksum pass of a plain decode uses,
+  // 3 * 4 * n >= 8 * G bytes that no decode-and-sum touches otherwise
   im.scale = scale ? *scale : 1.0f;  // a kernel parameter: a captured launch keeps the value it was captured with
+  if (narrowOut) {
+    void** t = reinterpret_cast<void**>(base + dp.checksum);
+    const int rc = uploadTable(t, narrowOut, sizeof(void*) * (size_t)groups, stream);
+    if (rc != DGB_OK) return rc;
+    return launchDecodeReduceNarrow(kind, pb, scale != nullptr, opt, sc.members, sc.next, im, groups, width,
+                                    totalChunks, accumulate, outSuccess_dev, stream, scaleDev, foundInf, t);
+  }
   return withKind(kind, [&](auto K) { return withPb(pb, [&](auto P) {
     constexpr int KIND = decltype(K)::value;
     constexpr int DK = denseKind(KIND);
@@ -2024,5 +2145,7 @@ int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool 
   DGB_CUDA_TRY(cudaGetLastError());
   return DGB_OK;
 }
+
+#endif  // DGB_DECODE_NARROW_TU
 
 }  // namespace dgb

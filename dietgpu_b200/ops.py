@@ -21,6 +21,7 @@ dtype, and archives and output rows must be 16 B aligned.
 """
 from __future__ import annotations
 
+import ctypes as C
 import numbers
 from typing import List, Optional, Sequence, Tuple
 
@@ -436,7 +437,8 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                            prob_bits: int = K_DEFAULT_PRECISION,
                            archive_dtype: Optional[torch.dtype] = None, sparse: bool = False,
                            scale: Optional[float] = None, scale_tensor: Optional[torch.Tensor] = None,
-                           found_inf: Optional[torch.Tensor] = None) -> int:
+                           found_inf: Optional[torch.Tensor] = None, reduce_dtype: Optional[torch.dtype] = None,
+                           acc: Optional[Sequence[torch.Tensor]] = None) -> int:
     """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
@@ -468,7 +470,19 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     found_inf (with scale_tensor only): a one-element float32 CUDA tensor on the same device, set to 1.0 when any
     element this call writes ends up inf or NaN, and never cleared (torch.amp's found_inf); with
     scale_tensor=torch.ones(1) it flags the unscaled sum.  Elements of a group left untouched never count.
-    These keywords raise ValueError before any archive is read."""
+    These keywords raise ValueError before any archive is read.
+
+    reduce_dtype=torch.float32 with float16 / bfloat16 outputs of archive_dtype (dense, or sparse=True)
+    (dgb_float_decompress_reduce_narrow): the sum is taken in float32 and rounded once to the outputs' dtype, so
+    ts_out[g] becomes S.to(dtype) with S = (acc[g] if accumulate else term(x(g, 0))) + term(x(g, 1)) + ... in
+    float32, term being the widening sum's term (x.float(), or (x.float() * s32) with scale / scale_tensor): bit for
+    bit the widening call into float32 outputs followed by torch's .to(dtype).  found_inf sees the rounded 16-bit
+    results, so a float32 sum that rounds to an fp16 infinity counts.  acc: G contiguous float32 CUDA tensors on the
+    outputs' device with ts_out[g].numel() elements each, holding the running sums accumulate starts from and taking
+    the intermediate sums of the call (their contents afterwards are unspecified); ts_out[g] is only written.  acc
+    is required with accumulate=True; otherwise None takes a stream-ordered temporary when W > 1.  reduce_dtype
+    None or the outputs' dtype is the call described above; any other reduce_dtype, an acc without this path, or an
+    acc of the wrong dtype, size or device raises ValueError before any archive is read."""
     scale32 = _scale32(scale)
     _check_dev_scale(scale32, scale_tensor, found_inf, ts_out[0].device if len(ts_out) else None)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
@@ -482,7 +496,30 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     if archive_dtype != dtype and not (dtype == torch.float32 and archive_dtype in (torch.float16, torch.bfloat16)):
         raise ValueError(f"decompress_data_reduce sums {archive_dtype} archives into {archive_dtype} outputs, or "
                          f"float16 / bfloat16 archives into float32 outputs; not into {dtype}")
+    narrow = reduce_dtype is not None and reduce_dtype != dtype
+    if narrow and not (reduce_dtype == torch.float32 and dtype in (torch.float16, torch.bfloat16)
+                       and archive_dtype == dtype):
+        raise ValueError(f"decompress_data_reduce: reduce_dtype is None, the outputs' dtype, or float32 for float16 / "
+                         f"bfloat16 outputs of the archives' dtype; not {reduce_dtype} for {archive_dtype} archives "
+                         f"into {dtype} outputs")
     dev = ts_out[0].device
+    if acc is not None:
+        if not narrow:
+            raise ValueError("decompress_data_reduce: acc needs reduce_dtype=torch.float32 with float16 / bfloat16 "
+                             "outputs")
+        if len(acc) != len(ts_out):
+            raise ValueError(f"decompress_data_reduce: acc needs one tensor per group ({len(ts_out)}), not {len(acc)}")
+        for a, to in zip(acc, ts_out):
+            if not isinstance(a, torch.Tensor) or a.dtype != torch.float32 or not a.is_contiguous():
+                raise ValueError("decompress_data_reduce: acc holds contiguous float32 tensors")
+            if not a.is_cuda or a.device != dev:
+                raise ValueError(f"decompress_data_reduce: acc must be on the outputs' device {dev}, not {a.device}")
+            if a.numel() != to.numel():
+                raise ValueError(f"decompress_data_reduce: acc[g] needs ts_out[g].numel() = {to.numel()} elements, "
+                                 f"not {a.numel()}")
+    elif narrow and accumulate:
+        raise ValueError("decompress_data_reduce: accumulate=True with reduce_dtype=torch.float32 needs acc (the "
+                         "float32 running sums)")
     ins = []
     for group, to in zip(ts_in, ts_out):
         _check(len(group) == width, "every group needs the same number of archives")
@@ -497,6 +534,26 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     st_ptr, _ = _validate_status(out_status, None, n, dev)
     ft, out_ft = (_SPARSE_TYPES if sparse else _REDUCE_TYPES)[archive_dtype], _REDUCE_TYPES[dtype]
     L = capi.lib()
+    if narrow:
+        if acc is None and width > 1:
+            flat = torch.empty(sum(t.numel() for t in ts_out), dtype=torch.float32, device=dev)
+            acc, o = [], 0
+            for to in ts_out:
+                acc.append(flat[o:o + to.numel()])
+                o += to.numel()
+        s = None if scale32 is None else C.c_float(float(scale32))
+        with torch.cuda.device(dev):
+            need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
+            tmp = _Temp(temp_mem, need, dev)
+            rc = L.dgb_float_decompress_reduce_narrow(
+                tmp.ptr, tmp.bytes, ft, prob_bits, g, width, capi.ptr_array([t.data_ptr() for t in ins]),
+                None if acc is None else capi.ptr_array([a.data_ptr() for a in acc]),
+                capi.ptr_array([t.data_ptr() for t in ts_out]), capi.u32_array([t.numel() for t in ts_out]),
+                int(bool(accumulate)), None if s is None else C.addressof(s),
+                None if scale_tensor is None else scale_tensor.data_ptr(),
+                None if found_inf is None else found_inf.data_ptr(), st_ptr, _stream())
+        capi.check(rc, "decompress_data_reduce")
+        return tmp.need
     entry = L.dgb_float_decompress_reduce_sparse if sparse else L.dgb_float_decompress_reduce_to
     extra = ()
     if scale32 is not None:

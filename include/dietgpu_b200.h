@@ -312,6 +312,30 @@ int dgb_float_decompress_reduce_scaled_dev(void* temp_dev, size_t temp_bytes, in
                                            int accumulate, const float* scale_dev, float* found_inf_dev,
                                            uint8_t* out_success_dev, void* stream);
 
+/* Narrowing decode-and-sum (new; no reference counterpart): fp16 / bf16 archives summed in fp32 and rounded once to
+ * the archives' 16-bit type, so a 16-bit result carries one rounding instead of one per add and needs no fp32
+ * output.  float_type: DGB_FLOAT16, DGB_BFLOAT16, DGB_FLOAT16_SPARSE or DGB_BFLOAT16_SPARSE; out[g] (2 B aligned)
+ * has that dense type, acc[g] (4 B aligned) is an fp32 accumulator of out_size[g] elements.
+ * out[g] = round(S) with S = (accumulate ? acc[g] : term(x(g,0))) + term(x(g,1)) + ... + term(x(g,W-1)) taken in
+ * fp32 in archive order, each + one fp32 round-to-nearest-even add, and round one round-to-nearest-even conversion
+ * to the 16-bit type: bit-identical to dgb_float_decompress_reduce_to (or _scaled / _scaled_dev) into fp32 outputs
+ * followed by torch's .to(dtype).  term is the widening entries' term: fp32(x), or fp32(x) * s with the host
+ * `scale` or the device scale *scale_dev (at most one of them).  The running sums of every archive but the last go
+ * through acc[g], which ends up unspecified; out[g] is only written, never read.  acc (the array, and each acc[g] with
+ * out_size[g] > 0) may be NULL when the call reads no accumulator: W = 1 without accumulate.  found_inf_dev (with
+ * scale_dev only; may be NULL): set to 1.0f when a 16-bit word this call stores is inf or NaN, so an fp32 sum that
+ * rounds to an fp16 infinity counts.  Everything else is as in dgb_float_decompress_reduce_scaled_dev: the validity
+ * rule, statuses, groups with an invalid archive left unwritten (acc[g] and out[g] both), num_groups = 0 returning
+ * DGB_OK, no synchronisation, graph capture (a replay reads *scale_dev's value then) and the scratch size
+ * dgb_float_decompress_temp_bytes(float_type, G * W, 0).  DGB_ERR_INVALID_ARG before any CUDA call: any other
+ * float_type, scale with scale_dev, found_inf_dev without scale_dev, a misaligned scale_dev or found_inf_dev, a NULL
+ * or misaligned acc[g] or out[g] where it is needed, and every argument the other decode-and-sum entries refuse. */
+int dgb_float_decompress_reduce_narrow(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
+                                       uint32_t num_groups, uint32_t archives_per_group, const void* const* in,
+                                       float* const* acc, void* const* out, const uint32_t* out_size,
+                                       int accumulate, const float* scale, const float* scale_dev,
+                                       float* found_inf_dev, uint8_t* out_success_dev, void* stream);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

@@ -17,6 +17,8 @@ the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_AR
 --scale: the scaled decode-and-sum against the unscaled one and against scaling the inputs with torch (bench_scale).
 --scale-tensor: the device-scale decode-and-sum with its non-finite flag against the host-scaled one and against
 an unscaled sum followed by torch.amp's unscale-and-check (bench_scale_tensor).
+--out-dtype: the narrowing decode-and-sum (fp32 sums rounded once to the 16-bit archive dtype) against the widening
+one followed by torch's .to() and against the same-type 16-bit sum (bench_out_dtype).
 """
 import argparse
 import json
@@ -369,6 +371,67 @@ def bench_scale_tensor(dtype, groups, width, n, iters, out_dtype, sparse):
     return r
 
 
+OUT_DTYPE_SHAPES = [  # (dtype, groups, width, words, sparse ReLU data)
+    (torch.bfloat16, 8, 8, 2 << 20, False),
+    (torch.float16, 64, 2, 512 << 10, False),
+    (torch.bfloat16, 8, 8, 2 << 20, True),
+]
+
+
+def bench_out_dtype(dtype, groups, width, n, iters, sparse):
+    """--out-dtype, on the same archives, alternated: (1) the narrowing decode-and-sum
+    (reduce_dtype=torch.float32, 16-bit outputs, a caller-owned fp32 accumulator); (2) the widening one into fp32
+    outputs followed by torch's .to(dtype) (bit-identical to (1), checked); (3) the same-type 16-bit sum.  Reported:
+    call time of all three and of (2)'s sum alone ("2_sum"); kernel time (timing=1) of (1), (2)'s sum and (3); the
+    modelled HBM bytes per output element of (1) and (2) (the archives are read in both)."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [sparse_data(dtype, n, "relu" if sparse else "0", g) for _ in range(groups * width)]
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    comp, sizes, _ = ops.compress_data(True, xs, sparse=sparse)
+    hs = sizes.cpu().tolist()
+    gi = [[comp[k * width + j, :hs[k * width + j]] for j in range(width)] for k in range(groups)]
+    del xs
+    outs = {k: [torch.empty(n, dtype=dtype, device="cuda") for _ in range(groups)] for k in ("1", "2", "3")}
+    acc = [torch.empty(n, dtype=torch.float32, device="cuda") for _ in range(groups)]
+    wide = [torch.empty(n, dtype=torch.float32, device="cuda") for _ in range(groups)]
+
+    def one():
+        ops.decompress_data_reduce(gi, outs["1"], False, temp, archive_dtype=dtype, sparse=sparse,
+                                   reduce_dtype=torch.float32, acc=acc)
+
+    def two_sum():
+        ops.decompress_data_reduce(gi, wide, False, temp, archive_dtype=dtype, sparse=sparse)
+
+    def two():
+        two_sum()
+        for w, o in zip(wide, outs["2"]):
+            o.copy_(w)
+
+    def three():
+        ops.decompress_data_reduce(gi, outs["3"], False, temp, archive_dtype=dtype, sparse=sparse)
+
+    fns = {"1": one, "2": two, "2_sum": two_sum, "3": three}
+    for f in fns.values():  # warm-up
+        f()
+    torch.cuda.synchronize()
+    same = all(bool(((a.view(torch.int16) == b.view(torch.int16)) | (a.isnan() & b.isnan())).all())
+               for a, b in zip(outs["1"], outs["2"]))
+    t = {k: [] for k in fns}
+    for _ in range(3):  # alternate
+        for k, f in fns.items():
+            t[k].append(timed(f, iters))
+    kt = {"1": kernel_us(one, iters), "2_sum": kernel_us(two_sum, iters), "3": kernel_us(three, iters)}
+    # the bytes per output element that differ (the archives and the fp32 running sums of every archive but the
+    # last are the same in both): (1) stores 2 B; (2) stores 4 B, then its cast reads 4 B and writes 2 B
+    r = {"shape": f"{'sparse relu ' if sparse else ''}{str(dtype).split('.')[-1]} {groups}x{width}x{n}",
+         "bit_equal_1_2": same, "call_us": {k: min(v) for k, v in t.items()},
+         "call_us_max": {k: max(v) for k, v in t.items()}, "kernel_us": kt,
+         "model_final_bytes_per_elem": {"1": 2, "2": 10}}
+    r["call_1_over_2"] = r["call_us"]["1"] / r["call_us"]["2"]
+    r["kernel_1_over_2_sum"] = kt["1"] / kt["2_sum"]
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -380,10 +443,18 @@ def main():
     ap.add_argument("--scale-tensor", action="store_true",
                     help="device-scale sums with the non-finite flag against host-scaled sums and torch.amp's "
                          "unscale (bench_scale_tensor)")
+    ap.add_argument("--out-dtype", action="store_true",
+                    help="narrowing sums against widening sums + .to() and same-type sums (bench_out_dtype)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    if args.scale_tensor:
+    if args.out_dtype:
+        for shape in OUT_DTYPE_SHAPES:
+            r = bench_out_dtype(*shape[:4], args.iters, shape[4])
+            info["results"].append(r)
+            print(json.dumps(r), flush=True)
+        shapes = []
+    elif args.scale_tensor:
         for shape in SCALE_SHAPES:
             r = bench_scale_tensor(*shape[:4], args.iters, *shape[4:])
             info["results"].append(r)
