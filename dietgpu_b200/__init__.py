@@ -26,11 +26,12 @@ from .ops import (  # noqa: F401
     max_any_compressed_size,
     max_float_compressed_output_size,
     max_float_compressed_size,
+    sq_norm,
 )
 
 __all__ = [
     "capi", "HostCodec", "PeerWorkspace", "all_gather_compressed", "all_to_all_compressed", "exchange_archives",
     "reduce_scatter_compressed", "all_reduce_compressed", "decompress_data_reduce", "compress_data", "compress_data_simple", "compress_data_split_size", "decompress_data",
     "decompress_data_simple", "decompress_data_split_size", "max_any_compressed_output_size",
-    "max_any_compressed_size", "max_float_compressed_output_size", "max_float_compressed_size",
+    "max_any_compressed_size", "max_float_compressed_output_size", "max_float_compressed_size", "sq_norm",
 ]

@@ -29,7 +29,10 @@ SYMBOLS = [
     "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_split_size",
     "dgb_float_decompress_pointer", "dgb_float_decompress_split_size", "dgb_float_decompress_reduce",
     "dgb_float_decompress_reduce_to", "dgb_float_decompress_reduce_sparse", "dgb_float_decompress_reduce_scaled",
-    "dgb_float_decompress_reduce_scaled_dev", "dgb_float_decompress_reduce_narrow", "dgb_float_get_compressed_info",
+    "dgb_float_decompress_reduce_scaled_dev", "dgb_float_decompress_reduce_narrow",
+    "dgb_float_decompress_reduce_scaled_dev_norm", "dgb_float_decompress_reduce_narrow_norm",
+    "dgb_float_decompress_reduce_norm_temp_bytes", "dgb_float_sq_norm", "dgb_float_sq_norm_temp_bytes",
+    "dgb_float_get_compressed_info",
     "dgb_copy_async", "dgb_copy_rows_async", "dgb_archives_pull",
     "dgb_set_option", "dgb_get_option", "dgb_set_thread_option", "dgb_clear_thread_options", "dgb_kernel_times",
 ]
@@ -118,6 +121,18 @@ def lib():
                                                          vp]
     L.dgb_float_decompress_reduce_narrow.restype = i32
     L.dgb_float_decompress_reduce_narrow.argtypes = [vp, sz, i32, i32, u32, u32, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp]
+    L.dgb_float_decompress_reduce_scaled_dev_norm.restype = i32
+    L.dgb_float_decompress_reduce_scaled_dev_norm.argtypes = [vp, sz, i32, i32, i32, u32, u32, vp, vp, vp, i32, vp, vp,
+                                                              vp, vp, vp]
+    L.dgb_float_decompress_reduce_narrow_norm.restype = i32
+    L.dgb_float_decompress_reduce_narrow_norm.argtypes = [vp, sz, i32, i32, u32, u32, vp, vp, vp, vp, i32, vp, vp, vp,
+                                                          vp, vp]
+    L.dgb_float_decompress_reduce_norm_temp_bytes.restype = sz
+    L.dgb_float_decompress_reduce_norm_temp_bytes.argtypes = [i32, u32, u32, vp]
+    L.dgb_float_sq_norm.restype = i32
+    L.dgb_float_sq_norm.argtypes = [vp, sz, i32, u32, vp, vp, vp, vp]
+    L.dgb_float_sq_norm_temp_bytes.restype = sz
+    L.dgb_float_sq_norm_temp_bytes.argtypes = [u32, vp]
     L.dgb_float_get_compressed_info.restype = i32
     L.dgb_float_get_compressed_info.argtypes = [vp, sz, vp, i32, u32, vp, vp, vp, vp]
     L.dgb_set_option.restype = i32

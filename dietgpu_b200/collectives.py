@@ -593,6 +593,30 @@ def _check_scale(what: str, scale, average: bool, scale_tensor=None, found_inf=N
     return s32
 
 
+def _check_sq_norm(what: str, sq_norm, scale_tensor, dev) -> None:
+    """sq_norm: None, or a one-element float64 CUDA tensor on dev, with scale_tensor (as found_inf needs it)."""
+    if sq_norm is None:
+        return
+    if scale_tensor is None:
+        raise ValueError(f"{what}: sq_norm needs scale_tensor (torch.ones(1) for the unscaled sum)")
+    ops._check_sq_norm(f"{what}: sq_norm", sq_norm, 1, dev)
+
+
+def _fold(out: torch.Tensor, values: torch.Tensor) -> None:
+    """out (one element) = ((values[0] + values[1]) + values[2]) + ..., fp64 adds on the device in index order
+    (torch's sum() does not specify its order)."""
+    out.copy_(values[0:1])
+    for i in range(1, values.numel()):
+        out.add_(values[i:i + 1])
+
+
+def _shard_sq_norm(out: Optional[torch.Tensor], res: torch.Tensor, bounds: List[int]) -> None:
+    """out = the member-order fold of ops.sq_norm of res's pieces [bounds[i], bounds[i + 1]): what the decode-and-sum
+    gives when it writes those pieces, for the shards torch finishes."""
+    if out is not None:
+        _fold(out, ops.sq_norm([res[bounds[i]:bounds[i + 1]] for i in range(len(bounds) - 1)]))
+
+
 def _term(x: torch.Tensor, acc_dtype: torch.dtype, s32) -> torch.Tensor:
     """What the scaled decode-and-sum adds for the words x: (x.float() * s32).to(acc_dtype), one float32 multiply
     by a float32 tensor and one rounding; x.to(acc_dtype) without a scale.  s32: a float32 number, or a device
@@ -625,7 +649,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               scale: Optional[float] = None, average: bool = False,
                               scale_tensor: Optional[torch.Tensor] = None,
                               found_inf: Optional[torch.Tensor] = None,
-                              out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                              out_dtype: Optional[torch.dtype] = None,
+                              sq_norm: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -671,8 +696,16 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     dtype: the sum is still taken in float32 and rounded once per element inside the decode-and-sum kernel, so the
     result is this call without out_dtype followed by .to(out_dtype), bit for bit on every rank, without a float32
     result (found_inf then sees the rounded elements).  Any other value raises ValueError before any
-    communication."""
+    communication.
+
+    sq_norm (with scale_tensor; a one-element float64 CUDA tensor on t's device) is overwritten with the squared norm
+    of the returned shard, for gradient clipping: the fp64 fold, in member order, of the squared norms
+    (ops.sq_norm's definition) of the shard's `members` pieces.  The decode-and-sum that writes the final values takes
+    them in the same kernel (decompress_data_reduce(sq_norm=)); the last rank and a world of one, which finish the
+    shard with torch, apply ops.sq_norm to the same pieces, so the value is the same function of the shard on every
+    path.  Misuse raises ValueError before any communication."""
     s32 = _check_scale("reduce_scatter_compressed", scale, average, scale_tensor, found_inf, t.device)
+    _check_sq_norm("reduce_scatter_compressed", sq_norm, scale_tensor, t.device)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
     narrow_dtype = _check_out_dtype("reduce_scatter_compressed", out_dtype, t.dtype, reduce_dtype, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
@@ -687,13 +720,16 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
-    if world == 1 or n == 0:
-        if res_dtype == acc_dtype:
-            return _local_sum(flat[: n // world].to(arch_dtype), acc_dtype, sd, found_inf)
-        return _local_sum(_term(flat[: n // world].to(arch_dtype), acc_dtype, sd), res_dtype, None, found_inf)
-    rank, dev = dist.get_rank(group), t.device
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
+    if world == 1 or n == 0:
+        if res_dtype == acc_dtype:
+            res = _local_sum(flat[:shard].to(arch_dtype), acc_dtype, sd, found_inf)
+        else:
+            res = _local_sum(_term(flat[:shard].to(arch_dtype), acc_dtype, sd), res_dtype, None, found_inf)
+        _shard_sq_norm(sq_norm, res, bounds)
+        return res
+    rank, dev = dist.get_rank(group), t.device
     m = len(bounds) - 1
     dests = [d for d in range(world) if d != rank]
     comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
@@ -724,18 +760,22 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
         statuses.append(st)
         out.add_(own)
     if rank + 1 < world:
-        # the last call writes the final values: the kernel checks them
+        # the last call writes the final values: the kernel checks them, and takes their squared norms
         st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
+        pieces_sq = None if sq_norm is None else torch.zeros(m, dtype=torch.float64, device=dev)
         ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)],
                                    [res[bounds[i]:bounds[i + 1]] for i in range(m)], True, temp_mem, st,
                                    archive_dtype=arch_dtype, sparse=sparse, scale=s32, scale_tensor=scale_tensor,
-                                   found_inf=found_inf, **narrow)
+                                   found_inf=found_inf, sq_norm=pieces_sq, **narrow)
         statuses.append(st)
+        if sq_norm is not None:
+            _fold(sq_norm, pieces_sq)
     else:
         # the last rank ends on torch's add of its own chunk (and torch's rounding of it when narrowing)
         if res is not out:
             res.copy_(out)
         _flag_non_finite(found_inf, res)
+        _shard_sq_norm(sq_norm, res, bounds)
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
     return res
@@ -746,7 +786,8 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
                           sparse: bool = False, scale: Optional[float] = None,
                           average: bool = False, scale_tensor: Optional[torch.Tensor] = None,
                           found_inf: Optional[torch.Tensor] = None,
-                          out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+                          out_dtype: Optional[torch.dtype] = None,
+                          sq_norm: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Elementwise sum over ranks of t (contiguous CUDA fp16 / bf16 / fp32, any numel, same shape on every rank),
     returned on every rank: reduce_scatter_compressed, then all_gather_compressed of the summed shard.  When
     t.numel() is not world x a multiple of 8, t is zero-padded to world x roundUp(ceil(n / world), 8) elements
@@ -762,8 +803,14 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     out_dtype is reduce_scatter_compressed's: t.dtype for a float16 / bfloat16 t summed with
     reduce_dtype=torch.float32 makes the shards come back rounded once to t.dtype, the second phase all-gathers
     16-bit archives instead of float32 ones, and the result is this call without out_dtype followed by
-    .to(out_dtype), bit for bit on every rank.  Any other out_dtype raises ValueError before any communication."""
+    .to(out_dtype), bit for bit on every rank.  Any other out_dtype raises ValueError before any communication.
+
+    sq_norm (with scale_tensor; a one-element float64 CUDA tensor on t's device) is overwritten with the squared norm
+    of the whole result, identical on every rank: the rank-order fp64 fold of the shards' reduce_scatter_compressed
+    sq_norm values, exchanged with one all-gather (padding zeros add +0).  A world of one, or an empty t, takes
+    reduce_scatter_compressed's value for t.  Misuse raises ValueError before any communication."""
     s32 = _check_scale("all_reduce_compressed", scale, average, scale_tensor, found_inf, t.device)
+    _check_sq_norm("all_reduce_compressed", sq_norm, scale_tensor, t.device)
     _check_sparse_wire(t.dtype, "all_reduce_compressed", sparse)
     narrow_dtype = _check_out_dtype("all_reduce_compressed", out_dtype, t.dtype, reduce_dtype, None)
     acc_dtype = _check_reducible(t, "all_reduce_compressed", reduce_dtype)
@@ -776,14 +823,26 @@ def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_me
     if world == 1 or n == 0:
         sd = s32 if scale_tensor is None else scale_tensor
         if res_dtype == acc_dtype:
-            return _local_sum(t, acc_dtype, sd, found_inf)
-        return _local_sum(_term(t, acc_dtype, sd), res_dtype, None, found_inf)
+            res = _local_sum(t, acc_dtype, sd, found_inf)
+        else:
+            res = _local_sum(_term(t, acc_dtype, sd), res_dtype, None, found_inf)
+        _shard_sq_norm(sq_norm, res.reshape(-1), _split(n, max(1, int(members)), 8))
+        return res
     per = _round_up(-(-n // world), 8)
     src = flat if world * per == n else torch.cat([flat, flat.new_zeros(world * per - n)])
     # (a padding zero's term is non-finite only for an inf or NaN scale, which makes every element's term so too)
     shard_inf = None if found_inf is None else torch.zeros(1, dtype=torch.float32, device=t.device)
+    shard_sq = None if sq_norm is None else torch.zeros(1, dtype=torch.float64, device=t.device)
     shard = reduce_scatter_compressed(src, group, members, temp_mem, check, reduce_dtype=acc_dtype, sparse=sparse,
-                                      scale=s32, scale_tensor=scale_tensor, found_inf=shard_inf, out_dtype=res_dtype)
+                                      scale=s32, scale_tensor=scale_tensor, found_inf=shard_inf, out_dtype=res_dtype,
+                                      sq_norm=shard_sq)
+    if sq_norm is not None:
+        # every rank folds the same gathered values in rank order (an all-reduce's order is not defined)
+        on_device = _device_collectives(group)
+        mine = shard_sq if on_device else shard_sq.cpu()
+        every = [torch.empty_like(mine) for _ in range(world)]
+        dist.all_gather(every, mine, group=group)
+        _fold(sq_norm, torch.cat(every).to(t.device))
     if found_inf is not None:
         on_device = _device_collectives(group)
         flag = shard_inf if on_device else shard_inf.cpu()

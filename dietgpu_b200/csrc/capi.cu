@@ -591,6 +591,55 @@ int dgb_float_decompress_reduce_narrow(void* temp, size_t tempBytes, int ft, int
                       scale, scale_dev, foundInf_dev, (cudaStream_t)stream, out);
 }
 
+int dgb_float_decompress_reduce_scaled_dev_norm(void* temp, size_t tempBytes, int ft, int outFt, int pb,
+                                                uint32_t numGroups, uint32_t archivesPerGroup, const void* const* in,
+                                                void* const* out, const uint32_t* outSize, int accumulate,
+                                                const float* scale_dev, float* foundInf_dev, double* sqNorm_dev,
+                                                uint8_t* outSuccess_dev, void* stream) {
+  // dgb_float_decompress_reduce_scaled_dev, and the squared norm of each group's stored words into sqNorm_dev[g]
+  if (!scale_dev || (reinterpret_cast<uintptr_t>(scale_dev) & 3u)) return DGB_ERR_INVALID_ARG;
+  if (reinterpret_cast<uintptr_t>(foundInf_dev) & 3u) return DGB_ERR_INVALID_ARG;
+  if (!sqNorm_dev || (reinterpret_cast<uintptr_t>(sqNorm_dev) & 7u)) return DGB_ERR_INVALID_ARG;
+  return decodeReduce(ft, outFt, temp, tempBytes, pb, numGroups, archivesPerGroup, in, out, outSize, accumulate != 0,
+                      outSuccess_dev, isSparseKind(ft), nullptr, scale_dev, foundInf_dev, (cudaStream_t)stream,
+                      nullptr, sqNorm_dev);
+}
+
+int dgb_float_decompress_reduce_narrow_norm(void* temp, size_t tempBytes, int ft, int pb, uint32_t numGroups,
+                                            uint32_t archivesPerGroup, const void* const* in, float* const* acc,
+                                            void* const* out, const uint32_t* outSize, int accumulate,
+                                            const float* scale_dev, float* foundInf_dev, double* sqNorm_dev,
+                                            uint8_t* outSuccess_dev, void* stream) {
+  // dgb_float_decompress_reduce_narrow with the device scale, and the squared norm of each group's 16-bit results
+  if (ft != kKindF16 && ft != kKindBF16 && ft != kKindF16S && ft != kKindBF16S) return DGB_ERR_INVALID_ARG;
+  if (!scale_dev || (reinterpret_cast<uintptr_t>(scale_dev) & 3u)) return DGB_ERR_INVALID_ARG;
+  if (reinterpret_cast<uintptr_t>(foundInf_dev) & 3u) return DGB_ERR_INVALID_ARG;
+  if (!sqNorm_dev || (reinterpret_cast<uintptr_t>(sqNorm_dev) & 7u)) return DGB_ERR_INVALID_ARG;
+  if (numGroups && !out) return DGB_ERR_INVALID_ARG;
+  return decodeReduce(ft, kKindF32, temp, tempBytes, pb, numGroups, archivesPerGroup, in,
+                      reinterpret_cast<void* const*>(acc), outSize, accumulate != 0, outSuccess_dev, isSparseKind(ft),
+                      nullptr, scale_dev, foundInf_dev, (cudaStream_t)stream, out, sqNorm_dev);
+}
+
+size_t dgb_float_decompress_reduce_norm_temp_bytes(int ft, uint32_t numGroups, uint32_t archivesPerGroup,
+                                                   const uint32_t* outSize) {
+  const uint64_t n = (uint64_t)numGroups * archivesPerGroup;
+  if (!validFloatType(ft) || n > 0xffffffffull || (numGroups && !outSize)) return 0;
+  return decodeTempBytes(ft, (uint32_t)n) + sqNormScratchBytes(numGroups, sqNormBlocks(numGroups, outSize));
+}
+
+size_t dgb_float_sq_norm_temp_bytes(uint32_t numGroups, const uint32_t* size) {
+  if (numGroups && !size) return 0;
+  return floatSqNormTempBytes(numGroups, size);
+}
+
+int dgb_float_sq_norm(void* temp, size_t tempBytes, int ft, uint32_t numGroups, const void* const* in,
+                      const uint32_t* size, double* sqNorm_dev, void* stream) {
+  if (ft != kKindF16 && ft != kKindBF16 && ft != kKindF32) return DGB_ERR_INVALID_ARG;
+  if (!sqNorm_dev || (reinterpret_cast<uintptr_t>(sqNorm_dev) & 7u)) return DGB_ERR_INVALID_ARG;
+  return floatSqNorm(ft, temp, tempBytes, numGroups, in, size, sqNorm_dev, (cudaStream_t)stream);
+}
+
 // ---- info ------------------------------------------------------------------
 
 int dgb_ans_get_compressed_info(void* temp, size_t tempBytes, const void* const* in,

@@ -209,7 +209,7 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
-                 cudaStream_t stream, void* const* narrowOut = nullptr);
+                 cudaStream_t stream, void* const* narrowOut = nullptr, double* sqNorm = nullptr);
 // the narrowing sums' kernels (decode_narrow.cu): decodeReduce's launches of kind | kWidenF32 | kNarrowOut, scaled
 // (host scale) or with scaleDev / foundInf, reading the groups' 16-bit outputs from the device table narrowTable
 int launchDecodeReduceNarrow(int kind, int pb, bool scaled, const Options& opt, MemberDesc* members, uint32_t* next,
@@ -231,6 +231,36 @@ inline uint32_t wordBytes(int kind) {  // the narrowing kinds: their float32 inp
                           : (kind == kKindF32 || kind == kKindF32S || isNarrowKind(kind) ? 4u : (kind == kKindBytes ? 1u : 2u));
 }
 inline size_t alignUp256(size_t v) { return (v + 255) & ~size_t(255); }
+
+// Squared norms (decode_norm.cu): the fp64 squared norm of each of G groups of float words, in the fixed order of
+// include/dietgpu_b200.h (lane, warp, group).  One fp64 partial per 4096-word block goes to scratch, and a fold
+// kernel (one CTA per group) writes sq_norm[g].
+struct SqNormScratch {
+  uint32_t* off;  // [G + 1] index of group g's first partial; off[G] = every group's blocks
+  uint32_t* size; // [G] the groups' word counts (right after off)
+  uint32_t* ok;   // [G] the decode-and-sum's verdict on group g (1: every archive valid); unused by floatSqNorm
+  double* part;   // [off[G]] one partial per block
+};
+inline uint64_t sqNormBlocks(uint32_t groups, const uint32_t* size) {
+  uint64_t b = 0;
+  for (uint32_t g = 0; g < groups; ++g) b += (size[g] + 4095u) / 4096u;
+  return b;
+}
+inline size_t sqNormScratchBytes(uint32_t groups, uint64_t blocks) {
+  return alignUp256(8 * (size_t)groups + 8) + alignUp256(4 * (size_t)groups) + alignUp256(8 * blocks);
+}
+// lays SqNormScratch out at `base` (256 B aligned) and uploads the offsets and sizes of size[0 .. G-1]
+int sqNormPrepare(uint8_t* base, uint32_t groups, const uint32_t* size, SqNormScratch* out, cudaStream_t stream);
+// decodeReduce's launches of the device-scale kinds | kSqNorm (narrowing ones when narrowTable is set), then the
+// fold into sqNorm[g] for the groups the reduce kernels found valid
+int launchDecodeReduceNorm(int kind, int pb, bool widen, const Options& opt, MemberDesc* members, uint32_t* next,
+                           const InlineMembers& im, uint32_t groups, uint32_t width, uint64_t totalChunks,
+                           bool accumulate, uint8_t* outSuccess, cudaStream_t stream, const float* scaleDev,
+                           float* foundInf, void* const* narrowTable, const SqNormScratch& norm, double* sqNorm);
+// dgb_float_sq_norm: dense fp16 / bf16 / fp32 words
+size_t floatSqNormTempBytes(uint32_t groups, const uint32_t* size);
+int floatSqNorm(int kind, void* temp, size_t tempBytes, uint32_t groups, const void* const* in, const uint32_t* size,
+                double* sqNorm, cudaStream_t stream);
 int smCount();  // SMs of the current device, cached per device
 
 // Resident CTAs per SM of `kernel` with `threads` threads and `smemBytes` of dynamic shared memory, into
@@ -247,6 +277,7 @@ struct HostStage {
   std::vector<uint8_t> encodeUpload;    // encoder member table + work index, uploaded together
   std::vector<MemberDesc> decodeTable;  // decoder member table
   std::vector<uint32_t> checksum;       // decoder checksum pass: computed, stored and decoded size per member
+  std::vector<uint32_t> sqNormOff;      // squared norms: first block partial of each group, and the total
 };
 HostStage& hostStage();
 

@@ -155,16 +155,19 @@ constexpr uint32_t kRingSlots = 3;              // groups resident per warp: cur
 // | kDevScale (kernels only, with kScaled) reads that scale from device memory when the kernel runs;
 // | kCheckFinite (writers only) also reports whether a word it stores is inf or NaN;
 // | kNarrowOut (with kWidenF32) sums in fp32 from an fp32 accumulator and stores the sum rounded once to the
-// archive's 16-bit type into a second output (the narrowing sums: kernels and the writer of a call's last archive)
+// archive's 16-bit type into a second output (the narrowing sums: kernels and the writer of a call's last archive);
+// | kSqNorm (device-scale kinds only) also takes the squared norm of the words the call stores (kernels, and with
+// kCheckFinite the writer of a call's last archive)
 constexpr int kAddWriter = 0x10;
 constexpr int kWidenF32 = 0x20;
 constexpr int kScaled = 0x80;
 constexpr int kDevScale = 0x100;
 constexpr int kCheckFinite = 0x200;
 constexpr int kNarrowOut = 0x400;
+constexpr int kSqNorm = 0x800;
 // the archive kind of a decode-and-sum kernel or writer kind
 __host__ __device__ constexpr int reduceArchiveKind(int k) {
-  return k & ~(kAddWriter | kWidenF32 | kScaled | kDevScale | kCheckFinite | kNarrowOut);
+  return k & ~(kAddWriter | kWidenF32 | kScaled | kDevScale | kCheckFinite | kNarrowOut | kSqNorm);
 }
 
 template <int KIND>
@@ -1082,7 +1085,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
 
 // XOR checksum of decoded outputs (ans/GpuChecksum.cuh:26-93 semantics: XOR of
 // all bytes folded to 8 bits).  grid = (n, Y).
-#ifndef DGB_DECODE_NARROW_TU
+#if !defined(DGB_DECODE_NARROW_TU) && !defined(DGB_DECODE_NORM_TU)
 __global__ void __launch_bounds__(256)
 checksumKernel(DecodeScratch sc) {
   const uint32_t m = blockIdx.x;
@@ -1294,6 +1297,25 @@ struct FiniteCheck {
   }
 };
 struct NoFiniteCheck { static __device__ __forceinline__ uint32_t note(uint32_t w) { return w; } };
+// The squared norm of the device-scale sums (| kSqNorm, with kCheckFinite): the same writer passes every word it
+// stores, after note(), through noteSq(), which widens it exactly to fp64 (SK, the stored type) and adds its square
+// to the lane's `sq` with one fma (v * v is exact in fp64, so this is sq + v * v).  The decoder stores a lane's
+// words in descending row order, so that is the order of the lane's sum; decodeReduceBlock folds the lanes.
+template <int SK>
+__device__ __forceinline__ double wordF64(uint32_t w) {
+  if constexpr (SK == kKindF32) return (double)__uint_as_float(w);
+  else return (double)__uint_as_float(widenWord<SK>(w));
+}
+template <int SK>
+struct SqNormSum {
+  mutable double sq = 0.0;
+  __device__ __forceinline__ uint32_t noteSq(uint32_t w) const {
+    const double v = wordF64<SK>(w);
+    sq = fma(v, v, sq);
+    return w;
+  }
+};
+struct NoSqNorm { static __device__ __forceinline__ uint32_t noteSq(uint32_t w) { return w; } };
 template <bool SCALED>
 struct SumScale { static constexpr float scale = 1.0f; };  // unscaled sums: combine ignores it
 template <>
@@ -1320,7 +1342,8 @@ __host__ __device__ constexpr int reduceStoreKind(int wk) {
 //      (| kScaled: scaleWord in the archive's dense type, scaleWiden when widening);
 //   3. (| kAddWriter) the term added to the element's running sum with one addWord in the sum kind;
 //   4. (| kNarrowOut) the fp32 result rounded once to the archive's 16-bit type (narrowWord);
-//   5. (| kCheckFinite) the result noted by FiniteCheck before it is stored.
+//   5. (| kCheckFinite) the result noted by FiniteCheck before it is stored;
+//   6. (| kSqNorm) its square added to the lane's fp64 sum by SqNormSum.
 // It stores one u16 (same-type fp16 / bf16 sums, and the narrowing writers) or one u32 (fp32 and widening sums: a
 // row is one 128 B store) per element.  Add writers load a row group's running sums when the group starts (volatile
 // loads in at(), so they are issued there), writeSlow and writePartial the one sum they add to.  A narrowing writer
@@ -1332,12 +1355,14 @@ template <int WK>
 struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
                       SumScale<(WK & kScaled) != 0>,
                       SumNarrowOut<(WK & kNarrowOut) != 0>,
-                      std::conditional<(WK & kCheckFinite) != 0, FiniteCheck<reduceStoreKind(WK)>, NoFiniteCheck>::type {
+                      std::conditional<(WK & kCheckFinite) != 0, FiniteCheck<reduceStoreKind(WK)>, NoFiniteCheck>::type,
+                      std::conditional<(WK & kSqNorm) != 0, SqNormSum<reduceStoreKind(WK)>, NoSqNorm>::type {
   typedef RowWriter<reduceArchiveKind(WK)> B;
   static constexpr int AK = reduceArchiveKind(WK), kSumKind = reduceSumKind(WK);
   static constexpr bool kAdd = (WK & kAddWriter) != 0, kWiden = (WK & kWidenF32) != 0;
   static constexpr bool kScale = (WK & kScaled) != 0, kNarrow = (WK & kNarrowOut) != 0;
   static_assert(!kNarrow || kWiden, "a narrowing writer sums in fp32");
+  static_assert((WK & kSqNorm) == 0 || (WK & kCheckFinite) != 0, "the squared norm is taken by the checking writer");
   typedef typename std::conditional<kSumKind == kKindF32, uint32_t, uint16_t>::type T;
   T* sum;
   struct Cursor {
@@ -1377,20 +1402,20 @@ struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
   template <int J>
   __device__ __forceinline__ void write(const Cursor& c, uint32_t entry) const {
     if constexpr (kNarrow)
-      c.d[J * 32] = (uint16_t)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
+      c.d[J * 32] = (uint16_t)this->noteSq(this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale)));
     else
-      c.o[J * 32] = (T)this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale));
+      c.o[J * 32] = (T)this->noteSq(this->note(combine(kAdd ? c.prev[J] : 0u, B::template word<J>(c.in, entry), this->scale)));
   }
   __device__ __forceinline__ void writeSlow(uint32_t row, uint32_t entry) const {
     if constexpr (isSparseKind(AK)) {
       writePartial(row, entry, true);
     } else if constexpr (kNarrow) {
-      this->dst[row * 32u] = (uint16_t)this->note(combine(kAdd ? sum[row * 32u] : 0u, B::wordSlow(row, entry), this->scale));
+      this->dst[row * 32u] = (uint16_t)this->noteSq(this->note(combine(kAdd ? sum[row * 32u] : 0u, B::wordSlow(row, entry), this->scale)));
     } else if constexpr (kAdd) {
       T* o = sum + row * 32u;
-      *o = (T)this->note(combine(*o, B::wordSlow(row, entry), this->scale));
+      *o = (T)this->noteSq(this->note(combine(*o, B::wordSlow(row, entry), this->scale)));
     } else {
-      sum[row * 32u] = (T)this->note(combine(0u, B::wordSlow(row, entry), this->scale));
+      sum[row * 32u] = (T)this->noteSq(this->note(combine(0u, B::wordSlow(row, entry), this->scale)));
     }
   }
   // sparse kinds: every lane takes part in the word's vote; lanes with valid = false store nothing
@@ -1399,9 +1424,9 @@ struct RowWriterSum : RowWriter<reduceArchiveKind(WK)>,
     if (valid) {
       T* o = sum + row * 32u;
       if constexpr (kNarrow)
-        this->dst[row * 32u] = (uint16_t)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
+        this->dst[row * 32u] = (uint16_t)this->noteSq(this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale)));
       else
-        *o = (T)this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale));
+        *o = (T)this->noteSq(this->note(combine(kAdd ? (uint32_t)*o : 0u, w, this->scale)));
     }
   }
 };
@@ -1424,13 +1449,14 @@ __device__ __forceinline__ bool reduceArchiveOk(const void* in, uint32_t words) 
 }
 
 // block `block` of one archive through writer kind WK (the single-launch decoder's block body); narrowOut: the
-// group's 16-bit output, which only the narrowing writers (| kNarrowOut) store to
+// group's 16-bit output, which only the narrowing writers (| kNarrowOut) store to; sqPart: the group's fp64 block
+// partials, which only the squared-norm writers (| kSqNorm) store to
 template <int WK, int PB>
 __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, uint32_t block, uint32_t nb,
                                                   const typename Lut<PB, false>::Entry* __restrict__ lut,
                                                   uint32_t ring, uint8_t* mySlot, uint32_t myBar, uint32_t& phase,
                                                   uint32_t slotWords, uint32_t lane, float scale,
-                                                  float* foundInf, void* narrowOut) {
+                                                  float* foundInf, void* narrowOut, double* sqPart = nullptr) {
   const ArchiveView av = openArchive<reduceArchiveKind(WK)>(in);
   const uint8_t* pStates = av.ans + kAnsHeaderBytes + kAnsPdfBytes;
   const uint2* pBlockWords = reinterpret_cast<const uint2*>(pStates + 128u * (size_t)nb);
@@ -1476,19 +1502,27 @@ __device__ __forceinline__ void decodeReduceBlock(const uint8_t* in, void* out, 
     // one vote per block; every lane that saw a non-finite word would store the same 1.0f
     if (__any_sync(0xffffffffu, wr.bad != 0u) && lane == 0 && foundInf) *foundInf = 1.0f;
   }
+  if constexpr ((WK & kSqNorm) != 0) {
+    // the block's partial q: the xor butterfly p += shfl_xor(p, o), o = 16, 8, 4, 2, 1 (every lane ends with the
+    // same value); the block is decoded once per call by this writer, so q is stored once
+    double q = wr.sq;
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    if (lane == 0) sqPart[block] = q;
+  }
 }
 
 // f(std::integral_constant<int, K>()) with K the writer kind of one archive: WK when it is stored (archive a0 of a
 // pass that does not add), WK | kAddWriter when it is added; | kNarrowOut as well for the last archive of a
 // narrowing sum (NARROW kinds only), and | kCheckFinite for the last archive of a checked sum (CHECK kinds only, so
-// the others instantiate no checking or narrowing writer)
-template <int WK, bool CHECK, bool NARROW = false, typename F>
+// the others instantiate no checking or narrowing writer), with | kSqNorm too in the squared-norm kinds (NORM)
+template <int WK, bool CHECK, bool NARROW = false, bool NORM = false, typename F>
 __device__ __forceinline__ void withWriterKind(bool store, bool last, F&& f) {
   if constexpr (NARROW) {
-    if (last) return withWriterKind<WK | kNarrowOut, CHECK>(store, true, f);
+    if (last) return withWriterKind<WK | kNarrowOut, CHECK, false, NORM>(store, true, f);
   }
   if constexpr (CHECK) {
-    if (last) return withWriterKind<WK | kCheckFinite, false>(store, false, f);
+    if (last) return withWriterKind<WK | kCheckFinite | (NORM ? kSqNorm : 0), false>(store, false, f);
   }
   if (store) f(std::integral_constant<int, WK>());
   else f(std::integral_constant<int, WK | kAddWriter>());
@@ -1505,15 +1539,22 @@ __device__ __forceinline__ void withWriterKind(bool store, bool last, F&& f) {
 // narrowOut[g] its 16-bit output; archive width - 1 goes through the narrowing writer, which reads the accumulator
 // and stores the rounded sum to narrowOut[g], and every other archive through the widening writers into the
 // accumulator.
+// | kSqNorm (decodeReduceNormKernel, device-scale kinds only): the writer of archive width - 1 also stores the fp64
+// squared-norm partial of each block of group g to sqPart[sqOff[g] + block], and groupOk[g] records whether every
+// archive of group g is valid (the fold kernel, decode_norm.cu, reads both).
 template <int KIND, int PB>
 __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
                                                  uint32_t width, uint32_t a0, uint32_t a1, bool addFirst,
                                                  uint32_t slotWords, uint8_t* __restrict__ outSuccess,
-                                                 const float* scaleDev, float* foundInf, void* const* narrowOut) {
+                                                 const float* scaleDev, float* foundInf, void* const* narrowOut,
+                                                 double* sqPart = nullptr, const uint32_t* sqOff = nullptr,
+                                                 uint32_t* groupOk = nullptr) {
   constexpr int AK = reduceArchiveKind(KIND);
   constexpr bool DEV = (KIND & kDevScale) != 0;
   constexpr bool NARROW = (KIND & kNarrowOut) != 0;
-  constexpr int WK = KIND & ~(kDevScale | kNarrowOut);  // the writer kind of archive 0; | kAddWriter for the others
+  constexpr bool NORM = (KIND & kSqNorm) != 0;
+  // the writer kind of archive 0; | kAddWriter for the others
+  constexpr int WK = KIND & ~(kDevScale | kNarrowOut | kSqNorm);
   constexpr int WARPS = kReduceWarps;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t K = 1u << PB;
@@ -1591,6 +1632,8 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
     const uint32_t blocksCap = gd.work0, nb = divUp(gd.size, kBlockBytes);
     void* nout = nullptr;
     if constexpr (NARROW) nout = narrowOut[g];
+    double* gpart = nullptr;
+    if constexpr (NORM) gpart = sqPart + sqOff[g];
 
     // ---- every archive of the group is checked before anything is stored to it: the decision depends on the
     //      headers and out_size alone, so every CTA and every pass takes the same one ----
@@ -1600,7 +1643,15 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
       if (report) outSuccess[g * width + j] = v ? 1 : 0;
       ok = ok && v;
     }
-    const bool work = __syncthreads_and(ok) && nb > 0;
+    bool work;
+    if constexpr (NORM) {
+      // the same decision on every CTA and in every pass, so whichever CTA leased the group may record it
+      const bool all = __syncthreads_and(ok);
+      if (t == 0) groupOk[g] = all ? 1u : 0u;
+      work = all && nb > 0;
+    } else {
+      work = __syncthreads_and(ok) && nb > 0;
+    }
     if (work) {
       for (uint32_t a = a0; a < a1; ++a)
         buildLut<PB, false, WARPS>(openArchive<AK>(static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in)).ans,
@@ -1621,10 +1672,10 @@ __device__ __forceinline__ void decodeReduceBody(const DecodeScratch& sc, const 
           const uint8_t* in = static_cast<const uint8_t*>(memberAt(im, sc.members, g * width + a).in);
           // archive width - 1 writes the final value of every element: the device-scale sums check it there, and
           // the narrowing sums round it there
-          withWriterKind<WK, DEV, NARROW>(a == a0 && !addFirst, a + 1 == width, [&](auto wk) {
+          withWriterKind<WK, DEV, NARROW, NORM>(a == a0 && !addFirst, a + 1 == width, [&](auto wk) {
             constexpr int W = decltype(wk)::value;
             decodeReduceBlock<W, PB>(in, gd.out, block, nb, lut[(W & kAddWriter) != 0 ? a - a0 : 0u], ring, mySlot,
-                                     myBar, phase, slotWords, lane, scale, foundInf, nout);
+                                     myBar, phase, slotWords, lane, scale, foundInf, nout, gpart);
           });
         }
       }
@@ -1666,15 +1717,31 @@ decodeReduceNarrowKernel(DecodeScratch sc, const __grid_constant__ InlineMembers
   decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf,
                              narrowOut);
 }
+// the squared-norm sums (a device-scale kind | kSqNorm, narrowing or not; decode_norm.cu): the device-scale kernels'
+// parameters, the narrowing table (null for the others), the block partials, their per-group offsets and the
+// per-group validity flags
+template <int KIND, int PB>
+__global__ void __launch_bounds__(kReduceWarps * 32, 4)
+decodeReduceNormKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, uint32_t groups,
+                       uint32_t width, uint32_t a0, uint32_t a1, bool addFirst, uint32_t slotWords,
+                       uint8_t* __restrict__ outSuccess, const float* __restrict__ scaleDev,
+                       float* __restrict__ foundInf, void* const* __restrict__ narrowOut,
+                       double* __restrict__ sqPart, const uint32_t* __restrict__ sqOff,
+                       uint32_t* __restrict__ groupOk) {
+  static_assert((KIND & (kScaled | kDevScale | kSqNorm)) == (kScaled | kDevScale | kSqNorm), "");
+  decodeReduceBody<KIND, PB>(sc, im, groups, width, a0, a1, addFirst, slotWords, outSuccess, scaleDev, foundInf,
+                             narrowOut, sqPart, sqOff, groupOk);
+}
 
 template <int KIND, int PB>
 int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const InlineMembers& im, uint32_t groups,
                        uint32_t width, uint64_t totalChunks, bool accumulate, uint8_t* outSuccess, cudaStream_t stream,
                        const float* scaleDev = nullptr, float* foundInf = nullptr,
-                       void* const* narrowOut = nullptr) {
-  constexpr bool DEV = (KIND & kDevScale) != 0, NARROW = (KIND & kNarrowOut) != 0;
+                       void* const* narrowOut = nullptr, const SqNormScratch* norm = nullptr) {
+  constexpr bool DEV = (KIND & kDevScale) != 0, NARROW = (KIND & kNarrowOut) != 0, NORM = (KIND & kSqNorm) != 0;
   const void* kern;
-  if constexpr (NARROW) kern = (const void*)decodeReduceNarrowKernel<KIND, PB>;
+  if constexpr (NORM) kern = (const void*)decodeReduceNormKernel<KIND, PB>;
+  else if constexpr (NARROW) kern = (const void*)decodeReduceNarrowKernel<KIND, PB>;
   else if constexpr (DEV) kern = (const void*)decodeReduceDevScaleKernel<KIND, PB>;
   else kern = (const void*)decodeReduceKernel<KIND, PB>;
   uint32_t slotWords;
@@ -1689,7 +1756,11 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
     DGB_CUDA_TRY(cudaMemsetAsync(sc.next, 0, 8 * (size_t)groups * width, stream));
     timerBegin(opt, kSlotDecode, stream);
     const uint32_t a1 = std::min(width, a0 + kReducePass);
-    if constexpr (NARROW)
+    if constexpr (NORM)
+      decodeReduceNormKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
+          sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess, scaleDev, foundInf, narrowOut,
+          norm->part, norm->off, norm->ok);
+    else if constexpr (NARROW)
       decodeReduceNarrowKernel<KIND, PB><<<grid, kReduceWarps * 32, smemBytes, stream>>>(
           sc, im, groups, width, a0, a1, accumulate || a0 > 0, slotWords, outSuccess, scaleDev, foundInf, narrowOut);
     else if constexpr (DEV)
@@ -1706,7 +1777,7 @@ int launchDecodeReduce(const Options& opt, const DecodeScratch& sc, const Inline
 
 }  // namespace
 
-#ifdef DGB_DECODE_NARROW_TU
+#if defined(DGB_DECODE_NARROW_TU)
 // decode_narrow.cu compiles this file once more with DGB_DECODE_NARROW_TU: that module holds the narrowing sums'
 // kernels and this launcher only.  In the main module their 36 kernels changed the code ptxas generated for the
 // sparse fp32 decode-and-sum kernels (the same sources gave a different and longer schedule), so they are kept apart.
@@ -1735,7 +1806,7 @@ int launchDecodeReduceNarrow(int kind, int pb, bool scaled, const Options& opt, 
     }
   }); });
 }
-#else
+#elif !defined(DGB_DECODE_NORM_TU)
 
 size_t decodeTempBytes(int /*kind*/, uint32_t n) { return planDecodeScratch(n).total + 256; }
 
@@ -1875,13 +1946,14 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
 int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, uint32_t groups, uint32_t width,
                  const void* const* in, void* const* out, const uint32_t* outSize, bool accumulate,
                  uint8_t* outSuccess_dev, bool sparse, const float* scale, const float* scaleDev, float* foundInf,
-                 cudaStream_t stream, void* const* narrowOut) {
+                 cudaStream_t stream, void* const* narrowOut, double* sqNorm) {
   // dense fp16 / bf16 / fp32 archives, or (sparse) their sparse types 5, 6 and 8; scale: null for a plain sum, else
   // the multiplier of the scaled kinds; scaleDev (device memory, read by the kernels) in place of scale for the
   // device-scale kinds, with the non-finite flag foundInf (may be null).  narrowOut (host array of G, or null): a
   // narrowing sum of fp16 / bf16 archives, whose out[g] (outKind fp32) is the group's accumulator and narrowOut[g]
   // its output of the archive's 16-bit type; out and out[g] may be null when the call reads no accumulator (W = 1
-  // without accumulate)
+  // without accumulate).  sqNorm (device, G doubles; with scaleDev only): the squared-norm kernels (decode_norm.cu),
+  // whose block partials take the scratch past the decode's own
   if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
   // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
   const int dk = denseKind(kind);
@@ -1896,7 +1968,8 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   if (n64 > 0xffffffffull) return DGB_ERR_INVALID_ARG;
   const uint32_t n = (uint32_t)n64;
   const DecodePlan dp = planDecodeScratch(n);
-  if (!temp || tempBytes < dp.total) return DGB_ERR_TEMP_TOO_SMALL;
+  const size_t need = dp.total + (sqNorm ? sqNormScratchBytes(groups, sqNormBlocks(groups, outSize)) : 0u);
+  if (!temp || tempBytes < need) return DGB_ERR_TEMP_TOO_SMALL;
   if (reinterpret_cast<uintptr_t>(temp) & 255u) return DGB_ERR_INVALID_ARG;
 
   const Options opt = options();  // one snapshot per call
@@ -1938,10 +2011,20 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   // the narrowing sums' table of 16-bit outputs: G pointers in the scratch the checksum pass of a plain decode uses,
   // 3 * 4 * n >= 8 * G bytes that no decode-and-sum touches otherwise
   im.scale = scale ? *scale : 1.0f;  // a kernel parameter: a captured launch keeps the value it was captured with
+  void** t = nullptr;
   if (narrowOut) {
-    void** t = reinterpret_cast<void**>(base + dp.checksum);
+    t = reinterpret_cast<void**>(base + dp.checksum);
     const int rc = uploadTable(t, narrowOut, sizeof(void*) * (size_t)groups, stream);
     if (rc != DGB_OK) return rc;
+  }
+  if (sqNorm) {
+    SqNormScratch ns;
+    const int rc = sqNormPrepare(base + dp.total, groups, outSize, &ns, stream);
+    if (rc != DGB_OK) return rc;
+    return launchDecodeReduceNorm(kind, pb, widen, opt, sc.members, sc.next, im, groups, width, totalChunks,
+                                  accumulate, outSuccess_dev, stream, scaleDev, foundInf, t, ns, sqNorm);
+  }
+  if (narrowOut) {
     return launchDecodeReduceNarrow(kind, pb, scale != nullptr, opt, sc.members, sc.next, im, groups, width,
                                     totalChunks, accumulate, outSuccess_dev, stream, scaleDev, foundInf, t);
   }
@@ -2146,6 +2229,6 @@ int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool 
   return DGB_OK;
 }
 
-#endif  // DGB_DECODE_NARROW_TU
+#endif  // DGB_DECODE_NARROW_TU, DGB_DECODE_NORM_TU
 
 }  // namespace dgb

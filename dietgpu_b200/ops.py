@@ -431,6 +431,17 @@ def _check_dev_scale(scale32, scale_tensor, found_inf, dev) -> None:
         _check_flag_tensor("found_inf", found_inf, dev)
 
 
+def _check_sq_norm(what: str, t, groups: int, dev) -> None:
+    """A contiguous float64 CUDA tensor of `groups` elements on dev (the squared norms of a call)."""
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{what} is a float64 CUDA tensor, not {type(t).__name__}")
+    if t.dtype != torch.float64 or t.numel() != groups or not t.is_contiguous():
+        raise ValueError(f"{what} is a contiguous float64 tensor of {groups} element(s), not {t.dtype} with "
+                         f"{t.numel()} element(s){'' if t.is_contiguous() else ', non-contiguous'}")
+    if not t.is_cuda or t.device != dev:
+        raise ValueError(f"{what} must be on the device {dev}, not {t.device}")
+
+
 def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequence[torch.Tensor],
                            accumulate: bool = False, temp_mem: Optional[torch.Tensor] = None,
                            out_status: Optional[torch.Tensor] = None, *,
@@ -438,7 +449,8 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                            archive_dtype: Optional[torch.dtype] = None, sparse: bool = False,
                            scale: Optional[float] = None, scale_tensor: Optional[torch.Tensor] = None,
                            found_inf: Optional[torch.Tensor] = None, reduce_dtype: Optional[torch.dtype] = None,
-                           acc: Optional[Sequence[torch.Tensor]] = None) -> int:
+                           acc: Optional[Sequence[torch.Tensor]] = None,
+                           sq_norm: Optional[torch.Tensor] = None) -> int:
     """Decode-and-sum (dgb_float_decompress_reduce_to): ts_in is G lists of W uint8 float archives each, ts_out G
     contiguous CUDA tensors of one dtype (float16, bfloat16 or float32).  ts_out[g] becomes
     (ts_out[g] if accumulate else x(g, 0)) + x(g, 1) + ... + x(g, W - 1), added left to right with torch's adds in
@@ -482,9 +494,22 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     the intermediate sums of the call (their contents afterwards are unspecified); ts_out[g] is only written.  acc
     is required with accumulate=True; otherwise None takes a stream-ordered temporary when W > 1.  reduce_dtype
     None or the outputs' dtype is the call described above; any other reduce_dtype, an acc without this path, or an
-    acc of the wrong dtype, size or device raises ValueError before any archive is read."""
+    acc of the wrong dtype, size or device raises ValueError before any archive is read.
+
+    sq_norm (with scale_tensor only; dgb_float_decompress_reduce_scaled_dev_norm / _narrow_norm): a contiguous float64
+    CUDA tensor of G elements on the outputs' device.  sq_norm[g] is overwritten with the squared norm of the
+    elements the call stores to ts_out[g] (after scaling, and after the 16-bit rounding with reduce_dtype), taken in
+    fp64 in the fixed order of include/dietgpu_b200.h, so it is bit-reproducible and equals sq_norm() of the
+    outputs.  A group with an invalid archive leaves sq_norm[g] untouched.  Works with archive_dtype, sparse,
+    reduce_dtype=torch.float32 / acc and found_inf; outputs and found_inf are bit-identical to the call without it.
+    Without scale_tensor, with scale, or of the wrong dtype, size or device it raises ValueError before any archive
+    is read."""
     scale32 = _scale32(scale)
     _check_dev_scale(scale32, scale_tensor, found_inf, ts_out[0].device if len(ts_out) else None)
+    if sq_norm is not None:
+        if scale_tensor is None:
+            raise ValueError("decompress_data_reduce: sq_norm needs scale_tensor (torch.ones(1) for the unscaled sum)")
+        _check_sq_norm("decompress_data_reduce: sq_norm", sq_norm, len(ts_out), ts_out[0].device if len(ts_out) else None)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
@@ -542,6 +567,19 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                 acc.append(flat[o:o + to.numel()])
                 o += to.numel()
         s = None if scale32 is None else C.c_float(float(scale32))
+        if sq_norm is not None:
+            sizes = capi.u32_array([t.numel() for t in ts_out])
+            with torch.cuda.device(dev):
+                need = L.dgb_float_decompress_reduce_norm_temp_bytes(ft, g, width, sizes)
+                tmp = _Temp(temp_mem, need, dev)
+                rc = L.dgb_float_decompress_reduce_narrow_norm(
+                    tmp.ptr, tmp.bytes, ft, prob_bits, g, width, capi.ptr_array([t.data_ptr() for t in ins]),
+                    None if acc is None else capi.ptr_array([a.data_ptr() for a in acc]),
+                    capi.ptr_array([t.data_ptr() for t in ts_out]), sizes, int(bool(accumulate)),
+                    scale_tensor.data_ptr(), None if found_inf is None else found_inf.data_ptr(), sq_norm.data_ptr(),
+                    st_ptr, _stream())
+            capi.check(rc, "decompress_data_reduce")
+            return tmp.need
         with torch.cuda.device(dev):
             need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
             tmp = _Temp(temp_mem, need, dev)
@@ -561,8 +599,14 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     elif scale_tensor is not None:
         entry = L.dgb_float_decompress_reduce_scaled_dev
         extra = (scale_tensor.data_ptr(), found_inf.data_ptr() if found_inf is not None else None)
+        if sq_norm is not None:
+            entry, extra = L.dgb_float_decompress_reduce_scaled_dev_norm, extra + (sq_norm.data_ptr(),)
     with torch.cuda.device(dev):
-        need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
+        if sq_norm is not None:
+            need = L.dgb_float_decompress_reduce_norm_temp_bytes(ft, g, width,
+                                                                 capi.u32_array([t.numel() for t in ts_out]))
+        else:
+            need = L.dgb_float_decompress_temp_bytes(ft, n, 0)
         tmp = _Temp(temp_mem, need, dev)
         rc = entry(tmp.ptr, tmp.bytes, ft, out_ft, prob_bits, g, width,
                    capi.ptr_array([t.data_ptr() for t in ins]),
@@ -571,6 +615,43 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                    st_ptr, _stream())
     capi.check(rc, "decompress_data_reduce")
     return tmp.need
+
+
+def sq_norm(tensors: Sequence[torch.Tensor], out: Optional[torch.Tensor] = None,
+            temp_mem: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The squared norm of each of G contiguous CUDA tensors of one dtype (float16, bfloat16 or float32) on one device,
+    as a float64 tensor [G] (dgb_float_sq_norm): each element widened exactly to fp64 and its square summed in the
+    fixed order of include/dietgpu_b200.h, the order decompress_data_reduce(sq_norm=) uses, so the two agree bit for
+    bit on the same elements.  inf or NaN elements give an inf or NaN norm; an empty tensor gives +0.  out: a
+    contiguous float64 CUDA tensor of G elements on the tensors' device, overwritten and returned.  Other inputs raise
+    ValueError before any device work."""
+    ts = list(tensors)
+    if not ts:
+        if out is not None:
+            _check_sq_norm("sq_norm: out", out, 0, out.device)
+            return out
+        return torch.empty(0, dtype=torch.float64, device="cuda")
+    dtype, dev = ts[0].dtype, ts[0].device
+    if dtype not in _REDUCE_TYPES:
+        raise ValueError(f"sq_norm takes float16, bfloat16 or float32 tensors, not {dtype}")
+    for t in ts:
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_cuda or t.device != dev \
+                or not t.is_contiguous():
+            raise ValueError("sq_norm takes contiguous CUDA tensors of one dtype on one device")
+        if t.numel() > 0xFFFFFFFF:
+            raise ValueError("sq_norm: a tensor of more than 2^32 - 1 elements")
+    if out is None:
+        out = torch.empty(len(ts), dtype=torch.float64, device=dev)
+    else:
+        _check_sq_norm("sq_norm: out", out, len(ts), dev)
+    L = capi.lib()
+    sizes = capi.u32_array([t.numel() for t in ts])
+    with torch.cuda.device(dev):
+        tmp = _Temp(temp_mem, L.dgb_float_sq_norm_temp_bytes(len(ts), sizes), dev)
+        rc = L.dgb_float_sq_norm(tmp.ptr, tmp.bytes, _REDUCE_TYPES[dtype], len(ts),
+                                 capi.ptr_array([t.data_ptr() for t in ts]), sizes, out.data_ptr(), _stream())
+    capi.check(rc, "sq_norm")
+    return out
 
 
 def decompress_data_split_size(compress_as_float: bool, ts_in: Sequence[torch.Tensor], t_out: torch.Tensor,

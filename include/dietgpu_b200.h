@@ -336,6 +336,67 @@ int dgb_float_decompress_reduce_narrow(void* temp_dev, size_t temp_bytes, int fl
                                        int accumulate, const float* scale, const float* scale_dev,
                                        float* found_inf_dev, uint8_t* out_success_dev, void* stream);
 
+/* Squared norms (new; no reference counterpart), for clipping a reduced gradient by its global norm without reading
+ * it again.  The squared norm of a group is an fp64 value over the float words v[0 .. n-1] of the group (for a
+ * decode-and-sum: the words the call stores, after scaling and after the narrowing sums' 16-bit rounding), taken in
+ * this order, whatever the grid or the order in which blocks were claimed:
+ *   1. lane: word i lies in block k = i / 4096, row r = (i mod 4096) / 32 and lane l = i mod 32.  Each lane starts
+ *      from +0 and adds, for its words of block k in DESCENDING row order (the decoder's order: a partial last row
+ *      first), v * v with v the word widened exactly to fp64 (v * v is exact, so this is one fp64 add; fma(v, v, p)).
+ *      A lane past the end of a partial row adds nothing; an elided sparse word is the +0 or -0 it stands for.
+ *   2. warp: the 32 lane sums p are combined by the xor butterfly p = p + shfl_xor(p, o) for o = 16, 8, 4, 2, 1,
+ *      which leaves every lane with the same value q[k], the block's partial.
+ *   3. group: thread t (0 <= t < 256) of one 256-thread CTA sums q[t], q[t + 256], q[t + 512], ... from +0 in
+ *      increasing block order; each of the 8 warps applies the butterfly of step 2 to its 32 sums, and the result is
+ *      ((w[0] + w[1]) + w[2]) + ... + w[7] over the warp sums w in warp order.
+ * Every add is one fp64 round-to-nearest-even add.  An inf or NaN word gives an inf or NaN norm; an empty group gets
+ * +0.  tests/sq_norm_reference.py restates the order in numpy. */
+
+/* dgb_float_decompress_reduce_scaled_dev, and sq_norm_dev[g] (device, G doubles, 8 B aligned; required) overwritten
+ * with the squared norm above of the out_size[g] words the call stores to out[g].  Only the writer of archive W - 1
+ * contributes, so a call of several launches (W > 4) takes the norm in its last.  A group with an invalid archive
+ * leaves sq_norm_dev[g] untouched, as it leaves out[g].  Outputs, statuses and found_inf_dev are bit-identical to
+ * dgb_float_decompress_reduce_scaled_dev's.  An unscaled caller passes a device 1.0f as scale_dev.
+ * Scratch: dgb_float_decompress_reduce_norm_temp_bytes(float_type, G, W, out_size).
+ * DGB_ERR_INVALID_ARG before any CUDA call: sq_norm_dev NULL or not 8 B aligned, and everything
+ * dgb_float_decompress_reduce_scaled_dev refuses.  num_groups = 0 returns DGB_OK and writes nothing; the call never
+ * synchronises and may be captured into a CUDA graph. */
+int dgb_float_decompress_reduce_scaled_dev_norm(void* temp_dev, size_t temp_bytes, int float_type,
+                                                int out_float_type, int prob_bits, uint32_t num_groups,
+                                                uint32_t archives_per_group, const void* const* in, void* const* out,
+                                                const uint32_t* out_size, int accumulate, const float* scale_dev,
+                                                float* found_inf_dev, double* sq_norm_dev, uint8_t* out_success_dev,
+                                                void* stream);
+
+/* dgb_float_decompress_reduce_narrow with the device scale (scale_dev required; there is no host scale), and
+ * sq_norm_dev[g] as in dgb_float_decompress_reduce_scaled_dev_norm, over the 16-bit words stored to out[g] (the
+ * rounded sums).  Scratch: dgb_float_decompress_reduce_norm_temp_bytes(float_type, G, W, out_size).
+ * DGB_ERR_INVALID_ARG before any CUDA call: scale_dev NULL or not 4 B aligned, sq_norm_dev NULL or not 8 B aligned,
+ * and everything dgb_float_decompress_reduce_narrow refuses. */
+int dgb_float_decompress_reduce_narrow_norm(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
+                                            uint32_t num_groups, uint32_t archives_per_group, const void* const* in,
+                                            float* const* acc, void* const* out, const uint32_t* out_size,
+                                            int accumulate, const float* scale_dev, float* found_inf_dev,
+                                            double* sq_norm_dev, uint8_t* out_success_dev, void* stream);
+
+/* Scratch of the two entries above: dgb_float_decompress_temp_bytes(float_type, G * W, 0) plus the squared norm's own
+ * part, 8 B per 4096-word block of every group (8 * sum of ceil(out_size[g] / 4096)) and 12 B per group for the block
+ * offsets, sizes and validity flags, each rounded up to 256 B.  0 for an invalid float_type. */
+size_t dgb_float_decompress_reduce_norm_temp_bytes(int float_type, uint32_t num_groups, uint32_t archives_per_group,
+                                                   const uint32_t* out_size);
+
+/* The squared norm above of G dense float tensors already in device memory: in[g] (host array of G device
+ * pointers, aligned to the word size) holds size[g] words of float_type (DGB_FLOAT16, DGB_BFLOAT16 or DGB_FLOAT32),
+ * and sq_norm_dev[g] (device, 8 B aligned, required) is overwritten with their squared norm, bit-identical to what
+ * the decode-and-sum norm entries give for the same stored words.  A plain read of the words (one warp per 4096-word
+ * block).  Scratch: dgb_float_sq_norm_temp_bytes(G, size), 256 B aligned.  DGB_ERR_INVALID_ARG before any CUDA
+ * call for another float_type, sq_norm_dev NULL or misaligned, in or size NULL, or in[g] NULL or misaligned with
+ * size[g] > 0; num_groups = 0 returns DGB_OK and writes nothing.  Never synchronises; capturable. */
+int dgb_float_sq_norm(void* temp_dev, size_t temp_bytes, int float_type, uint32_t num_groups, const void* const* in,
+                      const uint32_t* size, double* sq_norm_dev, void* stream);
+/* 8 B per group for the pointer table, plus the squared norm's part of dgb_float_decompress_reduce_norm_temp_bytes. */
+size_t dgb_float_sq_norm_temp_bytes(uint32_t num_groups, const uint32_t* size);
+
 /* float/GpuFloatCodec.h:252-292 / float/GpuFloatInfo.cu:17-64 floatGetCompressedInfo{,Device}. */
 int dgb_float_get_compressed_info(void* temp_dev, size_t temp_bytes, const void* const* in,
                                   int in_is_device_array, uint32_t num_in_batch,

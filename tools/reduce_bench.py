@@ -19,6 +19,8 @@ the library (make -C dietgpu_b200/csrc variant NAME=p2 DEFS=-DDGB_REDUCE_PASS_AR
 an unscaled sum followed by torch.amp's unscale-and-check (bench_scale_tensor).
 --out-dtype: the narrowing decode-and-sum (fp32 sums rounded once to the 16-bit archive dtype) against the widening
 one followed by torch's .to() and against the same-type 16-bit sum (bench_out_dtype).
+--sq-norm: the device-scale decode-and-sum with its fused squared norm against the same call followed by
+ops.sq_norm of the outputs and by torch's fp64 squared norm of the outputs (bench_sq_norm).
 """
 import argparse
 import json
@@ -432,6 +434,75 @@ def bench_out_dtype(dtype, groups, width, n, iters, sparse):
     return r
 
 
+SQ_NORM_SHAPES = SCALE_SHAPES + [  # (dtype, groups, width, words, out dtype, sparse ReLU data, narrowing)
+    (torch.bfloat16, 8, 8, 2 << 20, torch.bfloat16, False, True),
+]
+
+
+def bench_sq_norm(dtype, groups, width, n, iters, out_dtype, sparse, narrow=False):
+    """--sq-norm, on the same archives, alternated, every call with scale_tensor and found_inf: (1) the decode-and-sum
+    with sq_norm; (2) the same call without it, then ops.sq_norm of the outputs; (3) the same call without it, then
+    torch's fp64 squared norm of the outputs (one .double().square().sum() per group).  Reported: call time of all
+    three (lowest of three alternated runs); kernel time (timing=1) of (1), of the sum without the norm ("sum") and
+    of the standalone norm alone ("norm"); the fused norm's extra kernel time ("1" - "sum") against "norm"; and the
+    standalone norm's bytes read over its kernel time as a share of the H100 SXM data sheet's 3.35 TB/s."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xs = [sparse_data(dtype, n, "relu" if sparse else "0", g) for _ in range(groups * width)]
+    temp = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
+    comp, sizes, _ = ops.compress_data(True, xs, sparse=sparse)
+    hs = sizes.cpu().tolist()
+    gi = [[comp[k * width + j, :hs[k * width + j]] for j in range(width)] for k in range(groups)]
+    del xs
+    outs = [torch.empty(n, dtype=out_dtype, device="cuda") for _ in range(groups)]
+    kw = dict(archive_dtype=dtype, sparse=sparse, scale_tensor=torch.full((1,), 0.125, device="cuda"),
+              found_inf=torch.zeros(1, device="cuda"))
+    if narrow:
+        kw.update(reduce_dtype=torch.float32, acc=[torch.empty(n, dtype=torch.float32, device="cuda")
+                                                   for _ in range(groups)])
+    norms = {k: torch.empty(groups, dtype=torch.float64, device="cuda") for k in ("1", "2", "3")}
+
+    def one():
+        ops.decompress_data_reduce(gi, outs, False, temp, sq_norm=norms["1"], **kw)
+
+    def the_sum():
+        ops.decompress_data_reduce(gi, outs, False, temp, **kw)
+
+    def norm():
+        ops.sq_norm(outs, out=norms["2"], temp_mem=temp)
+
+    def two():
+        the_sum()
+        norm()
+
+    def three():
+        the_sum()
+        for k, o in enumerate(outs):
+            norms["3"][k].copy_(o.double().square().sum())
+
+    fns = {"1": one, "2": two, "3": three}
+    for f in list(fns.values()) + [the_sum, norm]:  # warm-up
+        f()
+    torch.cuda.synchronize()
+    one()
+    two()
+    same = bool(((norms["1"] == norms["2"]) | (norms["1"].isnan() & norms["2"].isnan())).all())
+    rel_torch = float(((norms["1"] - norms["3"]).abs() / norms["3"]).max())
+    t = {k: [] for k in fns}
+    for _ in range(3):  # alternate
+        for k, f in fns.items():
+            t[k].append(timed(f, iters))
+    kt = {"1": kernel_us(one, iters), "sum": kernel_us(the_sum, iters), "norm": kernel_us(norm, iters)}
+    es = torch.empty(0, dtype=out_dtype).element_size()
+    r = {"shape": f"{'sparse relu ' if sparse else ''}{'narrowing ' if narrow else ''}"
+                  f"{str(dtype).split('.')[-1]}->{str(out_dtype).split('.')[-1]} {groups}x{width}x{n}",
+         "bit_equal_1_2": same, "max_rel_diff_1_3": rel_torch, "call_us": {k: min(v) for k, v in t.items()},
+         "call_us_max": {k: max(v) for k, v in t.items()}, "kernel_us": kt,
+         "fused_extra_us": kt["1"] - kt["sum"],
+         "norm_share_of_3350GBs": groups * n * es / (kt["norm"] * 1e-6) / 1e9 / PEAK_GBS}
+    r["fused_extra_below_norm"] = r["fused_extra_us"] < kt["norm"]
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -445,10 +516,19 @@ def main():
                          "unscale (bench_scale_tensor)")
     ap.add_argument("--out-dtype", action="store_true",
                     help="narrowing sums against widening sums + .to() and same-type sums (bench_out_dtype)")
+    ap.add_argument("--sq-norm", action="store_true",
+                    help="device-scale sums with the fused squared norm against the sum + ops.sq_norm and the sum + "
+                         "torch's norm (bench_sq_norm)")
     args = ap.parse_args()
     info = {"card": card(), "lib": capi.LIB_PATH, "results": []}
     print(info["card"], flush=True)
-    if args.out_dtype:
+    if args.sq_norm:
+        for shape in SQ_NORM_SHAPES:
+            r = bench_sq_norm(*shape[:4], args.iters, *shape[4:])
+            info["results"].append(r)
+            print(json.dumps(r), flush=True)
+        shapes = []
+    elif args.out_dtype:
         for shape in OUT_DTYPE_SHAPES:
             r = bench_out_dtype(*shape[:4], args.iters, shape[4])
             info["results"].append(r)
