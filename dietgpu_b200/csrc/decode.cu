@@ -83,6 +83,16 @@ __device__ __forceinline__ ArchiveView openArchive(const uint8_t* in) {
   return v;
 }
 
+// (checksum flag, checksum) of a member archive: the ANS header's (at `ans`) for byte archives, the float
+// header's (at `in`) otherwise.  With the flag clear the checksum word is undefined (the reference never writes
+// it), so such a member is not verified.
+template <int KIND>
+__device__ __forceinline__ uint2 storedChecksumOf(const void* in, const uint8_t* ans) {
+  const uint2 w = KIND == kKindBytes ? __ldg(reinterpret_cast<const uint2*>(ans + 16))
+                                     : __ldg(reinterpret_cast<const uint2*>(in) + 1);
+  return make_uint2(w.x & 0x10u, w.y);
+}
+
 // ---------------------------------------------------------------------------
 // P: plan.  One CTA; member i handled by thread (i % blockDim) in rounds.
 // ---------------------------------------------------------------------------
@@ -101,7 +111,7 @@ planKernel(DecodeScratch sc, uint32_t m0, uint32_t m1, uint32_t part, int pb,
       const MemberDesc md = sc.members[i];
       const ArchiveView av = openArchive<KIND>(static_cast<const uint8_t*>(md.in));
       bool ok = av.ok;
-      uint32_t need = 0, nb = 0, storedChecksum = 0;
+      uint32_t need = 0, nb = 0;
       if (ok) {
         const uint4 h0 = __ldg(reinterpret_cast<const uint4*>(av.ans));
         const uint4 h1 = __ldg(reinterpret_cast<const uint4*>(av.ans) + 1);
@@ -109,17 +119,15 @@ planKernel(DecodeScratch sc, uint32_t m0, uint32_t m1, uint32_t part, int pb,
         need = h0.z;  // uncompressed bytes == float words for float kinds
         ok = h0.x == kAnsMagicVersion && (int)(h1.x & 0xfu) == pb && nb == divUp(need, kBlockBytes);
         if (KIND != kKindBytes) ok = ok && need == av.floatWords;
-        storedChecksum = KIND == kKindBytes
-            ? h1.y
-            : __ldg(reinterpret_cast<const uint32_t*>(md.in) + 3);
       }
       // ans/GpuANSDecode.cuh:326-337: success iff capacity suffices; size reported regardless
       const bool success = ok && md.size >= need;
       if (outSuccess) outSuccess[i] = success ? 1 : 0;
       if (outSize) outSize[i] = ok ? need : 0u;
       if (wantChecksum) {
-        sc.archiveChecksum[i] = storedChecksum;
-        sc.sizes[i] = success ? need : 0u;
+        const uint2 ck = success ? storedChecksumOf<KIND>(md.in, av.ans) : make_uint2(0u, 0u);
+        sc.archiveChecksum[i] = ck.y;
+        sc.sizes[i] = ck.x ? need : 0u;
       }
       blocks = success ? nb : 0u;
     }
@@ -1005,7 +1013,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
     // ---- header(s), validity, LUT ----
     const ArchiveView av = openArchive<KIND>(static_cast<const uint8_t*>(md.in));
     bool ok = av.ok;
-    uint32_t need = 0, storedChecksum = 0, nb = 0;
+    uint32_t need = 0, nb = 0;
     if (ok) {
       const uint4 h0 = __ldg(reinterpret_cast<const uint4*>(av.ans));
       const uint4 h1 = __ldg(reinterpret_cast<const uint4*>(av.ans) + 1);
@@ -1013,7 +1021,6 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
       need = h0.z;  // uncompressed bytes == float words for float kinds
       ok = h0.x == kAnsMagicVersion && (int)(h1.x & 0xfu) == PB && nb == divUp(need, kBlockBytes);
       if (KIND != kKindBytes) ok = ok && need == av.floatWords;
-      storedChecksum = KIND == kKindBytes ? h1.y : __ldg(reinterpret_cast<const uint32_t*>(md.in) + 3);
     }
     // ans/GpuANSDecode.cuh:326-337: success iff capacity suffices; size reported regardless
     const bool memberOk = ok && md.size >= need;
@@ -1021,8 +1028,9 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
       if (outSuccess) outSuccess[m] = memberOk ? 1 : 0;
       if (outSize) outSize[m] = ok ? need : 0u;
       if (wantChecksum) {
-        sc.archiveChecksum[m] = storedChecksum;
-        sc.sizes[m] = memberOk ? need : 0u;
+        const uint2 ck = memberOk ? storedChecksumOf<KIND>(md.in, av.ans) : make_uint2(0u, 0u);
+        sc.archiveChecksum[m] = ck.y;
+        sc.sizes[m] = ck.x ? need : 0u;
       }
     }
     const bool work = memberOk && nb > 0;
@@ -1933,7 +1941,8 @@ int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     DGB_CUDA_TRY(cudaStreamSynchronize(stream));
     bool bad = false;
     for (uint32_t i = 0; i < n; ++i) {
-      // members that were skipped (capacity / bad header) are reported through outSuccess
+      // members that were skipped (capacity / bad header) are reported through outSuccess; members whose
+      // archive has the checksum flag clear carry no checksum and have size 0 here
       const bool mm = sizes[i] != 0 && got[i] != want[i];
       if (mismatchHost) mismatchHost[i] = mm ? 1 : 0;
       bad = bad || mm;

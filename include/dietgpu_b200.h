@@ -133,7 +133,9 @@ int dgb_ans_encode_split_size(void* temp_dev, size_t temp_bytes, int prob_bits, 
  * skipped (size = required bytes, or 0 for an invalid header).
  * With use_checksum != 0 the call synchronises `stream`, compares checksums
  * and returns DGB_ERR_CHECKSUM on mismatch; checksum_mismatch_host (optional
- * host u8[n]) then flags the failing members.  That synchronisation cannot be
+ * host u8[n]) then flags the failing members.  A member whose archive was
+ * written without a checksum (flag bit 4 of its options clear) is not
+ * verified: its checksum word is undefined.  That synchronisation cannot be
  * captured into a CUDA graph: on a capturing stream such a call returns
  * DGB_ERR_CAPTURING before it enqueues anything, and the capture stays valid. */
 int dgb_ans_decode_pointer(void* temp_dev, size_t temp_bytes, int prob_bits, int use_checksum,

@@ -220,6 +220,114 @@ def float_roundtrip(kind, word_arrays, pb=10, checksum=False, offsets=None, **kw
     return roundtrip(kind, word_arrays, pb, checksum, in_offsets=offsets, **kw)
 
 
+# ---- the bits the reference leaves undefined -------------------------------------
+#
+# The reference sets its header flags by read-modify-write over uninitialised memory and never writes the
+# fields below, so an archive it wrote into a reused buffer carries whatever was there; the pdf of an empty
+# member is whatever its scratch held.  Every reader must ignore them; `scribble` writes garbage into exactly
+# these places and nowhere else.
+
+_ANS_MAGIC, _FLOAT_MAGIC = 0xD00D0001, 0xF00F0001
+
+
+def _u32(a, off):
+    return int(a[off:off + 4].view(np.uint32)[0])
+
+
+def _ans_regions(a, base):
+    """(name, start, stop, bitmask) of the undefined bits of the ANS archive at byte `base` of `a`."""
+    opts = _u32(a, base + 16)
+    regs = [("ans options bits 5-31", base + 16, base + 20, 0xE0, 0xFF, 0xFF, 0xFF)]
+    if not opts & 0x10:
+        regs.append(("ans checksum (flag clear)", base + 20, base + 24))
+    regs.append(("ans unused0/1", base + 24, base + 32))
+    if _u32(a, base + 8) == 0:
+        # an empty member's pdf: the reference copies a table its statistics pass never wrote for it
+        regs.append(("pdf of an empty archive", base + 32, base + 544))
+    nb = _u32(a, base + 4)
+    bw_at = base + 544 + 128 * nb
+    if nb & 1:
+        regs.append(("block table pad entry", bw_at + 8 * nb, bw_at + 8 * nb + 8))
+    data = bw_at + 8 * (nb + (nb & 1))
+    bw = a[bw_at:bw_at + 8 * nb].view(np.uint32).reshape(nb, 2).astype(np.int64)
+    words, off = bw[:, 0] & 0xFFFF, bw[:, 1]
+    for k in np.flatnonzero(words % 8):
+        regs.append(("stream padding", data + 2 * int(off[k] + words[k]), data + 2 * int(off[k] + (words[k] + 7) // 8 * 8)))
+    return regs
+
+
+def undefined_regions(archive):
+    """The places of a byte or fp16 / bf16 / fp32 archive that the reference leaves undefined, as
+    (name, start, stop) byte ranges or (name, start, stop, m0, m1, m2, m3) for a word of which only the bits
+    set in the byte masks m0..m3 are undefined.  Derived from the defined fields only."""
+    a = np.ascontiguousarray(archive).view(np.uint8).reshape(-1)
+    magic = _u32(a, 0)
+    if magic == _ANS_MAGIC:
+        return _ans_regions(a, 0)
+    assert magic == _FLOAT_MAGIC, f"not an ANS or float archive (magic {magic:#x})"
+    opts, n = _u32(a, 8), _u32(a, 4)
+    ft = opts & 0xF
+    assert ft in (O.F16, O.BF16, O.F32), f"float type {ft} has no reference counterpart"
+    regs = [("float options bits 5-31", 8, 12, 0xE0, 0xFF, 0xFF, 0xFF)]
+    if not opts & 0x10:
+        regs.append(("float checksum (flag clear)", 12, 16))
+    nc = O.float_noncomp_bytes(ft, n)
+    if ft == O.F32:
+        p1 = 16 + 2 * ((n + 7) // 8 * 8)
+        regs += [("plane padding", 16 + 2 * n, p1), ("plane padding", p1 + n, 16 + nc)]
+    else:
+        regs.append(("plane padding", 16 + n, 16 + nc))
+    return regs + _ans_regions(a, 16 + nc)
+
+
+def undefined_mask(archive):
+    """uint8 array as long as the archive: per byte, the bits `scribble` may change."""
+    a = np.ascontiguousarray(archive).view(np.uint8).reshape(-1)
+    m = np.zeros(a.size, np.uint8)
+    for r in undefined_regions(a):
+        m[r[1]:r[2]] = r[3:] if len(r) > 3 else 0xFF
+    return m
+
+
+def _defined_fields(a):
+    """Every defined field of a byte or float archive, as comparable values."""
+    f = {}
+    base = 0
+    if _u32(a, 0) == _FLOAT_MAGIC:
+        n, opts = _u32(a, 4), _u32(a, 8)
+        ft = opts & 0xF
+        f.update(fmagic=_FLOAT_MAGIC, fsize=n, fopts=opts & 0x1F, fchecksum=_u32(a, 12) if opts & 0x10 else None)
+        if ft == O.F32:
+            p1 = 16 + 2 * ((n + 7) // 8 * 8)
+            f["planes"] = (a[16:16 + 2 * n].tobytes(), a[p1:p1 + n].tobytes())
+        else:
+            f["planes"] = (a[16:16 + n].tobytes(),)
+        base = 16 + O.float_noncomp_bytes(ft, n)
+    p = O.parse_ans(a[base:])
+    for k in ("magic", "num_blocks", "uncompressed", "total_words", "prob_bits", "use_checksum", "size"):
+        f[k] = p[k]
+    f["checksum"] = p["checksum"] if p["use_checksum"] else None
+    f["pdf"] = p["pdf"].tobytes() if p["uncompressed"] else None
+    f["states"], f["block_words"] = p["states"].tobytes(), p["block_words"].tobytes()
+    f["streams"] = [s.tobytes() for s in p["streams"]]
+    return f
+
+
+def scribble(archive, rng):
+    """A copy of a byte or fp16 / bf16 / fp32 archive with random values in every undefined place (the
+    options' undefined bits always change), checked to leave every defined field as it was."""
+    a = np.ascontiguousarray(archive).view(np.uint8).reshape(-1)
+    mask = undefined_mask(a)
+    out = (a & ~mask) | (rng.integers(0, 256, a.size, dtype=np.uint8) & mask)
+    # the options' bits 5-31 (of the float header and of the ANS header) always get a nonzero garbage value
+    for r in undefined_regions(a):
+        if "options" in r[0]:
+            w = out[r[1]:r[2]].view(np.uint32)
+            w[0] = (_u32(a, r[1]) & 0x1F) | (int(rng.integers(1, 1 << 27)) << 5)
+    assert _defined_fields(out) == _defined_fields(a), "scribble changed a defined field"
+    return out
+
+
 # ---- statistics helpers --------------------------------------------------------
 
 def coded_bytes(t, kind):

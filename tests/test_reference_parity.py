@@ -3,12 +3,11 @@ unmodified for sm_90a (oracle/build_ref.sh), produced on an H100 for seeded inpu
 written by tests/golden/make_ref_golden.py).  Pins what the reference's own tests leave unpinned (SURVEY 8c):
 byte-exact compressed sizes, field-exact archives (masking only the bits the reference leaves undefined), and
 decoding of the reference's archives.
-What this no longer tests directly, with the reference absent at test time:
-  * the reference decoding OUR archives (streams in completion order).  It is implied, not tested: its decoder reads
-    only the defined fields, which are equal here, and finds every block's stream through the block table.
-  * members of many blocks.  The stored members stop at 40000 bytes / 30001 floats (at most 10 blocks of 4 KiB) to keep the file
-    small; longer members (300000 bytes, 512 Ki floats, 256 MiB batches) are pinned through the CPU oracle in
-    tests/test_gpu_codec.py, and the oracle in turn to these archives by tests/test_oracle.py."""
+These stored archives stop at 40000 bytes / 30001 floats (at most 10 blocks of 4 KiB) and, for floats, at probBits
+10, so the file stays small and the checks here need no reference build.  Where build() compiled the reference
+(oracle/_ref/), tests/test_gpu_reference_interchange.py runs it live: the reference decoding OUR archives (every
+encoder variant, streams in completion order), encode parity at probBits 9-11 past 65536 blocks and on batches of
+64 x 1 Mi elements, and our readers on the reference's archives written over a 0xFF-filled buffer."""
 import os
 
 import numpy as np
