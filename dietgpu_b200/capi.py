@@ -26,7 +26,7 @@ SYMBOLS = [
     "dgb_ans_encode_pointer", "dgb_ans_encode_stride", "dgb_ans_encode_split_size",
     "dgb_ans_decode_pointer", "dgb_ans_decode_stride", "dgb_ans_decode_split_size",
     "dgb_ans_get_compressed_info",
-    "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_split_size",
+    "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_to_ef", "dgb_float_compress_split_size",
     "dgb_float_decompress_pointer", "dgb_float_decompress_split_size", "dgb_float_decompress_reduce",
     "dgb_float_decompress_reduce_to", "dgb_float_decompress_reduce_sparse", "dgb_float_decompress_reduce_scaled",
     "dgb_float_decompress_reduce_scaled_dev", "dgb_float_decompress_reduce_narrow",
@@ -101,6 +101,8 @@ def lib():
     L.dgb_float_compress_pointer.argtypes = [vp, sz, i32, i32, i32, u32, vp, vp, vp, vp, vp]
     L.dgb_float_compress_to.restype = i32
     L.dgb_float_compress_to.argtypes = [vp, sz, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp]
+    L.dgb_float_compress_to_ef.restype = i32
+    L.dgb_float_compress_to_ef.argtypes = [vp, sz, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp, vp]
     L.dgb_float_compress_split_size.restype = i32
     L.dgb_float_compress_split_size.argtypes = [vp, sz, i32, i32, i32, u32, vp, vp, vp, u32, vp, vp]
     L.dgb_float_decompress_pointer.restype = i32

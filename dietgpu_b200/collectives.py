@@ -343,11 +343,41 @@ def _check_sparse_wire(dtype: torch.dtype, what: str, sparse: bool, wire_dtype: 
         raise ValueError(f"{what}: sparse=True is not supported with the peer-memory transports")
 
 
+def _check_feedback(what: str, e: Optional[torch.Tensor], t: torch.Tensor, wire_dtype: Optional[torch.dtype]) -> None:
+    """error_feedback: None, or a float32 CUDA tensor shaped like t, laid out like it (contiguous, same address modulo
+    16) and not overlapping it, with wire_dtype (it holds the rounding error of the narrowing compress)."""
+    if e is None:
+        return
+    if wire_dtype is None:
+        raise ValueError(f"{what}: error_feedback needs wire_dtype (it holds the rounding error of the float32 -> "
+                         "wire_dtype compress)")
+    if getattr(e, "dtype", None) != torch.float32 or not getattr(e, "is_cuda", False) or e.device != t.device \
+            or e.shape != t.shape or not e.is_contiguous():
+        raise ValueError(f"{what}: error_feedback must be a contiguous float32 CUDA tensor shaped like t "
+                         f"({tuple(t.shape)} on {t.device}); got {getattr(e, 'dtype', type(e))} "
+                         f"{tuple(getattr(e, 'shape', ()))} on {getattr(e, 'device', None)}")
+    if e.numel() and e.data_ptr() % 16 != t.data_ptr() % 16:
+        raise ValueError(f"{what}: error_feedback must start at t's address modulo 16 ({t.data_ptr() % 16} B), "
+                         f"not {e.data_ptr() % 16} B")
+    if e.numel() and e.data_ptr() < t.data_ptr() + 4 * t.numel() and t.data_ptr() < e.data_ptr() + 4 * e.numel():
+        raise ValueError(f"{what}: error_feedback overlaps t")
+
+
+def _feedback_step(x: torch.Tensor, e: torch.Tensor, wire_dtype: torch.dtype) -> torch.Tensor:
+    """The error-feedback step in torch, for the words no compress kernel takes: returns y = x + e and overwrites e
+    with the residual torch.where(w.isfinite(), y - w.float(), 0), w = y.to(wire_dtype) (what
+    ops.compress_data(error_feedback=) writes)."""
+    y = x + e
+    w = y.to(wire_dtype)
+    e.copy_(torch.where(w.isfinite(), y - w.float(), 0))
+    return y
+
+
 def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksum: bool = False,
                           temp_mem: Optional[torch.Tensor] = None, stages: int = 2,
                           peer: Optional[PeerWorkspace] = None, check: bool = True,
                           peer_mode: str = "auto", wire_dtype: Optional[torch.dtype] = None,
-                          sparse: bool = False) -> torch.Tensor:
+                          sparse: bool = False, error_feedback: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Every rank contributes the CUDA tensor `t` (same shape and dtype on every rank; fp16 / bf16 / fp32 go
     through the float codec, anything else through the byte codec) and receives the concatenation
     [world * t.numel()] in rank order, bit-exact.  `members` = archives per rank (the codec's parallelism
@@ -367,13 +397,23 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
     sparse=True (float16 / bfloat16 / float32 t): the archives are sparse ones (ops.compress_data(sparse=True)),
     which store no bits for +0 and -0 words, so mostly-zero tensors (ReLU activations, pruned weights) take fewer
     bytes on the wire; the result is the same, bit for bit.  NCCL / gloo transport only, and not with wire_dtype:
-    either raises ValueError before any communication."""
+    either raises ValueError before any communication.
+
+    error_feedback=e (with wire_dtype; a contiguous float32 CUDA tensor shaped like t, at t's address modulo 16):
+    the rounding error of the previous call's compress, added back before this one rounds.  The result is exactly
+    all_gather_compressed(t + e, wire_dtype=wire_dtype), and e is overwritten with this call's error,
+    torch.where(w.isfinite(), y - w.float(), 0) for y = t + e and w = y.to(wire_dtype), inside the compress kernels
+    (ops.compress_data(error_feedback=)).  This is the "server error" of the second phase of an fp32 all-reduce
+    composed as all_gather_compressed(reduce_scatter_compressed(g, wire_dtype=w, error_feedback=e_w), wire_dtype=w,
+    error_feedback=e_s).  Misuse raises ValueError before any communication."""
     _check_sparse_wire(t.dtype, "all_gather_compressed", sparse, wire_dtype, peer)
     if not t.is_cuda or not t.is_contiguous():
         raise ValueError("all_gather_compressed: contiguous CUDA tensor expected (no CPU fallback)")
     _check_wire(t, "all_gather_compressed", wire_dtype)
     if wire_dtype is not None and peer is not None:
         raise ValueError("all_gather_compressed: wire_dtype is not supported with the peer-memory transports")
+    _check_feedback("all_gather_compressed", error_feedback, t, wire_dtype)
+    ef = None if error_feedback is None else error_feedback.reshape(-1)
     as_float = t.dtype in (torch.float16, torch.bfloat16, torch.float32)
     flat = t.reshape(-1) if as_float else t.reshape(-1).view(torch.uint8)
     n = flat.numel()
@@ -399,7 +439,9 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
 
     def compress(a, b):
         comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem,
-                                           archive_dtype=wire_dtype, sparse=sparse)
+                                           archive_dtype=wire_dtype, sparse=sparse,
+                                           error_feedback=None if ef is None else
+                                           [ef[bounds[i]:bounds[i + 1]] for i in range(a, b)])
         return comp, sizes
 
     def decompress(a, b, gathered):
@@ -650,7 +692,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               scale_tensor: Optional[torch.Tensor] = None,
                               found_inf: Optional[torch.Tensor] = None,
                               out_dtype: Optional[torch.dtype] = None,
-                              sq_norm: Optional[torch.Tensor] = None) -> torch.Tensor:
+                              sq_norm: Optional[torch.Tensor] = None,
+                              error_feedback: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -703,13 +746,24 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     (ops.sq_norm's definition) of the shard's `members` pieces.  The decode-and-sum that writes the final values takes
     them in the same kernel (decompress_data_reduce(sq_norm=)); the last rank and a world of one, which finish the
     shard with torch, apply ops.sq_norm to the same pieces, so the value is the same function of the shard on every
-    path.  Misuse raises ValueError before any communication."""
+    path.  Misuse raises ValueError before any communication.
+
+    error_feedback=e (with wire_dtype; a contiguous float32 CUDA tensor shaped like t, at t's address modulo 16)
+    keeps the rounding error of the float32 -> wire_dtype compress from one step to the next instead of dropping it
+    (DeepSpeed's "worker error"): the result is exactly reduce_scatter_compressed(t + e, wire_dtype=wire_dtype, ...)
+    with every other keyword unchanged, on every rank, and all of e is overwritten with this step's error,
+    torch.where(w.isfinite(), y - w.float(), 0) for y = t + e and w = y.to(wire_dtype).  The chunks sent to other
+    ranks get their new error from the compress kernels (ops.compress_data(error_feedback=)); the own chunk, which is
+    never compressed, and a world of one or an empty t get it from that torch expression.  The error of a word that
+    rounds to inf or NaN is +0: that step carries the non-finite word (found_inf sees it), the next starts clean.
+    Misuse raises ValueError before any communication."""
     s32 = _check_scale("reduce_scatter_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sq_norm("reduce_scatter_compressed", sq_norm, scale_tensor, t.device)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
     narrow_dtype = _check_out_dtype("reduce_scatter_compressed", out_dtype, t.dtype, reduce_dtype, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
+    _check_feedback("reduce_scatter_compressed", error_feedback, t, wire_dtype)
     arch_dtype = wire_dtype or t.dtype  # the archives' (and the own chunk's) dtype
     res_dtype = narrow_dtype or acc_dtype
     world = _world(group)
@@ -720,9 +774,12 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     n = flat.numel()
     if n % world:
         raise ValueError(f"reduce_scatter_compressed: numel {n} is not divisible by the world size {world}")
+    ef = None if error_feedback is None else error_feedback.reshape(-1)
     shard = n // world
     bounds = _split(shard, max(1, int(members)), 8)
     if world == 1 or n == 0:
+        if ef is not None:
+            flat = _feedback_step(flat, ef, arch_dtype)
         if res_dtype == acc_dtype:
             res = _local_sum(flat[:shard].to(arch_dtype), acc_dtype, sd, found_inf)
         else:
@@ -734,7 +791,10 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     dests = [d for d in range(world) if d != rank]
     comp, sizes, _ = ops.compress_data(True, [flat[d * shard + bounds[i]: d * shard + bounds[i + 1]]
                                               for d in dests for i in range(m)], False, temp_mem,
-                                       archive_dtype=arch_dtype, sparse=sparse)
+                                       archive_dtype=arch_dtype, sparse=sparse,
+                                       error_feedback=None if ef is None else
+                                       [ef[d * shard + bounds[i]: d * shard + bounds[i + 1]]
+                                        for d in dests for i in range(m)])
     hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
     per_dest = [[comp.new_empty(0)] * m for _ in range(world)]  # nothing for this rank's own chunk
     for k, d in enumerate(dests):
@@ -745,7 +805,10 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     # narrowing: the later sources' call rounds the float32 sums once into res, accumulating from out
     res = out if res_dtype == acc_dtype else torch.empty(shard, dtype=res_dtype, device=dev)
     narrow = {} if res is out else dict(reduce_dtype=torch.float32, acc=outs)
-    own = flat[rank * shard:(rank + 1) * shard].to(arch_dtype)
+    own = flat[rank * shard:(rank + 1) * shard]
+    if ef is not None:
+        own = _feedback_step(own, ef[rank * shard:(rank + 1) * shard], arch_dtype)
+    own = own.to(arch_dtype)
     if sd is not None:
         own = _term(own, acc_dtype, sd)  # the kernel's term of the own chunk, already in the result's dtype
     statuses = []

@@ -439,6 +439,28 @@ int dgb_float_compress_to(void* temp, size_t tempBytes, int inFt, int ft, int pb
   return encodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev, (cudaStream_t)stream);
 }
 
+int dgb_float_compress_to_ef(void* temp, size_t tempBytes, int inFt, int ft, int pb, int useChecksum, uint32_t n,
+                             const void* const* in, const uint32_t* inSize, float* const* err, void* const* out,
+                             uint32_t* outSize_dev, void* stream) {
+  int kind;
+  if (inFt == DGB_FLOAT32 && ft == DGB_FLOAT16)
+    kind = kKindF32toF16EF;
+  else if (inFt == DGB_FLOAT32 && ft == DGB_BFLOAT16)
+    kind = kKindF32toBF16EF;
+  else
+    return DGB_ERR_INVALID_ARG;
+  if (!err) return DGB_ERR_INVALID_ARG;
+  HostMember* v = nullptr;
+  int rc = buildPointer(n, in, inSize, out, &v);
+  if (rc) return rc;
+  for (uint32_t i = 0; i < n; ++i) {
+    if (v[i].size == 0) continue;  // an empty member reads no residual (nor input)
+    if (!err[i] || ((reinterpret_cast<uintptr_t>(err[i]) ^ reinterpret_cast<uintptr_t>(v[i].in)) & 15u))
+      return DGB_ERR_INVALID_ARG;
+  }
+  return encodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev, (cudaStream_t)stream, err);
+}
+
 int dgb_float_compress_split_size(void* temp, size_t tempBytes, int ft, int pb, int useChecksum,
                                   uint32_t n, const void* in_dev, const uint32_t* splitSizes,
                                   void* out_dev, uint32_t outStride, uint32_t* outSize_dev,

@@ -119,11 +119,19 @@ enum CodecKind : int {
   // before it takes the coded and stored bytes out of it, so the archive is an ordinary fp16 / bf16 archive.
   // Encoder only: decode.cu never dispatches them.
   kKindF32toF16 = 0x40 | DGB_FLOAT16,
-  kKindF32toBF16 = 0x40 | DGB_BFLOAT16
+  kKindF32toBF16 = 0x40 | DGB_BFLOAT16,
+  // The same with error feedback (dgb_float_compress_to_ef), 0x80 | the narrowing kind: each word is y = x + e, with
+  // e the member's float32 residual word, and the coder overwrites e with y - float(round(y)) (+0 where the rounded
+  // word is not finite).  Encoder only, never on the wire; their kernels also take the residual table (EfMembers).
+  kKindF32toF16EF = 0x80 | kKindF32toF16,
+  kKindF32toBF16EF = 0x80 | kKindF32toBF16
 };
-__host__ __device__ constexpr bool isNarrowKind(int k) { return k == kKindF32toF16 || k == kKindF32toBF16; }
+__host__ __device__ constexpr bool isEfKind(int k) { return k == kKindF32toF16EF || k == kKindF32toBF16EF; }
+__host__ __device__ constexpr bool isNarrowKind(int k) {
+  return k == kKindF32toF16 || k == kKindF32toBF16 || isEfKind(k);
+}
 // the float type a kind's archives carry (header, size bound, plane layout, table format)
-__host__ __device__ constexpr int archiveKind(int k) { return isNarrowKind(k) ? (k & ~0x40) : k; }
+__host__ __device__ constexpr int archiveKind(int k) { return isNarrowKind(k) ? (k & ~0xc0) : k; }
 
 struct MemberDesc {
   const void* in;     // encode: raw input (bytes / float words); decode: archive
@@ -149,6 +157,17 @@ __device__ __forceinline__ MemberDesc memberAt(const InlineMembers& im, const Me
 __device__ __forceinline__ uint32_t memberWork0(const InlineMembers& im, const MemberDesc* global, uint32_t i) {
   return im.count ? im.m[i].work0 : __ldg(&global[i].work0);
 }
+
+// The residual buffers of the error-feedback kinds, member by member.  Only their kernels take this table, so the
+// member table every other kernel receives keeps its layout.  Up to kInlineMembers pointers travel inside the
+// kernel parameters (when the member table does); otherwise `global` is a copy in the scratch, uploaded with the
+// member table (uploadTable), so no host memory is read after the call returns.
+struct EfMembers {
+  float* const* global;  // used when count == 0
+  uint32_t count;
+  float* e[kInlineMembers];
+};
+__device__ __forceinline__ float* efAt(const EfMembers& ef, uint32_t i) { return ef.count ? ef.e[i] : ef.global[i]; }
 
 // ---- encoder symbol table entry (one per symbol, 8 B, shared memory) -------
 // magic = ceil(2^(32+shift)/pdf): state / pdf == hi32(state * magic) >> shift for state < 2^31
@@ -200,9 +219,10 @@ struct HostMember {
   uint32_t size;  // see MemberDesc::size
 };
 
+// err: the error-feedback kinds' residual buffers, one per member (nullptr for every other kind)
 int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, uint32_t n,
                 const HostMember* members, const uint32_t* histogram_dev, uint32_t* outSize_dev,
-                cudaStream_t stream);
+                cudaStream_t stream, float* const* err = nullptr);
 int decodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, uint32_t n,
                 const HostMember* members, uint8_t* outSuccess_dev, uint32_t* outSize_dev,
                 uint8_t* mismatchHost, cudaStream_t stream);

@@ -1,5 +1,5 @@
 // encode.cu -- batched rANS encode (bytes) and float compress (fp16/bf16/fp32/fp64, sparse fp16/bf16/fp32, and
-// float32 inputs narrowed to fp16/bf16 archives)
+// float32 inputs narrowed to fp16/bf16 archives, with or without error feedback)
 // for sm_90a (H100).  Two launches per call, whatever the batch size:
 //
 //   K1  stats*Kernel     a pure read of the raw input: 256-bin histogram of the coded byte, taken out of
@@ -366,7 +366,7 @@ __device__ __forceinline__ void histAdd(uint32_t* wh, uint32_t byteOff) {
 template <int KIND>
 __device__ __forceinline__ uint32_t narrowPair(uint32_t lo, uint32_t hi) {
   uint32_t r;
-  if (KIND == kKindF32toF16)
+  if (archiveKind(KIND) == DGB_FLOAT16)
     asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
   else
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
@@ -377,6 +377,27 @@ __device__ __forceinline__ uint32_t narrowPair(uint32_t lo, uint32_t hi) {
 template <int KIND>
 __device__ __forceinline__ uint32_t narrowWord(uint32_t w) {
   return narrowPair<KIND>(w, 0u);
+}
+
+// ---- error feedback (the EF kinds) ----
+// y = x + e: one round-to-nearest fp32 add, subnormals kept (torch's CUDA add); __fadd_rn never joins a multiply
+__device__ __forceinline__ uint32_t efSum(uint32_t x, uint32_t e) {
+  return __float_as_uint(__fadd_rn(__uint_as_float(x), __uint_as_float(e)));
+}
+// The residual of y whose rounded 16-bit word is h (bits 0..15): y - float(h), exact for a finite h, and +0 when h
+// is inf or NaN, so that one overflow or one non-finite gradient does not poison every later step.
+template <int KIND>
+__device__ __forceinline__ uint32_t efResidual(uint32_t y, uint32_t h) {
+  float wf;
+  bool finite;
+  if constexpr (archiveKind(KIND) == DGB_FLOAT16) {
+    asm("cvt.f32.f16 %0, %1;" : "=f"(wf) : "h"((unsigned short)h));
+    finite = (h & 0x7c00u) != 0x7c00u;
+  } else {
+    wf = __uint_as_float(h << 16);
+    finite = (h & 0x7f80u) != 0x7f80u;
+  }
+  return finite ? __float_as_uint(__fsub_rn(__uint_as_float(y), wf)) : 0u;
 }
 
 template <int FT>
@@ -390,23 +411,42 @@ __device__ __forceinline__ uint32_t codedScalar(const uint8_t* in, uint32_t e) {
   const uint32_t w = reinterpret_cast<const uint16_t*>(in)[e];
   return FT == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8;
 }
+// EF kinds: the rounded word of y = x + e (statistics pass: e is read, never written)
+template <int FT>
+__device__ __forceinline__ uint32_t efWordScalar(const uint8_t* in, const float* err, uint32_t e) {
+  return narrowWord<FT>(efSum(reinterpret_cast<const uint32_t*>(in)[e], __float_as_uint(err[e])));
+}
+template <int FT>
+__device__ __forceinline__ uint32_t codedScalarEf(const uint8_t* in, const float* err, uint32_t e) {
+  const uint32_t w = efWordScalar<FT>(in, err, e);
+  return archiveKind(FT) == DGB_BFLOAT16 ? (w >> 7) & 0xffu : w >> 8;
+}
 
 // The vector body of a float statistics slab: vectors [v0, v1) of the member, 16 B each: a pure
 // read (the coder takes the coded byte out of the raw words itself and writes the stored planes).
+// EF kinds: `evec` is the member's residual words, vector for vector beside `vec` (same address mod 16), and the
+// words counted are round(x + e).
 template <int FT, bool STAGED>
 __device__ __forceinline__ void histVectors(const uint4* __restrict__ vec, const StatsStage& stage, uint32_t v0,
-                                            uint32_t v1, uint32_t t, uint32_t* wh) {
+                                            uint32_t v1, uint32_t t, uint32_t* wh,
+                                            const uint4* __restrict__ evec = nullptr) {
   for (uint32_t i0 = v0 + t; i0 < v1; i0 += kStatsUnroll * kStatsThreads) {
     uint4 vv[kStatsUnroll];
+    [[maybe_unused]] uint4 ev[kStatsUnroll];
 #pragma unroll
     for (int k = 0; k < kStatsUnroll; ++k) {
       const uint32_t i = i0 + k * kStatsThreads;
       vv[k] = i < v1 ? (STAGED ? stage.buf[i - v0] : ldStream16(vec + i)) : make_uint4(0, 0, 0, 0);
+      if constexpr (isEfKind(FT)) ev[k] = i < v1 ? ldStream16(evec + i) : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int k = 0; k < kStatsUnroll; ++k) {
       const uint32_t i = i0 + k * kStatsThreads;
       if (i >= v1) break;
+      if constexpr (isEfKind(FT)) {
+        vv[k] = make_uint4(efSum(vv[k].x, ev[k].x), efSum(vv[k].y, ev[k].y), efSum(vv[k].z, ev[k].z),
+                           efSum(vv[k].w, ev[k].w));
+      }
       if constexpr (isNarrowKind(FT)) {  // four float32 words -> two packed pairs of the archive type
         constexpr int AT = archiveKind(FT);
         const uint32_t p0 = narrowPair<FT>(vv[k].x, vv[k].y), p1 = narrowPair<FT>(vv[k].z, vv[k].w);
@@ -646,7 +686,8 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
                                                bool useChecksum, uint32_t slabVecs, const MemberDesc& md,
                                                uint32_t m, uint32_t y,
                                                uint32_t Y, uint32_t* __restrict__ outSize,
-                                               const StatsStage& stage = StatsStage()) {
+                                               const StatsStage& stage = StatsStage(),
+                                               const float* __restrict__ err = nullptr) {  // EF kinds: residuals
   constexpr bool SPARSE = isSparseKind(FT);
   constexpr int BT = denseKind(FT);  // the dense type whose natural symbols the histogram counts
   constexpr bool NARROW = isNarrowKind(FT);  // float32 input words, archives of type AT
@@ -700,6 +741,8 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
         histZeroVectors32(vec, v0, v1, t, wh, head, blockZeros(sc, md.work0), pz, nz);
       else if constexpr (SPARSE)
         histZeroVectors<BT>(vec, v0, v1, t, wh, head, blockZeros(sc, md.work0), pz, nz);
+      else if constexpr (isEfKind(FT))  // err has in's address mod 16, so its vectors start at the same element
+        histVectors<FT, STAGED>(vec, stage, v0, v1, t, wh, reinterpret_cast<const uint4*>(err + head));
       else
         histVectors<FT, STAGED>(vec, stage, v0, v1, t, wh);
     }
@@ -744,8 +787,13 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
     } else if (y == 0) {
       // ---- scalar head and tail (fewer than one vector each) ----
       const uint32_t tailStart = head + nVec * EPV;
-      if (t < head) atomicAdd(&wh[codedScalar<FT>(in, t)], 1u);
-      if (t < size - tailStart) atomicAdd(&wh[codedScalar<FT>(in, tailStart + t)], 1u);
+      if constexpr (isEfKind(FT)) {
+        if (t < head) atomicAdd(&wh[codedScalarEf<FT>(in, err, t)], 1u);
+        if (t < size - tailStart) atomicAdd(&wh[codedScalarEf<FT>(in, err, tailStart + t)], 1u);
+      } else {
+        if (t < head) atomicAdd(&wh[codedScalar<FT>(in, t)], 1u);
+        if (t < size - tailStart) atomicAdd(&wh[codedScalar<FT>(in, tailStart + t)], 1u);
+      }
       // float header (float/GpuFloatCompress.cuh:324-337) and zero padding of the planes
       if (t == 0) {
         // float-level checksum is patched in by the epilogue CTA
@@ -765,7 +813,11 @@ __device__ __forceinline__ bool statsFloatItem(const EncodeScratch& sc, uint32_t
         for (uint32_t i = size + t; i < nonBytes; i += kStatsThreads) non[i] = 0;
       }
     }
-    if (NARROW && useChecksum) {
+    if (isEfKind(FT) && useChecksum) {  // the rounded words of y = x + e
+      for (uint32_t j = y * kStatsThreads + t; j < (size >> 1); j += participants * kStatsThreads)
+        xorAcc ^= efWordScalar<FT>(in, err, j);
+      if ((size & 1u) && y == 0 && t == 0) xorAcc ^= efWordScalar<FT>(in, err, size >> 1) & 0xffu;
+    } else if (NARROW && useChecksum) {
       // the same rule over the ROUNDED data: its first size / 2 16-bit words, then the low byte of the next
       // one when size is odd (foldXor folds both bytes of a word into the byte checksum)
       const uint32_t* in32 = reinterpret_cast<const uint32_t*>(in);
@@ -811,6 +863,17 @@ statsFloatKernel(EncodeScratch sc, const __grid_constant__ InlineMembers im, int
   const uint32_t m = blockIdx.x + memberBase;
   statsFloatItem<FT, false>(sc, sHist, pb, useChecksum, slabVecs, memberAt(im, sc.members, m), m, blockIdx.y, gridDim.y,
                             outSize);
+}
+
+// K1 of the EF kinds: statsFloatKernel plus the residual table (read only: the coder overwrites the residuals)
+template <int FT>
+__global__ void __launch_bounds__(kStatsThreads)
+statsFloatEfKernel(EncodeScratch sc, const __grid_constant__ InlineMembers im, const __grid_constant__ EfMembers ef,
+                   int pb, bool useChecksum, uint32_t slabVecs, uint32_t memberBase, uint32_t* __restrict__ outSize) {
+  __shared__ uint32_t sHist[kStatsWarps][kNumSymbols];
+  const uint32_t m = blockIdx.x + memberBase;
+  statsFloatItem<FT, false>(sc, sHist, pb, useChecksum, slabVecs, memberAt(im, sc.members, m), m, blockIdx.y, gridDim.y,
+                            outSize, StatsStage(), efAt(ef, m));
 }
 
 // K1 with the slab landed in shared memory by one TMA bulk copy per CTA (option stats_stage): the
@@ -872,6 +935,7 @@ struct StoredPlanes {
   // sparse kinds: `non` holds the kept words' bytes, block k's from table[k] on
   const uint32_t* table;
   uint32_t keepAll;  // 1: nothing is elided (esc == 0), every word stores its byte
+  float* err;        // EF kinds: the member's residual words (indexed like the member's elements)
 };
 
 template <int KIND>
@@ -1087,6 +1151,62 @@ struct EncInNarrow : EncIn16<archiveKind(KIND)> {
 };
 template <> struct EncIn<kKindF32toF16> : EncInNarrow<kKindF32toF16> {};
 template <> struct EncIn<kKindF32toBF16> : EncInNarrow<kKindF32toBF16> {};
+
+// Error-feedback kinds: the narrowing kind's coder on y = x + e.  storeGroup runs on a ring slot before encodeGroup
+// reads it; here it also loads the residual vectors beside the slot's input vectors, forms y, writes y back over x in
+// the slot (so the narrowing tabOffset codes round(y)), stores round(y)'s stored bytes and writes each residual
+// y - float(round(y)) over e.  The scalar paths do the same per word (loadWordEf).  Every element is visited once,
+// by one lane, which reads its e before it writes e'.  The ring is the cp.async one only: a TMA bulk copy into a slot
+// these generic-proxy stores have written would need a proxy fence first (encodeMemberBlocks).
+template <int KIND>
+struct EncInNarrowEf : EncInNarrow<KIND & ~0x80> {
+  static constexpr int NK = KIND & ~0x80;  // the narrowing kind
+  static constexpr int AT = archiveKind(KIND);
+  static __device__ __forceinline__ void storeGroup(uint32_t slot, const StoredPlanes& pl, uint32_t elem0,
+                                                    uint32_t lane) {
+    float4* ep = reinterpret_cast<float4*>(pl.err + elem0);
+    uint4 ev[4];
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {  // all four residual loads in flight before the first is used
+      const float4 f = __ldcs(ep + lane + 32u * h);
+      ev[h] = make_uint4(__float_as_uint(f.x), __float_as_uint(f.y), __float_as_uint(f.z), __float_as_uint(f.w));
+    }
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const uint32_t v = lane + 32u * h;
+      uint4 x;
+      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w) : "r"(slot + v * 16u));
+      const uint4 y = make_uint4(efSum(x.x, ev[h].x), efSum(x.y, ev[h].y), efSum(x.z, ev[h].z), efSum(x.w, ev[h].w));
+      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(slot + v * 16u), "r"(y.x), "r"(y.y), "r"(y.z), "r"(y.w)
+                   : "memory");
+      const uint32_t p0 = narrowPair<NK>(y.x, y.y), p1 = narrowPair<NK>(y.z, y.w);
+      *reinterpret_cast<uint32_t*>(pl.non + elem0 + v * 4u) = __byte_perm(rot16x2<AT>(p0), rot16x2<AT>(p1), 0x6420);
+      __stcs(ep + v, make_float4(__uint_as_float(efResidual<KIND>(y.x, p0 & 0xffffu)),
+                                 __uint_as_float(efResidual<KIND>(y.y, p0 >> 16)),
+                                 __uint_as_float(efResidual<KIND>(y.z, p1 & 0xffffu)),
+                                 __uint_as_float(efResidual<KIND>(y.w, p1 >> 16))));
+    }
+    __syncwarp();  // encodeGroup's lanes read words other lanes have just written
+  }
+  // one word of the scalar paths: element e of the block, whose residual is err[e]; returns round(y)
+  static __device__ __forceinline__ uint32_t loadWordEf(const uint8_t* in, uint32_t e, float* err) {
+    const uint32_t y = efSum(__ldg(reinterpret_cast<const uint32_t*>(in) + e), __float_as_uint(err[e]));
+    const uint32_t w = narrowWord<NK>(y);
+    err[e] = __uint_as_float(efResidual<KIND>(y, w));
+    return w;
+  }
+};
+template <> struct EncIn<kKindF32toF16EF> : EncInNarrowEf<kKindF32toF16EF> {};
+template <> struct EncIn<kKindF32toBF16EF> : EncInNarrowEf<kKindF32toBF16EF> {};
+
+// the word the scalar paths code: EF kinds also form y and write its residual
+template <int KIND>
+__device__ __forceinline__ auto encLoadWord(const uint8_t* in, uint32_t e, const StoredPlanes& pl, uint32_t elem0) {
+  if constexpr (isEfKind(KIND))
+    return EncIn<KIND>::loadWordEf(in, e, pl.err + elem0);
+  else
+    return EncIn<KIND>::loadWord(in, e);
+}
 
 // Sparse fp32: a +0 / -0 word looks up table entry 256 / 257, every other word its exponent symbol.  The kept words'
 // 16 + 8 stored bits are compacted into the u16 and u8 planes in element order.  A group of 16 rows (512 words in the
@@ -1493,6 +1613,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   // groups in flight ahead of the one being coded: two, or one in a two-slot ring
   constexpr uint32_t kAhead = In::kRingSlots > 2 ? 2u : 1u;
   static_assert(In::kRingSlots >= 2 && (!TMA || kAhead == 2), "");
+  static_assert(!TMA || !isEfKind(KIND), "the EF kinds write their ring slots: cp.async ring only");
   constexpr bool kSparse = isSparseKind(KIND);
   uint32_t state = kStateMin;
   uint32_t wa = stageAddr;
@@ -1581,7 +1702,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   uint32_t e = r * 32u + lane;
   for (uint32_t j = 0; r < fullRows; ++r, ++j, e += 32) {
     if (sp.area && (j % U) == 0 && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
-    const auto w = In::loadWord(in, e);
+    const auto w = encLoadWord<KIND>(in, e, planes, elem0);
     if constexpr (kSparse)
       In::storeRow(planes, pcur, w, true, rc.ltMask);
     else
@@ -1592,7 +1713,7 @@ __device__ __forceinline__ uint32_t encodeBlockWarp(const uint8_t* __restrict__ 
   if (rem) {
     if (sp.area && wa - stageAddr > sp.limitBytes) spillOut(sp, stageAddr, stage, wa, lane);
     const bool valid = lane < rem;
-    const auto w = valid ? In::loadWord(in, e) : 0u;
+    const auto w = valid ? encLoadWord<KIND>(in, e, planes, elem0) : 0u;
     if constexpr (kSparse)
       In::storeRow(planes, pcur, w, valid, rc.ltMask);
     else if (valid)
@@ -1674,10 +1795,11 @@ __device__ __forceinline__ uint32_t sparsePlanes(void* out, uint32_t size, Store
   }
 }
 
+// The body of encodeKernel; `ef` is the EF kinds' residual table (nullptr for every other kind)
 template <int KIND>
-__global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
-                             uint32_t numMembers, uint32_t totalTickets,
-                             uint32_t* __restrict__ outSize) {
+__device__ __forceinline__ void encodeCanonical(const EncodeScratch& sc, int pb, bool useChecksum, uint32_t numMembers,
+                                                uint32_t totalTickets, uint32_t* __restrict__ outSize,
+                                                const EfMembers* ef) {
   constexpr int kind = KIND;
   extern __shared__ __align__(16) uint8_t smem[];
   const uint32_t t = threadIdx.x, lane = t & 31u;
@@ -1713,6 +1835,7 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
     uint8_t* ansOut;
     uint32_t extraBytes = 0;
     StoredPlanes planes{nullptr, nullptr, nullptr};
+    if constexpr (isEfKind(KIND)) planes.err = efAt(*ef, m);
     ansIn = static_cast<const uint8_t*>(md.in);
     if (kind == kKindBytes) {
       ansOut = static_cast<uint8_t*>(md.out);
@@ -1790,6 +1913,20 @@ __global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
   }
 }
 
+template <int KIND>
+__global__ void encodeKernel(EncodeScratch sc, int pb, bool useChecksum,
+                             uint32_t numMembers, uint32_t totalTickets,
+                             uint32_t* __restrict__ outSize) {
+  encodeCanonical<KIND>(sc, pb, useChecksum, numMembers, totalTickets, outSize, nullptr);
+}
+
+// the canonical K2 of the EF kinds: encodeKernel plus the residual table
+template <int KIND>
+__global__ void encodeKernelEf(EncodeScratch sc, const __grid_constant__ EfMembers ef, int pb, bool useChecksum,
+                               uint32_t numMembers, uint32_t totalTickets, uint32_t* __restrict__ outSize) {
+  encodeCanonical<KIND>(sc, pb, useChecksum, numMembers, totalTickets, outSize, &ef);
+}
+
 // ---------------------------------------------------------------------------
 // K2, default flavour: no inter-block dependency at all.  The archive format
 // addresses every block's stream through blockWords[k].y, so streams may sit in
@@ -1861,7 +1998,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
                                                    uint32_t first, uint32_t last, int pb,
                                                    bool useChecksum, uint32_t tabAddr, WarpSmem& ws,
                                                    uint32_t warp, uint32_t W, uint32_t lane,
-                                                   uint32_t* __restrict__ outSize) {
+                                                   uint32_t* __restrict__ outSize, float* err = nullptr) {
   constexpr int kind = KIND;
   const uint32_t size = md.size;
   const uint32_t nb = divUp(size, kBlockBytes);
@@ -1869,6 +2006,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
   uint8_t* ansOut;
   uint32_t extraBytes = 0;
   StoredPlanes planes{nullptr, nullptr, nullptr};
+  if constexpr (isEfKind(KIND)) planes.err = err;
   ansIn = static_cast<const uint8_t*>(md.in);
   if (kind == kKindBytes) {
     ansOut = static_cast<uint8_t*>(md.out);
@@ -1899,7 +2037,7 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
     const uint32_t start = block * kBlockBytes;
     const uint32_t blockLen = min(kBlockBytes, size - start);
     uint32_t state;
-    const uint32_t words = encodeBlockWarp<WIDE, KIND, kEncTma>(ansIn + (size_t)start * EncIn<KIND>::kWordBytes, blockLen, start,
+    const uint32_t words = encodeBlockWarp<WIDE, KIND, kEncTma && !isEfKind(KIND)>(ansIn + (size_t)start * EncIn<KIND>::kWordBytes, blockLen, start,
                                                                 planes, tabAddr, pb, ws.stageAddr, ws.stage, ws.sp, ws.ringAddr,
                                                                 lane, state, ws.ringBar, &ws.ringPhase);
     const uint32_t padded = roundUp(words, 8u);
@@ -1928,12 +2066,12 @@ __device__ __forceinline__ void encodeMemberBlocks(const EncodeScratch& sc, cons
   }
 }
 
+// The body of encodeKernelFast; `ef` is the EF kinds' residual table (nullptr for every other kind)
 template <bool WIDE, int KIND>
-__global__ void
-encodeKernelFast(EncodeScratch sc, const __grid_constant__ InlineMembers im, int pb, bool useChecksum,
-                                 uint32_t numMembers, uint32_t blockBegin, uint32_t blockEnd,
-                                 uint32_t slotWords, uint32_t spillWarpBase,
-                                 uint32_t* __restrict__ outSize) {
+__device__ __forceinline__ void encodeFast(const EncodeScratch& sc, const InlineMembers& im, int pb, bool useChecksum,
+                                           uint32_t numMembers, uint32_t blockBegin, uint32_t blockEnd,
+                                           uint32_t slotWords, uint32_t spillWarpBase, uint32_t* __restrict__ outSize,
+                                           const EfMembers* ef) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(16) uint4 sTab[encTabVecs(WIDE, KIND)];  // static: constant base for the hot LDS
   __shared__ uint32_t sMember;
@@ -1968,11 +2106,35 @@ encodeKernelFast(EncodeScratch sc, const __grid_constant__ InlineMembers im, int
     const uint32_t memberEnd = min(end, md.work0 + nb);
     loadTable<WIDE, KIND>(sc, sTab, m);
     __syncthreads();
-    encodeMemberBlocks<WIDE, KIND>(sc, md, m, cur - md.work0, memberEnd - md.work0, pb, useChecksum, tabAddr, ws,
-                                   warp, W, lane, outSize);
+    if constexpr (isEfKind(KIND))
+      encodeMemberBlocks<WIDE, KIND>(sc, md, m, cur - md.work0, memberEnd - md.work0, pb, useChecksum, tabAddr, ws,
+                                     warp, W, lane, outSize, efAt(*ef, m));
+    else
+      encodeMemberBlocks<WIDE, KIND>(sc, md, m, cur - md.work0, memberEnd - md.work0, pb, useChecksum, tabAddr, ws,
+                                     warp, W, lane, outSize);
     cur = memberEnd;
     __syncthreads();  // table is replaced for the next member
   }
+}
+
+template <bool WIDE, int KIND>
+__global__ void
+encodeKernelFast(EncodeScratch sc, const __grid_constant__ InlineMembers im, int pb, bool useChecksum,
+                                 uint32_t numMembers, uint32_t blockBegin, uint32_t blockEnd,
+                                 uint32_t slotWords, uint32_t spillWarpBase,
+                                 uint32_t* __restrict__ outSize) {
+  encodeFast<WIDE, KIND>(sc, im, pb, useChecksum, numMembers, blockBegin, blockEnd, slotWords, spillWarpBase, outSize,
+                         nullptr);
+}
+
+// K2 of the EF kinds: encodeKernelFast plus the residual table
+template <bool WIDE, int KIND>
+__global__ void
+encodeKernelFastEf(EncodeScratch sc, const __grid_constant__ InlineMembers im, const __grid_constant__ EfMembers ef,
+                   int pb, bool useChecksum, uint32_t numMembers, uint32_t blockBegin, uint32_t blockEnd,
+                   uint32_t slotWords, uint32_t spillWarpBase, uint32_t* __restrict__ outSize) {
+  encodeFast<WIDE, KIND>(sc, im, pb, useChecksum, numMembers, blockBegin, blockEnd, slotWords, spillWarpBase, outSize,
+                         &ef);
 }
 
 // ---------------------------------------------------------------------------
@@ -2167,6 +2329,8 @@ int withEncodeKind(int kind, F&& f) {
   switch (kind) {
     case kKindF32toF16: return f(IntC<kKindF32toF16>{});
     case kKindF32toBF16: return f(IntC<kKindF32toBF16>{});
+    case kKindF32toF16EF: return f(IntC<kKindF32toF16EF>{});
+    case kKindF32toBF16EF: return f(IntC<kKindF32toBF16EF>{});
     default: return withKind(kind, f);
   }
 }
@@ -2187,10 +2351,11 @@ size_t encodeTempBytes(int kind, uint32_t n, uint32_t maxSize) {
 
 int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, uint32_t n,
                 const HostMember* members, const uint32_t* histogram_dev, uint32_t* outSize_dev,
-                cudaStream_t stream) {
+                cudaStream_t stream, float* const* err) {
   if (n == 0) return DGB_OK;
   if (pb < 9 || pb > 11) return DGB_ERR_INVALID_ARG;
   if (kind != kKindBytes && histogram_dev) return DGB_ERR_INVALID_ARG;
+  if (isEfKind(kind) != (err != nullptr)) return DGB_ERR_INVALID_ARG;
   const Options opt = options();  // one snapshot per call
   const uint32_t W = (uint32_t)std::max(1, std::min(opt.encode_warps, 8));  // warps per CTA (two-kernel path)
   const uint32_t elemBytes = wordBytes(kind);
@@ -2248,6 +2413,11 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     if (tickets > 0x7fffffffull || items > 0x7fffffffull) return DGB_ERR_TOO_LARGE;
   }
   workIdx[n] = make_uint2((uint32_t)items, (uint32_t)chunks);
+  if (err) {
+    // the EF kinds never run the fused launch: their residual table takes its work index's place (8 n <= 8 (n + 1) B)
+    float** et = reinterpret_cast<float**>(hs.encodeUpload.data() + idxOff);
+    for (uint32_t i = 0; i < n; ++i) et[i] = err[i];
+  }
   const uint32_t totalTickets = (uint32_t)tickets;
   const ScratchPlan sp = planScratch(kind, n, maxSize, totalTickets, spillWarpBound(n, tickets));
   if (!temp || tempBytes < sp.total || (reinterpret_cast<uintptr_t>(temp) & 255u))
@@ -2273,6 +2443,11 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
   static thread_local InlineMembers im;
   const bool inlined = opt.inline_members != 0 && n <= kInlineMembers && !fused && !canonical && !stagedK1;
   im.count = inlined ? n : 0u;
+  // EF kinds: the residual table goes where the member table goes
+  static thread_local EfMembers ef;
+  ef.global = reinterpret_cast<float* const*>(base + sp.workIdx);
+  ef.count = err && inlined ? n : 0u;
+  if (err && inlined) std::memcpy(ef.e, err, sizeof(float*) * (size_t)n);
   if (inlined) {
     std::memcpy(im.m, desc, descBytes);
   } else {
@@ -2330,7 +2505,11 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
     constexpr int KIND = decltype(K)::value;
     constexpr bool WIDE = decltype(WD)::value;
     // K2: the canonical coder (ordered, packed table; wideTable is false) or the fast coder
-    const void* coder = canonical ? (const void*)encodeKernel<KIND> : (const void*)encodeKernelFast<WIDE, KIND>;
+    const void* coder;
+    if constexpr (isEfKind(KIND))
+      coder = canonical ? (const void*)encodeKernelEf<KIND> : (const void*)encodeKernelFastEf<WIDE, KIND>;
+    else
+      coder = canonical ? (const void*)encodeKernel<KIND> : (const void*)encodeKernelFast<WIDE, KIND>;
     int perSm = 1;
     int rc = residentCtasPerSm(coder, (int)(W * 32), smemBytes, 200 * 1024, &perSm);
     if (rc != DGB_OK) return rc;
@@ -2360,6 +2539,8 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
       timerBegin(opt, kSlotStats, ps);
       if constexpr (KIND == kKindBytes) {
         statsBytesKernel<<<grid1, kStatsThreads, 0, ps>>>(sc, im, histogram_dev, pb, checksum, slabVecs, m0, outSize_dev);
+      } else if constexpr (isEfKind(KIND)) {
+        statsFloatEfKernel<KIND><<<grid1, kStatsThreads, 0, ps>>>(sc, im, ef, pb, checksum, slabVecs, m0, outSize_dev);
       } else if constexpr (isSparseKind(KIND) || isNarrowKind(KIND)) {
         statsFloatKernel<KIND><<<grid1, kStatsThreads, 0, ps>>>(sc, im, pb, checksum, slabVecs, m0, outSize_dev);
       } else if (stagedK1 && gridY * (uint64_t)slabVecsK1 >= maxVecs) {
@@ -2381,15 +2562,23 @@ int encodeBatch(int kind, void* temp, size_t tempBytes, int pb, bool checksum, u
       timerBegin(opt, kSlotEncode, ps);
       if (canonical) {
         const uint32_t grid2 = std::min<uint32_t>(divUp(totalTickets, W), (uint32_t)resident);
-        encodeKernel<KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, pb, checksum, n, totalTickets, outSize_dev);
+        if constexpr (isEfKind(KIND))
+          encodeKernelEf<KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, ef, pb, checksum, n, totalTickets, outSize_dev);
+        else
+          encodeKernel<KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, pb, checksum, n, totalTickets, outSize_dev);
       } else {
         // one resident wave, equal rounds per warp (see launchPlanDecode)
         const uint64_t rounds = std::max<uint64_t>(1, (partBlocks + resident * W - 1) / (resident * W));
         const uint64_t want = ((uint64_t)partBlocks + W * rounds - 1) / (W * rounds);
         uint32_t grid2 = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(want, resident));
         grid2 = std::max(1u, std::min(grid2, spillWarpsPerPart / W));  // every warp owns a spill slot
-        encodeKernelFast<WIDE, KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, im, pb, checksum, n, blockBegin, blockEnd, slotWords,
-                                                                      (uint32_t)part * spillWarpsPerPart, outSize_dev);
+        if constexpr (isEfKind(KIND))
+          encodeKernelFastEf<WIDE, KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, im, ef, pb, checksum, n, blockBegin, blockEnd,
+                                                                          slotWords, (uint32_t)part * spillWarpsPerPart,
+                                                                          outSize_dev);
+        else
+          encodeKernelFast<WIDE, KIND><<<grid2, W * 32, smemBytes, ps>>>(sc, im, pb, checksum, n, blockBegin, blockEnd, slotWords,
+                                                                        (uint32_t)part * spillWarpsPerPart, outSize_dev);
       }
       DGB_CUDA_TRY(cudaGetLastError());
       timerEnd(opt, kSlotEncode, ps);

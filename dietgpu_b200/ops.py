@@ -184,14 +184,28 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
                   temp_mem: Optional[torch.Tensor] = None, out_compressed: Optional[torch.Tensor] = None,
                   out_compressed_bytes: Optional[torch.Tensor] = None, *,
                   prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False,
-                  archive_dtype: Optional[torch.dtype] = None):
+                  archive_dtype: Optional[torch.dtype] = None,
+                  error_feedback: Optional[Sequence[torch.Tensor]] = None):
     """archive_dtype (float16 / bfloat16, with float32 inputs): narrowing compress (dgb_float_compress_to).
     Every member's archive is exactly the archive of t.to(archive_dtype) (torch's CUDA cast), with rows sized by
     that type's bound, and no 16-bit temporary is made.  None, or the inputs' dtype, is the ordinary call; any
-    other combination raises ValueError."""
+    other combination raises ValueError.
+
+    error_feedback=[e_0, ...] (narrowing compress only; dgb_float_compress_to_ef): one contiguous float32 CUDA
+    tensor per input, with its numel, on its device and at its address modulo 16, holding the rounding error the
+    previous call left.  Member i is compressed as y = ts_in[i] + e_i (torch's add), so its archive is exactly the
+    archive of y.to(archive_dtype), and e_i is overwritten in place with
+    torch.where(w.isfinite(), y - w.float(), 0) for w = y.to(archive_dtype), bit for bit, in the same kernels.
+    Error buffers must not overlap the inputs or each other.  Any misuse raises ValueError before any device work."""
     narrow = _narrow_type(compress_as_float, ts_in, sparse, archive_dtype)
+    if error_feedback is not None and narrow is None:
+        raise ValueError("compress_data: error_feedback needs a narrowing compress (float32 inputs, archive_dtype "
+                         "float16 or bfloat16, compress_as_float=True, sparse=False); got "
+                         f"{ts_in[0].dtype if len(ts_in) else None} inputs, archive_dtype={archive_dtype}, "
+                         f"compress_as_float={compress_as_float}, sparse={sparse}")
     if narrow is not None:
-        return _compress_narrow(ts_in, narrow, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits)
+        return _compress_narrow(ts_in, narrow, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits,
+                                error_feedback)
     _check_sparse(compress_as_float, sparse)
     _check(len(ts_in) > 0, "empty batch")
     dev = ts_in[0].device
@@ -226,10 +240,47 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
     return comp, sizes, tmp.need
 
 
-def _compress_narrow(ts_in, ft: int, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits):
+def _byte_range(t: torch.Tensor) -> Tuple[int, int]:
+    return t.data_ptr(), t.data_ptr() + t.numel() * t.element_size()
+
+
+def _check_error_feedback(ts_in: Sequence[torch.Tensor], errs, others: Sequence[Optional[torch.Tensor]]) -> None:
+    """error_feedback of a narrowing compress: one float32 residual buffer per input, laid out like it (numel,
+    device, contiguity, address modulo 16), overlapping no input, no other residual buffer and none of `others`
+    (the caller's output and scratch).  Reads metadata only."""
+    if isinstance(errs, torch.Tensor) or not isinstance(errs, (list, tuple)) or len(errs) != len(ts_in):
+        raise ValueError(f"compress_data: error_feedback is a list of {len(ts_in)} tensors, one per input")
+    for i, (t, e) in enumerate(zip(ts_in, errs)):
+        if getattr(e, "dtype", None) != torch.float32 or not getattr(e, "is_cuda", False) or e.device != t.device:
+            raise ValueError(f"compress_data: error_feedback[{i}] must be a float32 CUDA tensor on {t.device}; got "
+                             f"{getattr(e, 'dtype', type(e))} on {getattr(e, 'device', None)}")
+        if e.numel() != t.numel() or not e.is_contiguous():
+            raise ValueError(f"compress_data: error_feedback[{i}] must be contiguous with {t.numel()} elements; got "
+                             f"{e.numel()} elements, contiguous={e.is_contiguous()}")
+        if e.numel() and e.data_ptr() % 16 != t.data_ptr() % 16:
+            raise ValueError(f"compress_data: error_feedback[{i}] starts at {e.data_ptr() % 16} B modulo 16, its input "
+                             f"at {t.data_ptr() % 16} B: the two must match")
+    # sweep in address order: a residual buffer may touch nothing else, inputs may overlap each other
+    spans = sorted([(*_byte_range(e), True) for e in errs if e.numel()]
+                   + [(*_byte_range(t), False) for t in list(ts_in) + [o for o in others if o is not None]
+                      if t.numel()])
+    end_any = end_err = 0
+    for lo, hi, is_err in spans:
+        if lo < (end_any if is_err else end_err):
+            raise ValueError("compress_data: an error_feedback buffer overlaps an input, the output, the scratch or "
+                             "another error_feedback buffer")
+        end_any = max(end_any, hi)
+        if is_err:
+            end_err = max(end_err, hi)
+
+
+def _compress_narrow(ts_in, ft: int, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits,
+                     error_feedback=None):
     dev = ts_in[0].device
     for t in ts_in:
         _check(t.is_cuda and t.is_contiguous() and t.device == dev and t.dtype == torch.float32)
+    if error_feedback is not None:
+        _check_error_feedback(ts_in, error_feedback, (out_compressed, temp_mem))
     n = len(ts_in)
     mx, _ = _max_numel_and_bytes(ts_in)
     L = capi.lib()
@@ -239,11 +290,12 @@ def _compress_narrow(ts_in, ft: int, checksum, temp_mem, out_compressed, out_com
     with torch.cuda.device(dev):
         need = L.dgb_float_compress_temp_bytes(ft, n, mx)
         tmp = _Temp(temp_mem, need, dev)
-        rc = L.dgb_float_compress_to(tmp.ptr, tmp.bytes, capi.FLOAT32, ft, prob_bits, int(checksum), n,
-                                     capi.ptr_array([t.data_ptr() for t in ts_in]),
-                                     capi.u32_array([t.numel() for t in ts_in]),
-                                     capi.ptr_array([comp.data_ptr() + i * row for i in range(n)]),
-                                     sizes.data_ptr(), _stream())
+        args = (capi.ptr_array([t.data_ptr() for t in ts_in]), capi.u32_array([t.numel() for t in ts_in]))
+        if error_feedback is not None:
+            args += (capi.ptr_array([e.data_ptr() for e in error_feedback]),)
+        args += (capi.ptr_array([comp.data_ptr() + i * row for i in range(n)]), sizes.data_ptr(), _stream())
+        f = L.dgb_float_compress_to if error_feedback is None else L.dgb_float_compress_to_ef
+        rc = f(tmp.ptr, tmp.bytes, capi.FLOAT32, ft, prob_bits, int(checksum), n, *args)
     capi.check(rc, "compress_data")
     return comp, sizes, tmp.need
 

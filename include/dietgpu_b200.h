@@ -194,6 +194,29 @@ int dgb_float_compress_to(void* temp_dev, size_t temp_bytes, int in_float_type, 
                           int use_checksum, uint32_t num_in_batch, const void* const* in, const uint32_t* in_size,
                           void* const* out, uint32_t* out_size_dev, void* stream);
 
+/* Narrowing compress with error feedback (new; no reference counterpart).  The allowed pairs are the narrowing
+ * ones, (DGB_FLOAT32, DGB_FLOAT16) and (DGB_FLOAT32, DGB_BFLOAT16).  err is a host array of num_in_batch device
+ * pointers: err[i] holds in_size[i] float32 residual words, one per input word.  For each input word x, its
+ * residual word e and the archive type T:
+ *   y  = x + e                            one round-to-nearest float32 add, subnormals kept (torch's CUDA add)
+ *   w  = round_T(y)                       cvt.rn.f16.f32 / cvt.rn.bf16.f32, as dgb_float_compress_to rounds
+ *   e' = y - float(w) if w is finite, else +0   (one float32 subtraction, exact for a finite w; no fused multiply-add)
+ * out[i] receives exactly the archive dgb_float_compress_to(DGB_FLOAT32, float_type, ...) writes for the words y
+ * (with encode_canonical = 1 the same bytes; by default the same fields, size and decoded words, with the streams in
+ * completion order), and the checksum option covers w.  err[i] is overwritten with e'; the input is not modified.
+ * The residual of a word that rounds to inf or NaN is +0 so that the buffer never holds an inf or a NaN: that step
+ * still carries the non-finite word, and the next starts clean.  So e' is bit for bit the torch expression
+ * torch.where(w.isfinite(), y - w.float(), 0) with y = x + e and w = y.to(T).
+ * err[i] must have the same address modulo 16 as in[i], and the err buffers must not overlap each other, any input,
+ * any output or the scratch.  A pair other than the two above, a NULL err, a NULL err[i] for a non-empty member, or
+ * an err[i] whose address modulo 16 differs from in[i]'s returns DGB_ERR_INVALID_ARG before any CUDA call, as do
+ * dgb_float_compress_to's refusals.  Scratch: dgb_float_compress_temp_bytes(float_type, n, max in_size); output
+ * bounds: dgb_float_compress_to's.  Never synchronises; capturable into a CUDA graph (a replay reads the residuals
+ * the previous replay wrote). */
+int dgb_float_compress_to_ef(void* temp_dev, size_t temp_bytes, int in_float_type, int float_type, int prob_bits,
+                             int use_checksum, uint32_t num_in_batch, const void* const* in, const uint32_t* in_size,
+                             float* const* err, void* const* out, uint32_t* out_size_dev, void* stream);
+
 /* float/GpuFloatCodec.h:141-170 / float/GpuFloatCompress.cu:103-159 floatCompressSplitSize. */
 int dgb_float_compress_split_size(void* temp_dev, size_t temp_bytes, int float_type, int prob_bits,
                                   int use_checksum, uint32_t num_in_batch, const void* in_dev,
