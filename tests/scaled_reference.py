@@ -14,6 +14,11 @@ the casts.
 
 scaled_fold_ref(words_list, archive_type, out_type, s, init=None) is the left fold of the terms with the output
 type's adds (fold_ref), after init when given; init is the running value taken in by accumulate and is not scaled.
+
+narrow_fold_ref(words_list, t, s, init32) is the narrowing decode-and-sum (dgb_float_decompress_reduce_narrow): the
+fp32 fold of the fp16 / bf16 words (scaled_fold_ref into "f32", or fold_ref for the unscaled sum, s = None), after
+the fp32 running sums init32 when given, rounded once to t.  The fp32 sum is exact in float64, so round_to rounds it
+once, as cvt.rn.f16.f32 / cvt.rn.bf16.f32 do.
 """
 from __future__ import annotations
 
@@ -40,3 +45,10 @@ def term_ref(words, archive_type, out_type, s):
 def scaled_fold_ref(words_list, archive_type, out_type, s, init=None):
     """Raw out_type words of init (unscaled, when given) + s(x_0) + s(x_1) + ..., left to right."""
     return fold_ref([term_ref(w, archive_type, out_type, s) for w in words_list], out_type, out_type, init)
+
+
+def narrow_fold_ref(words_list, t, s=None, init32=None):
+    """Raw t words of round_t((init32 or term(x_0)) + term(x_1) + ... in fp32), term unscaled when s is None."""
+    assert t in ("f16", "bf16"), t
+    f32 = fold_ref(words_list, t, "f32", init32) if s is None else scaled_fold_ref(words_list, t, "f32", s, init32)
+    return round_to(to_f64(f32, "f32"), t)
