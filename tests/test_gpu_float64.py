@@ -21,6 +21,7 @@ import torch
 
 import f64_oracle as F
 from codec_helpers import GUARD, SENTINEL, assert_guard_intact, codec_options, guarded_out
+from multirank import run_ranks
 from oracle import oracle as O
 from test_gpu_variants import VARIANTS
 
@@ -166,6 +167,12 @@ def test_variant_matches_oracle(pb, opts, role):
 
 
 def test_every_float64_instantiation_runs():
+    # in a fresh process: in a long-lived one the GPU's timestamps drift against the host clock that bounds the
+    # profiler's window, and every record of a window can fall outside it
+    run_ranks(_every_float64_instantiation_runs, 1, backend="gloo")
+
+
+def _every_float64_instantiation_runs(rank, world, dev):
     from torch.profiler import ProfilerActivity, profile
 
     from dietgpu_b200 import ops

@@ -23,6 +23,7 @@ import torch
 
 import sparse_oracle as S
 from codec_helpers import GUARD, SENTINEL, assert_guard_intact, codec_options, guarded_out
+from multirank import run_ranks
 from oracle import oracle as O
 from test_oracle_sparse import TYPES, edge_corpus, relu_words
 
@@ -157,6 +158,12 @@ def test_fallback_options_give_the_default_archives():
 
 
 def test_every_sparse_instantiation_runs():
+    # in a fresh process: in a long-lived one the GPU's timestamps drift against the host clock that bounds the
+    # profiler's window, and every record of a window can fall outside it
+    run_ranks(_every_sparse_instantiation_runs, 1, backend="gloo")
+
+
+def _every_sparse_instantiation_runs(rank, world, dev):
     from torch.profiler import ProfilerActivity, profile
 
     from dietgpu_b200 import ops

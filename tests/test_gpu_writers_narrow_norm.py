@@ -34,6 +34,7 @@ import pytest
 import torch
 
 from codec_helpers import SENTINEL, assert_guard_intact, codec_options, guarded_out
+from multirank import run_ranks
 from reduce_reference import assert_same_words, to_f64
 from scaled_reference import SCALES, narrow_fold_ref, scaled_fold_ref
 import sq_norm_reference as R
@@ -84,6 +85,12 @@ def _flag():
 # ---- a: every instantiation runs, and no kernel of another family on these paths ------------------------------------
 
 def test_profiler_sees_every_instantiation():
+    # in a fresh process: in a long-lived one the GPU's timestamps drift against the host clock that bounds the
+    # profiler's window, and every record of a window can fall outside it
+    run_ranks(_profiler_sees_every_instantiation, 1, backend="gloo")
+
+
+def _profiler_sees_every_instantiation(rank, world, dev):
     from torch.profiler import ProfilerActivity, profile
 
     from dietgpu_b200 import ops
