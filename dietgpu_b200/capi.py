@@ -16,6 +16,7 @@ OK, ERR_INVALID_ARG, ERR_TEMP_TOO_SMALL, ERR_CUDA, ERR_CHECKSUM, ERR_TOO_LARGE, 
 FLOAT16, BFLOAT16, FLOAT32, FLOAT64 = 1, 2, 3, 4  # FLOAT64: archives the reference cannot read
 FLOAT16_SPARSE, BFLOAT16_SPARSE = 5, 6  # +-0 words coded as two spare symbols; the reference cannot read these either
 FLOAT32_SPARSE = 8  # the same for float32 words (7 is unassigned)
+FLOAT8_E4M3, FLOAT8_E5M2 = 10, 11  # fp8 words: byte archives, taken by dgb_float_cast_fp8 and the fp8 sums (9 is unassigned)
 
 # every symbol include/dietgpu_b200.h declares (tests check the .so exports all of them)
 SYMBOLS = [
@@ -26,7 +27,8 @@ SYMBOLS = [
     "dgb_ans_encode_pointer", "dgb_ans_encode_stride", "dgb_ans_encode_split_size",
     "dgb_ans_decode_pointer", "dgb_ans_decode_stride", "dgb_ans_decode_split_size",
     "dgb_ans_get_compressed_info",
-    "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_to_ef", "dgb_float_compress_split_size",
+    "dgb_float_compress_pointer", "dgb_float_compress_to", "dgb_float_compress_to_ef", "dgb_float_cast_fp8",
+    "dgb_float_compress_split_size",
     "dgb_float_decompress_pointer", "dgb_float_decompress_split_size", "dgb_float_decompress_reduce",
     "dgb_float_decompress_reduce_to", "dgb_float_decompress_reduce_sparse", "dgb_float_decompress_reduce_scaled",
     "dgb_float_decompress_reduce_scaled_dev", "dgb_float_decompress_reduce_narrow",
@@ -103,6 +105,8 @@ def lib():
     L.dgb_float_compress_to.argtypes = [vp, sz, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp]
     L.dgb_float_compress_to_ef.restype = i32
     L.dgb_float_compress_to_ef.argtypes = [vp, sz, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp, vp]
+    L.dgb_float_cast_fp8.restype = i32
+    L.dgb_float_cast_fp8.argtypes = [i32, i32, u32, vp, vp, vp, vp, vp, vp]
     L.dgb_float_compress_split_size.restype = i32
     L.dgb_float_compress_split_size.argtypes = [vp, sz, i32, i32, i32, u32, vp, vp, vp, u32, vp, vp]
     L.dgb_float_decompress_pointer.restype = i32

@@ -321,12 +321,31 @@ def _split(n: int, parts: int, quantum: int) -> List[int]:
 
 
 def _check_wire(t: torch.Tensor, what: str, wire_dtype: Optional[torch.dtype]) -> None:
-    """wire_dtype: None, or float16 / bfloat16 for a float32 t (narrowing compress on the send side)."""
+    """wire_dtype: None, float16 / bfloat16 for a float32 t (narrowing compress on the send side), or an fp8 dtype for
+    a float32 or bfloat16 t (the scaled fp8 cast on the send side)."""
     if wire_dtype is None:
         return
+    if wire_dtype in ops.FP8_TYPES and t.dtype in (torch.float32, torch.bfloat16):
+        return
     if wire_dtype not in (torch.float16, torch.bfloat16) or t.dtype != torch.float32:
-        raise ValueError(f"{what}: wire_dtype is None, or float16 / bfloat16 for a float32 tensor; "
-                         f"not {wire_dtype} for {t.dtype}")
+        raise ValueError(f"{what}: wire_dtype is None, or float16 / bfloat16 for a float32 tensor, or float8_e4m3fn / "
+                         f"float8_e5m2 for a float32 or bfloat16 tensor; not {wire_dtype} for {t.dtype}")
+
+
+def _check_wire_scale(what: str, wire_scale, wire_dtype: Optional[torch.dtype], dev) -> None:
+    """wire_scale: None, or (with an fp8 wire_dtype) a one-element float32 CUDA tensor on dev."""
+    if wire_scale is None:
+        return
+    if wire_dtype not in ops.FP8_TYPES:
+        raise ValueError(f"{what}: wire_scale is the scale of an fp8 wire (wire_dtype torch.float8_e4m3fn or "
+                         f"torch.float8_e5m2), not of wire_dtype={wire_dtype}")
+    ops._check_flag_tensor(f"{what}: wire_scale", wire_scale, dev)
+
+
+def _check_fp8_wire(what: str, wire_dtype: Optional[torch.dtype], error_feedback) -> None:
+    """An fp8 wire takes no error feedback (the residual of a scaled quantiser is not the narrowing compress's)."""
+    if wire_dtype in ops.FP8_TYPES and error_feedback is not None:
+        raise ValueError(f"{what}: error_feedback is not supported with an fp8 wire_dtype")
 
 
 def _check_sparse_wire(dtype: torch.dtype, what: str, sparse: bool, wire_dtype: Optional[torch.dtype] = None,
@@ -377,7 +396,8 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
                           temp_mem: Optional[torch.Tensor] = None, stages: int = 2,
                           peer: Optional[PeerWorkspace] = None, check: bool = True,
                           peer_mode: str = "auto", wire_dtype: Optional[torch.dtype] = None,
-                          sparse: bool = False, error_feedback: Optional[torch.Tensor] = None) -> torch.Tensor:
+                          sparse: bool = False, error_feedback: Optional[torch.Tensor] = None,
+                          wire_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Every rank contributes the CUDA tensor `t` (same shape and dtype on every rank; fp16 / bf16 / fp32 go
     through the float codec, anything else through the byte codec) and receives the concatenation
     [world * t.numel()] in rank order, bit-exact.  `members` = archives per rank (the codec's parallelism
@@ -405,15 +425,24 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
     torch.where(w.isfinite(), y - w.float(), 0) for y = t + e and w = y.to(wire_dtype), inside the compress kernels
     (ops.compress_data(error_feedback=)).  This is the "server error" of the second phase of an fp32 all-reduce
     composed as all_gather_compressed(reduce_scatter_compressed(g, wire_dtype=w, error_feedback=e_w), wire_dtype=w,
-    error_feedback=e_s).  Misuse raises ValueError before any communication."""
+    error_feedback=e_s).  Misuse raises ValueError before any communication.
+
+    wire_dtype=torch.float8_e4m3fn / torch.float8_e5m2 with a float32 or bfloat16 t (fp8 parameters gathered for an
+    fp8 forward pass): every member is cast with ops.cast_fp8 at the scale wire_scale (a one-element float32 CUDA
+    tensor on t's device, the same value on every rank; None means 1) and sent as an fp8 byte archive, and the result
+    has wire_dtype and equals cat([ops.cast_fp8([t_r], wire_dtype, wire_scale)[0] for every rank r]) bit for bit.
+    NCCL / gloo transport only, and not with error_feedback; wire_scale without an fp8 wire_dtype raises ValueError."""
     _check_sparse_wire(t.dtype, "all_gather_compressed", sparse, wire_dtype, peer)
     if not t.is_cuda or not t.is_contiguous():
         raise ValueError("all_gather_compressed: contiguous CUDA tensor expected (no CPU fallback)")
     _check_wire(t, "all_gather_compressed", wire_dtype)
     if wire_dtype is not None and peer is not None:
         raise ValueError("all_gather_compressed: wire_dtype is not supported with the peer-memory transports")
+    _check_wire_scale("all_gather_compressed", wire_scale, wire_dtype, t.device)
+    _check_fp8_wire("all_gather_compressed", wire_dtype, error_feedback)
     _check_feedback("all_gather_compressed", error_feedback, t, wire_dtype)
     ef = None if error_feedback is None else error_feedback.reshape(-1)
+    fp8 = wire_dtype in ops.FP8_TYPES
     as_float = t.dtype in (torch.float16, torch.bfloat16, torch.float32)
     flat = t.reshape(-1) if as_float else t.reshape(-1).view(torch.uint8)
     n = flat.numel()
@@ -438,10 +467,11 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
     pieces = _pieces(members, max(1, min(int(stages), members)))
 
     def compress(a, b):
+        kw = dict(scale_tensor=wire_scale) if fp8 else {}  # fp8: the scaled cast, then byte archives
         comp, sizes, _ = ops.compress_data(as_float, [flat[bounds[i]:bounds[i + 1]] for i in range(a, b)], checksum, temp_mem,
                                            archive_dtype=wire_dtype, sparse=sparse,
                                            error_feedback=None if ef is None else
-                                           [ef[bounds[i]:bounds[i + 1]] for i in range(a, b)])
+                                           [ef[bounds[i]:bounds[i + 1]] for i in range(a, b)], **kw)
         return comp, sizes
 
     def decompress(a, b, gathered):
@@ -449,10 +479,11 @@ def all_gather_compressed(t: torch.Tensor, group=None, members: int = 8, checksu
         for w in range(world):
             for j, i in enumerate(range(a, b)):
                 ins.append(gathered[w][j])
-                outs.append(out[w * n + bounds[i]: w * n + bounds[i + 1]])
+                o = out[w * n + bounds[i]: w * n + bounds[i + 1]]
+                outs.append(o.view(torch.uint8) if fp8 else o)
         # gathered views are 16 B aligned inside the receive buffer; the decoder needs nothing else
         status = torch.zeros(len(ins), dtype=torch.uint8, device=t.device)
-        ops.decompress_data(as_float, ins, outs, checksum, temp_mem, status, sparse=sparse)
+        ops.decompress_data(as_float and not fp8, ins, outs, checksum, temp_mem, status, sparse=sparse)
         return status
 
     statuses = []
@@ -693,7 +724,8 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
                               found_inf: Optional[torch.Tensor] = None,
                               out_dtype: Optional[torch.dtype] = None,
                               sq_norm: Optional[torch.Tensor] = None,
-                              error_feedback: Optional[torch.Tensor] = None) -> torch.Tensor:
+                              error_feedback: Optional[torch.Tensor] = None,
+                              wire_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Like dist.reduce_scatter_tensor with a sum: t (contiguous CUDA fp16 / bf16 / fp32, t.numel() divisible by the
     world size, same shape on every rank) is cut into world chunks, and this rank returns the elementwise sum over
     ranks of chunk `rank`.  Rank r sends chunk d to rank d as `members` float archives (the same split on every
@@ -756,10 +788,24 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     ranks get their new error from the compress kernels (ops.compress_data(error_feedback=)); the own chunk, which is
     never compressed, and a world of one or an empty t get it from that torch expression.  The error of a word that
     rounds to inf or NaN is +0: that step carries the non-finite word (found_inf sees it), the next starts clean.
-    Misuse raises ValueError before any communication."""
+    Misuse raises ValueError before any communication.
+
+    wire_dtype=torch.float8_e4m3fn / torch.float8_e5m2 with a float32 or bfloat16 t (fp8 gradient communication):
+    each rank casts every element of t once with ops.cast_fp8 at the scale wire_scale (a one-element float32 CUDA
+    tensor on t's device, the same value on every rank, as an fp8 recipe's scales are; None means 1), sends the other
+    ranks' chunks as fp8 byte archives and sums with the dequantisation scale d = u / wire_scale (one float32
+    division by torch on the device; d = u without wire_scale), where u is 1, np.float32(scale), np.float32(1 / world)
+    with average=True, or scale_tensor.  The float32 result is the rank-order fold of q_r.float() * d, q_r the fp8
+    cast of t_r's chunk, bit for bit on every rank; found_inf and sq_norm work as above (with scale_tensor).
+    reduce_dtype and out_dtype must be None or float32; error_feedback is not supported.  wire_scale without an fp8
+    wire_dtype raises ValueError before any communication."""
     s32 = _check_scale("reduce_scatter_compressed", scale, average, scale_tensor, found_inf, t.device)
     _check_sq_norm("reduce_scatter_compressed", sq_norm, scale_tensor, t.device)
     _check_sparse_wire(t.dtype, "reduce_scatter_compressed", sparse, wire_dtype)
+    if wire_dtype in ops.FP8_TYPES:
+        return _reduce_scatter_fp8(t, group, members, temp_mem, check, reduce_dtype, wire_dtype, s32, average,
+                                   scale_tensor, found_inf, out_dtype, sq_norm, error_feedback, wire_scale)
+    _check_wire_scale("reduce_scatter_compressed", wire_scale, wire_dtype, t.device)
     narrow_dtype = _check_out_dtype("reduce_scatter_compressed", out_dtype, t.dtype, reduce_dtype, wire_dtype)
     acc_dtype = _check_reducible(t, "reduce_scatter_compressed", reduce_dtype)
     _check_wire(t, "reduce_scatter_compressed", wire_dtype)
@@ -842,6 +888,83 @@ def reduce_scatter_compressed(t: torch.Tensor, group=None, members: int = 8,
     if check and not all(bool(st.all()) for st in statuses):
         raise RuntimeError("reduce_scatter_compressed: a received archive failed to decode")
     return res
+
+
+def _reduce_scatter_fp8(t, group, members, temp_mem, check, reduce_dtype, wire_dtype, s32, average, scale_tensor,
+                        found_inf, out_dtype, sq_norm, error_feedback, wire_scale) -> torch.Tensor:
+    """reduce_scatter_compressed with an fp8 wire_dtype (its docstring has the contract)."""
+    what = "reduce_scatter_compressed"
+    _check_reducible(t, what, None)
+    _check_wire(t, what, wire_dtype)
+    if reduce_dtype not in (None, torch.float32) or out_dtype not in (None, torch.float32):
+        raise ValueError(f"{what}: an fp8 wire sums in float32: reduce_dtype and out_dtype are None or float32, not "
+                         f"{reduce_dtype} and {out_dtype}")
+    _check_fp8_wire(what, wire_dtype, error_feedback)
+    _check_wire_scale(what, wire_scale, wire_dtype, t.device)
+    world = _world(group)
+    dev = t.device
+    if average:
+        s32 = np.float32(1 / world)
+    # the dequantisation scale d = u / wire_scale, a device tensor the decode-and-sum reads
+    if scale_tensor is not None:
+        u = scale_tensor
+    else:
+        u = torch.full((1,), 1.0 if s32 is None else float(s32), dtype=torch.float32, device=dev)
+    d = u if wire_scale is None else u / wire_scale
+    flat = t.reshape(-1)
+    n = flat.numel()
+    if n % world:
+        raise ValueError(f"{what}: numel {n} is not divisible by the world size {world}")
+    shard = n // world
+    bounds = _split(shard, max(1, int(members)), 8)
+
+    def own_term(rank):
+        q = ops.cast_fp8([flat[rank * shard:(rank + 1) * shard]], wire_dtype, wire_scale)[0]
+        return q.float() * d.reshape(())
+
+    if world == 1 or n == 0:
+        res = own_term(0)
+        _flag_non_finite(found_inf, res)
+        _shard_sq_norm(sq_norm, res, bounds)
+        return res
+    rank = dist.get_rank(group)
+    m = len(bounds) - 1
+    dests = [k for k in range(world) if k != rank]
+    comp, sizes, _ = ops.compress_data(True, [flat[k * shard + bounds[i]: k * shard + bounds[i + 1]]
+                                              for k in dests for i in range(m)], False, temp_mem,
+                                       archive_dtype=wire_dtype, scale_tensor=wire_scale)
+    hs = sizes.cpu().tolist()  # host sync: the packed layout needs the archive sizes
+    per_dest = [[comp.new_empty(0)] * m for _ in range(world)]  # nothing for this rank's own chunk
+    for j, k in enumerate(dests):
+        per_dest[k] = [comp[j * m + i, :hs[j * m + i]] for i in range(m)]
+    archives, _ = _send_to_each(per_dest, group)
+    out = torch.empty(shard, dtype=torch.float32, device=dev)
+    outs = [out[bounds[i]:bounds[i + 1]] for i in range(m)]
+    own = own_term(rank)  # the kernel's term of the own chunk, from the same cast kernel
+    statuses = []
+    if rank == 0:
+        out.copy_(own)
+    else:
+        st = torch.zeros(m * rank, dtype=torch.uint8, device=dev)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank)] for i in range(m)], outs, False, temp_mem, st,
+                                   archive_dtype=wire_dtype, scale_tensor=d)
+        statuses.append(st)
+        out.add_(own)
+    if rank + 1 < world:
+        st = torch.zeros(m * (world - rank - 1), dtype=torch.uint8, device=dev)
+        pieces_sq = None if sq_norm is None else torch.zeros(m, dtype=torch.float64, device=dev)
+        ops.decompress_data_reduce([[archives[s][i] for s in range(rank + 1, world)] for i in range(m)], outs, True,
+                                   temp_mem, st, archive_dtype=wire_dtype, scale_tensor=d, found_inf=found_inf,
+                                   sq_norm=pieces_sq)
+        statuses.append(st)
+        if sq_norm is not None:
+            _fold(sq_norm, pieces_sq)
+    else:
+        _flag_non_finite(found_inf, out)
+        _shard_sq_norm(sq_norm, out, bounds)
+    if check and not all(bool(st.all()) for st in statuses):
+        raise RuntimeError(f"{what}: a received archive failed to decode")
+    return out
 
 
 def all_reduce_compressed(t: torch.Tensor, group=None, members: int = 8, temp_mem: Optional[torch.Tensor] = None,

@@ -363,7 +363,8 @@ size_t dgb_float_compress_temp_bytes(int ft, uint32_t n, uint32_t maxFloats) {
   return validFloatType(ft) ? encodeTempBytes(ft, n, maxFloats) : 0;
 }
 size_t dgb_float_decompress_temp_bytes(int ft, uint32_t n, uint32_t /*maxFloats*/) {
-  return validFloatType(ft) ? decodeTempBytes(ft, n) : 0;
+  // the fp8 types: the scratch of their decode-and-sum
+  return validFloatType(ft) || isFp8Kind(ft) ? decodeTempBytes(ft, n) : 0;
 }
 
 // ---- encode ----------------------------------------------------------------
@@ -459,6 +460,13 @@ int dgb_float_compress_to_ef(void* temp, size_t tempBytes, int inFt, int ft, int
       return DGB_ERR_INVALID_ARG;
   }
   return encodeBatch(kind, temp, tempBytes, pb, useChecksum != 0, n, v, nullptr, outSize_dev, (cudaStream_t)stream, err);
+}
+
+int dgb_float_cast_fp8(int inFt, int fp8Ft, uint32_t n, const void* const* in, const uint32_t* inSize,
+                       const float* scale_dev, void* const* out, uint32_t* histogram_dev, void* stream) {
+  if ((inFt != DGB_FLOAT32 && inFt != DGB_BFLOAT16) || !isFp8Kind(fp8Ft)) return DGB_ERR_INVALID_ARG;
+  if (reinterpret_cast<uintptr_t>(scale_dev) & 3u) return DGB_ERR_INVALID_ARG;
+  return castFp8(inFt, fp8Ft, n, in, inSize, scale_dev, out, histogram_dev, (cudaStream_t)stream);
 }
 
 int dgb_float_compress_split_size(void* temp, size_t tempBytes, int ft, int pb, int useChecksum,
@@ -646,7 +654,7 @@ int dgb_float_decompress_reduce_narrow_norm(void* temp, size_t tempBytes, int ft
 size_t dgb_float_decompress_reduce_norm_temp_bytes(int ft, uint32_t numGroups, uint32_t archivesPerGroup,
                                                    const uint32_t* outSize) {
   const uint64_t n = (uint64_t)numGroups * archivesPerGroup;
-  if (!validFloatType(ft) || n > 0xffffffffull || (numGroups && !outSize)) return 0;
+  if (!(validFloatType(ft) || isFp8Kind(ft)) || n > 0xffffffffull || (numGroups && !outSize)) return 0;
   return decodeTempBytes(ft, (uint32_t)n) + sqNormScratchBytes(numGroups, sqNormBlocks(numGroups, outSize));
 }
 

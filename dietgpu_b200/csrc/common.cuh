@@ -124,8 +124,12 @@ enum CodecKind : int {
   // e the member's float32 residual word, and the coder overwrites e with y - float(round(y)) (+0 where the rounded
   // word is not finite).  Encoder only, never on the wire; their kernels also take the residual table (EfMembers).
   kKindF32toF16EF = 0x80 | kKindF32toF16,
-  kKindF32toBF16EF = 0x80 | kKindF32toBF16
+  kKindF32toBF16EF = 0x80 | kKindF32toBF16,
+  // fp8 words: their archives are byte archives, so only the fp8 decode-and-sum (decode_fp8.cu) dispatches them
+  kKindE4M3 = DGB_FLOAT8_E4M3,
+  kKindE5M2 = DGB_FLOAT8_E5M2
 };
+__host__ __device__ constexpr bool isFp8Kind(int k) { return k == kKindE4M3 || k == kKindE5M2; }
 __host__ __device__ constexpr bool isEfKind(int k) { return k == kKindF32toF16EF || k == kKindF32toBF16EF; }
 __host__ __device__ constexpr bool isNarrowKind(int k) {
   return k == kKindF32toF16 || k == kKindF32toBF16 || isEfKind(k);
@@ -277,6 +281,17 @@ int launchDecodeReduceNorm(int kind, int pb, bool widen, const Options& opt, Mem
                            const InlineMembers& im, uint32_t groups, uint32_t width, uint64_t totalChunks,
                            bool accumulate, uint8_t* outSuccess, cudaStream_t stream, const float* scaleDev,
                            float* foundInf, void* const* narrowTable, const SqNormScratch& norm, double* sqNorm);
+// the fold of the block partials into sqNorm[g] for the groups the decode-and-sum kernels found valid (decode_norm.cu)
+int sqNormFoldValid(const Options& opt, const SqNormScratch& norm, uint32_t groups, double* sqNorm, cudaStream_t stream);
+// decodeReduce's launches of the fp8 kinds (decode_fp8.cu): fp8 byte archives summed into fp32 with the device scale,
+// | kSqNorm when norm is not null (then followed by the fold into sqNorm)
+int launchDecodeReduceFp8(int kind, int pb, const Options& opt, MemberDesc* members, uint32_t* next,
+                          const InlineMembers& im, uint32_t groups, uint32_t width, uint64_t totalChunks,
+                          bool accumulate, uint8_t* outSuccess, cudaStream_t stream, const float* scaleDev,
+                          float* foundInf, const SqNormScratch* norm, double* sqNorm);
+// dgb_float_cast_fp8 (cast_fp8.cu): inKind fp32 or bf16, fp8Kind e4m3 or e5m2 (checked by the entry point)
+int castFp8(int inKind, int fp8Kind, uint32_t n, const void* const* in, const uint32_t* size, const float* scaleDev,
+            void* const* out, uint32_t* histogram, cudaStream_t stream);
 // dgb_float_sq_norm: dense fp16 / bf16 / fp32 words
 size_t floatSqNormTempBytes(uint32_t groups, const uint32_t* size);
 int floatSqNorm(int kind, void* temp, size_t tempBytes, uint32_t groups, const void* const* in, const uint32_t* size,

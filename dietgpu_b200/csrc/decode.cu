@@ -58,6 +58,12 @@ __device__ __forceinline__ ArchiveView openArchive(const uint8_t* in) {
     v.non = nullptr;
     v.floatWords = 0;
     v.ok = true;
+  } else if constexpr (isFp8Kind(KIND)) {
+    // a byte archive of fp8 words: floatWords is the ANS header's uncompressed size, one byte per word
+    v.ans = in;
+    v.non = nullptr;
+    v.floatWords = __ldg(reinterpret_cast<const uint32_t*>(in) + 2);
+    v.ok = true;
   } else if constexpr (isSparseKind(KIND)) {
     // the 32 B header: the dense 16 B, then S and esc (DESIGN.md section 0)
     const uint4 fh = __ldg(reinterpret_cast<const uint4*>(in));
@@ -254,6 +260,23 @@ struct RowWriter16 {
 };
 template <> struct RowWriter<kKindF16> : RowWriter16<kKindF16> {};
 template <> struct RowWriter<kKindBF16> : RowWriter16<kKindBF16> {};
+
+// fp8 archives (decode-and-sum only, as the base of RowWriterSum): the decoded symbol is the whole fp8 word, so there
+// is no stored plane and no ring
+template <int KIND>
+struct RowWriterFp8 {
+  static constexpr uint32_t kRingSlotBytes = 0;
+  struct Cursor {};
+  __device__ __forceinline__ void setRing(uint32_t, uint32_t) {}
+  __device__ __forceinline__ void setBlock(const ArchiveView&, void*, uint32_t, uint32_t) {}
+  __device__ __forceinline__ Cursor at(uint32_t, uint32_t) const { return Cursor{}; }
+  __device__ __forceinline__ void issue(uint32_t, uint32_t) const {}
+  template <int J>
+  __device__ __forceinline__ uint32_t word(const Cursor&, uint32_t entry) const { return entry & 0xffu; }
+  __device__ __forceinline__ uint32_t wordSlow(uint32_t, uint32_t entry) const { return entry & 0xffu; }
+};
+template <> struct RowWriter<kKindE4M3> : RowWriterFp8<kKindE4M3> {};
+template <> struct RowWriter<kKindE5M2> : RowWriterFp8<kKindE5M2> {};
 
 // Sparse fp16 / bf16: the block's segment of stored bytes, [table[k], table[k + 1] or S), sits in the warp's ring
 // (one copy per block, widened to 16 B bounds: at most 4112 bytes).  Rows are walked backwards, so the cursor
@@ -1093,7 +1116,7 @@ decodeFusedKernel(DecodeScratch sc, const __grid_constant__ InlineMembers im, ui
 
 // XOR checksum of decoded outputs (ans/GpuChecksum.cuh:26-93 semantics: XOR of
 // all bytes folded to 8 bits).  grid = (n, Y).
-#if !defined(DGB_DECODE_NARROW_TU) && !defined(DGB_DECODE_NORM_TU)
+#if !defined(DGB_DECODE_NARROW_TU) && !defined(DGB_DECODE_NORM_TU) && !defined(DGB_DECODE_FP8_TU)
 __global__ void __launch_bounds__(256)
 checksumKernel(DecodeScratch sc) {
   const uint32_t m = blockIdx.x;
@@ -1132,8 +1155,10 @@ DecodePlan planDecodeScratch(uint32_t n) {
 template <int KIND, int PB>
 size_t decoderSmem(int warps, const Options& opt, uint32_t* slotWords) {
   // fp64's stored-plane ring is 10.5 KiB per warp: with a 1024-word slot two 8-warp CTAs fit on an SM
+  // fp8 archives code whole words, about 7 bits each for gradients: the worst-case slot, as for byte archives
   uint32_t slot = opt.decode_slot_words > 0 ? (uint32_t)opt.decode_slot_words
-                                            : (KIND == kKindBytes ? maxBlockWords(PB) : (KIND == kKindF64 ? 1024u : 1536u));
+                                            : (KIND == kKindBytes || isFp8Kind(KIND) ? maxBlockWords(PB)
+                                                                                    : (KIND == kKindF64 ? 1024u : 1536u));
   slot = std::min(roundUp(slot, 8u), maxBlockWords(PB));
   *slotWords = slot;
   return (2 * kNumSymbols + 64) * 4 + ((warps + 1) & ~1) * 8 + (size_t)warps * kRingSlots * RowWriter<KIND>::kRingSlotBytes +
@@ -1253,6 +1278,16 @@ template <int KIND>
 __device__ __forceinline__ uint32_t widenWord(uint32_t w) {
   if constexpr (KIND == kKindBF16) {
     return w << 16;
+  } else if constexpr (isFp8Kind(KIND)) {
+    // an fp8 word (low byte; the byte above it is dropped) to f16 and f16 to fp32, both exact
+    uint32_t h;
+    if constexpr (KIND == kKindE4M3)
+      asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((unsigned short)w));
+    else
+      asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(h) : "h"((unsigned short)w));
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)h));
+    return __float_as_uint(f);
   } else {
     float f;
     asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)w));
@@ -1814,7 +1849,7 @@ int launchDecodeReduceNarrow(int kind, int pb, bool scaled, const Options& opt, 
     }
   }); });
 }
-#elif !defined(DGB_DECODE_NORM_TU)
+#elif !defined(DGB_DECODE_NORM_TU) && !defined(DGB_DECODE_FP8_TU)
 
 size_t decodeTempBytes(int /*kind*/, uint32_t n) { return planDecodeScratch(n).total + 256; }
 
@@ -1963,11 +1998,15 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
   // its output of the archive's 16-bit type; out and out[g] may be null when the call reads no accumulator (W = 1
   // without accumulate).  sqNorm (device, G doubles; with scaleDev only): the squared-norm kernels (decode_norm.cu),
   // whose block partials take the scratch past the decode's own
-  if (sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32)) return DGB_ERR_INVALID_ARG;
+  // fp8 byte archives (decode_fp8.cu): fp32 outputs, device scale only
+  const bool fp8 = isFp8Kind(kind);
+  if (fp8 ? (sparse || !scaleDev || narrowOut || outKind != kKindF32)
+          : sparse ? !isSparseKind(kind) : (kind != kKindF16 && kind != kKindBF16 && kind != kKindF32))
+    return DGB_ERR_INVALID_ARG;
   // outputs of the archive's dense kind, or fp32 sums of (sparse) fp16 / bf16 archives
   const int dk = denseKind(kind);
   const bool widen = outKind != dk;
-  if (widen && !(outKind == kKindF32 && (dk == kKindF16 || dk == kKindBF16))) return DGB_ERR_INVALID_ARG;
+  if (widen && !fp8 && !(outKind == kKindF32 && (dk == kKindF16 || dk == kKindBF16))) return DGB_ERR_INVALID_ARG;
   if (narrowOut && !widen) return DGB_ERR_INVALID_ARG;
   if (pb < 9 || pb > 11 || width == 0) return DGB_ERR_INVALID_ARG;
   if (groups == 0) return DGB_OK;
@@ -2025,6 +2064,15 @@ int decodeReduce(int kind, int outKind, void* temp, size_t tempBytes, int pb, ui
     t = reinterpret_cast<void**>(base + dp.checksum);
     const int rc = uploadTable(t, narrowOut, sizeof(void*) * (size_t)groups, stream);
     if (rc != DGB_OK) return rc;
+  }
+  if (fp8) {
+    SqNormScratch ns;
+    if (sqNorm) {
+      const int rc = sqNormPrepare(base + dp.total, groups, outSize, &ns, stream);
+      if (rc != DGB_OK) return rc;
+    }
+    return launchDecodeReduceFp8(kind, pb, opt, sc.members, sc.next, im, groups, width, totalChunks, accumulate,
+                                 outSuccess_dev, stream, scaleDev, foundInf, sqNorm ? &ns : nullptr, sqNorm);
   }
   if (sqNorm) {
     SqNormScratch ns;
@@ -2238,6 +2286,6 @@ int getInfo(int kind, void* temp, size_t tempBytes, const void* const* in, bool 
   return DGB_OK;
 }
 
-#endif  // DGB_DECODE_NARROW_TU, DGB_DECODE_NORM_TU
+#endif  // DGB_DECODE_NARROW_TU, DGB_DECODE_NORM_TU, DGB_DECODE_FP8_TU
 
 }  // namespace dgb

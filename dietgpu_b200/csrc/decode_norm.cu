@@ -97,6 +97,11 @@ int launchSqNormFold(const Options& opt, const SqNormScratch& ns, uint32_t group
 
 }  // namespace
 
+int sqNormFoldValid(const Options& opt, const SqNormScratch& norm, uint32_t groups, double* sqNorm,
+                    cudaStream_t stream) {
+  return launchSqNormFold(opt, norm, groups, true, sqNorm, stream);
+}
+
 int sqNormPrepare(uint8_t* base, uint32_t groups, const uint32_t* size, SqNormScratch* out, cudaStream_t stream) {
   const uint64_t blocks = sqNormBlocks(groups, size);
   if (blocks > 0xffffffffull) return DGB_ERR_TOO_LARGE;

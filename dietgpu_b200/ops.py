@@ -163,6 +163,80 @@ def _validate_out(out_compressed, out_sizes, n: int, cols: int, dev):
 
 
 _NARROW_TYPES = {torch.float16: capi.FLOAT16, torch.bfloat16: capi.BFLOAT16}
+# fp8 archives: byte archives of the scaled fp8 cast (dgb_float_cast_fp8) of float32 / bfloat16 inputs
+FP8_TYPES = {torch.float8_e4m3fn: capi.FLOAT8_E4M3, torch.float8_e5m2: capi.FLOAT8_E5M2}
+_FP8_INPUT_TYPES = {torch.float32: capi.FLOAT32, torch.bfloat16: capi.BFLOAT16}
+
+
+def _check_fp8_inputs(what: str, ts_in: Sequence[torch.Tensor], dtype, scale_tensor) -> None:
+    """The arguments of a scaled fp8 cast: an fp8 dtype, a non-empty list of contiguous CUDA tensors of one dtype
+    (float32 or bfloat16) on one device, and scale_tensor None or a one-element float32 CUDA tensor on that device.
+    Reads metadata only."""
+    if dtype not in FP8_TYPES:
+        raise ValueError(f"{what}: the fp8 dtype is torch.float8_e4m3fn or torch.float8_e5m2, not {dtype}")
+    if isinstance(ts_in, torch.Tensor) or len(ts_in) == 0:
+        raise ValueError(f"{what}: a non-empty list of tensors expected")
+    d0, dev = ts_in[0].dtype, ts_in[0].device
+    for t in ts_in:
+        if getattr(t, "dtype", None) not in _FP8_INPUT_TYPES or t.dtype != d0 or not t.is_cuda \
+                or t.device != dev or not t.is_contiguous():
+            raise ValueError(f"{what}: contiguous float32 or bfloat16 CUDA tensors of one dtype on one device expected")
+        if t.numel() > 0xFFFFFFFF:
+            raise ValueError(f"{what}: a tensor of more than 2^32 - 1 elements")
+    if scale_tensor is not None:
+        _check_flag_tensor(f"{what}: scale_tensor", scale_tensor, dev)
+
+
+def _cast_fp8_ptrs(ts_in: Sequence[torch.Tensor], ft: int, scale_tensor, out_ptrs, hist_ptr) -> None:
+    L = capi.lib()
+    with torch.cuda.device(ts_in[0].device):
+        rc = L.dgb_float_cast_fp8(_FP8_INPUT_TYPES[ts_in[0].dtype], ft, len(ts_in),
+                                  capi.ptr_array([t.data_ptr() for t in ts_in]),
+                                  capi.u32_array([t.numel() for t in ts_in]),
+                                  None if scale_tensor is None else scale_tensor.data_ptr(), out_ptrs, hist_ptr,
+                                  _stream())
+    capi.check(rc, "cast_fp8")
+
+
+def cast_fp8(ts_in: Sequence[torch.Tensor], dtype: torch.dtype,
+             scale_tensor: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+    """The scaled fp8 cast (dgb_float_cast_fp8) of contiguous float32 or bfloat16 CUDA tensors of one dtype on one
+    device: returns one tensor of `dtype` (torch.float8_e4m3fn or torch.float8_e5m2) per input, shaped like it,
+    holding (t.float() * s).clamp(-M, M).to(dtype) byte for byte, with s = scale_tensor (a one-element float32 CUDA
+    tensor read by the kernel, never by the host; None means 1) and M the dtype's largest finite value (448 or 57344).
+    A NaN product gives the byte 0x7F.  One pass over each input.  Misuse raises ValueError before any device work."""
+    _check_fp8_inputs("cast_fp8", ts_in, dtype, scale_tensor)
+    outs = [torch.empty(t.shape, dtype=dtype, device=t.device) for t in ts_in]
+    _cast_fp8_ptrs(ts_in, FP8_TYPES[dtype], scale_tensor, capi.ptr_array([o.data_ptr() for o in outs]), None)
+    return outs
+
+
+def _compress_fp8(ts_in, dtype, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits, scale_tensor):
+    """compress_data(True, ts_in, archive_dtype=<fp8>): the cast with its histogram into a 16 B-aligned temporary,
+    then the byte encoder given that histogram."""
+    n = len(ts_in)
+    dev = ts_in[0].device
+    mx, _ = _max_numel_and_bytes(ts_in)
+    L = capi.lib()
+    cols = _bound(L.dgb_ans_max_compressed_size(mx), mx)
+    comp, sizes = _validate_out(out_compressed, out_compressed_bytes, n, cols, dev)
+    row = comp.size(1)
+    offs, o = [], 0
+    for t in ts_in:
+        offs.append(o)
+        o += (t.numel() + 15) // 16 * 16
+    with torch.cuda.device(dev):
+        q = torch.empty(max(o, 16), dtype=torch.uint8, device=dev)
+        hist = torch.empty(n * 256, dtype=torch.int32, device=dev)
+        q_ptrs = capi.ptr_array([q.data_ptr() + k for k in offs])
+        _cast_fp8_ptrs(ts_in, FP8_TYPES[dtype], scale_tensor, q_ptrs, hist.data_ptr())
+        tmp = _Temp(temp_mem, L.dgb_ans_encode_temp_bytes(n, mx), dev)
+        rc = L.dgb_ans_encode_pointer(tmp.ptr, tmp.bytes, prob_bits, int(checksum), n, q_ptrs,
+                                      capi.u32_array([t.numel() for t in ts_in]), hist.data_ptr(),
+                                      capi.ptr_array([comp.data_ptr() + i * row for i in range(n)]), sizes.data_ptr(),
+                                      _stream())
+    capi.check(rc, "compress_data")
+    return comp, sizes, tmp.need
 
 
 def _narrow_type(compress_as_float: bool, ts_in: Sequence[torch.Tensor], sparse: bool,
@@ -185,7 +259,8 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
                   out_compressed_bytes: Optional[torch.Tensor] = None, *,
                   prob_bits: int = K_DEFAULT_PRECISION, sparse: bool = False,
                   archive_dtype: Optional[torch.dtype] = None,
-                  error_feedback: Optional[Sequence[torch.Tensor]] = None):
+                  error_feedback: Optional[Sequence[torch.Tensor]] = None,
+                  scale_tensor: Optional[torch.Tensor] = None):
     """archive_dtype (float16 / bfloat16, with float32 inputs): narrowing compress (dgb_float_compress_to).
     Every member's archive is exactly the archive of t.to(archive_dtype) (torch's CUDA cast), with rows sized by
     that type's bound, and no 16-bit temporary is made.  None, or the inputs' dtype, is the ordinary call; any
@@ -196,7 +271,26 @@ def compress_data(compress_as_float: bool, ts_in: Sequence[torch.Tensor], checks
     previous call left.  Member i is compressed as y = ts_in[i] + e_i (torch's add), so its archive is exactly the
     archive of y.to(archive_dtype), and e_i is overwritten in place with
     torch.where(w.isfinite(), y - w.float(), 0) for w = y.to(archive_dtype), bit for bit, in the same kernels.
-    Error buffers must not overlap the inputs or each other.  Any misuse raises ValueError before any device work."""
+    Error buffers must not overlap the inputs or each other.  Any misuse raises ValueError before any device work.
+
+    archive_dtype=torch.float8_e4m3fn / torch.float8_e5m2 (float32 or bfloat16 inputs, compress_as_float=True,
+    sparse=False, no error_feedback): fp8 compress.  Member i's archive is the byte archive (compress_data(False, ...))
+    of cast_fp8([ts_in[i]], archive_dtype, scale_tensor)[0] viewed as uint8, rows sized by
+    max_any_compressed_output_size: the cast writes the fp8 bytes and their histogram into a temporary in one pass,
+    and the byte encoder, given that histogram, skips its own statistics pass.  Decode with
+    decompress_data(False, [archive], [out.view(torch.uint8)]) or sum with decompress_data_reduce(archive_dtype=).
+    scale_tensor (fp8 compress only): the cast's scale, a one-element float32 CUDA tensor (None means 1)."""
+    if archive_dtype in FP8_TYPES:
+        if not compress_as_float or sparse or error_feedback is not None:
+            raise ValueError("compress_data: an fp8 archive_dtype needs compress_as_float=True, sparse=False and no "
+                             f"error_feedback; got compress_as_float={compress_as_float}, sparse={sparse}, "
+                             f"error_feedback={'set' if error_feedback is not None else None}")
+        _check_fp8_inputs("compress_data", ts_in, archive_dtype, scale_tensor)
+        return _compress_fp8(ts_in, archive_dtype, checksum, temp_mem, out_compressed, out_compressed_bytes, prob_bits,
+                             scale_tensor)
+    if scale_tensor is not None:
+        raise ValueError("compress_data: scale_tensor is the scale of an fp8 compress (archive_dtype "
+                         f"torch.float8_e4m3fn or torch.float8_e5m2), not of archive_dtype={archive_dtype}")
     narrow = _narrow_type(compress_as_float, ts_in, sparse, archive_dtype)
     if error_feedback is not None and narrow is None:
         raise ValueError("compress_data: error_feedback needs a narrowing compress (float32 inputs, archive_dtype "
@@ -555,13 +649,22 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
     outputs.  A group with an invalid archive leaves sq_norm[g] untouched.  Works with archive_dtype, sparse,
     reduce_dtype=torch.float32 / acc and found_inf; outputs and found_inf are bit-identical to the call without it.
     Without scale_tensor, with scale, or of the wrong dtype, size or device it raises ValueError before any archive
-    is read."""
+    is read.
+
+    archive_dtype=torch.float8_e4m3fn / torch.float8_e5m2: fp8 archives (compress_data(archive_dtype=) or the byte
+    archives of fp8 words) summed into float32 outputs with the device scale d = scale_tensor, which is required: the
+    result is torch's fold acc = q(g, 0).float() * d (or ts_out[g] when accumulating); acc = acc + q(g, 1).float() * d;
+    ... bit for bit, with found_inf and sq_norm as above.  Float32 outputs only; scale, sparse, acc and a reduce_dtype
+    other than None or float32 raise ValueError before any archive is read."""
     scale32 = _scale32(scale)
     _check_dev_scale(scale32, scale_tensor, found_inf, ts_out[0].device if len(ts_out) else None)
     if sq_norm is not None:
         if scale_tensor is None:
             raise ValueError("decompress_data_reduce: sq_norm needs scale_tensor (torch.ones(1) for the unscaled sum)")
         _check_sq_norm("decompress_data_reduce: sq_norm", sq_norm, len(ts_out), ts_out[0].device if len(ts_out) else None)
+    if archive_dtype in FP8_TYPES:
+        return _reduce_fp8(ts_in, ts_out, accumulate, temp_mem, out_status, prob_bits, archive_dtype, sparse,
+                           scale32, scale_tensor, found_inf, reduce_dtype, acc, sq_norm)
     _check(len(ts_in) > 0 and len(ts_in) == len(ts_out), "one output per group")
     width = len(ts_in[0])
     _check(width > 0, "a group needs at least one archive")
@@ -665,6 +768,50 @@ def decompress_data_reduce(ts_in: Sequence[Sequence[torch.Tensor]], ts_out: Sequ
                    capi.ptr_array([t.data_ptr() for t in ts_out]),
                    capi.u32_array([t.numel() for t in ts_out]), int(bool(accumulate)), *extra,
                    st_ptr, _stream())
+    capi.check(rc, "decompress_data_reduce")
+    return tmp.need
+
+
+def _reduce_fp8(ts_in, ts_out, accumulate, temp_mem, out_status, prob_bits, archive_dtype, sparse, scale32,
+                scale_tensor, found_inf, reduce_dtype, acc, sq_norm_out) -> int:
+    """decompress_data_reduce of fp8 archives (dgb_float_decompress_reduce_scaled_dev / _norm)."""
+    if scale_tensor is None or scale32 is not None or sparse or acc is not None \
+            or reduce_dtype not in (None, torch.float32):
+        raise ValueError("decompress_data_reduce: fp8 archives are summed into float32 with scale_tensor (the "
+                         f"dequantisation scale), without scale, sparse or acc; got scale={scale32}, sparse={sparse}, "
+                         f"reduce_dtype={reduce_dtype}, acc={'set' if acc is not None else None}")
+    if len(ts_out) == 0 or any(not isinstance(o, torch.Tensor) or o.dtype != torch.float32 for o in ts_out):
+        raise ValueError("decompress_data_reduce: fp8 archives are summed into float32 outputs")
+    _check(len(ts_in) == len(ts_out), "one output per group")
+    width = len(ts_in[0])
+    _check(width > 0, "a group needs at least one archive")
+    dev = ts_out[0].device
+    ins = []
+    for group, to in zip(ts_in, ts_out):
+        _check(len(group) == width, "every group needs the same number of archives")
+        _check(to.is_cuda and to.device == dev and to.is_contiguous(),
+               "outputs must be contiguous CUDA tensors on one device")
+        _check(to.numel() <= 0xFFFFFFFF)
+        for ti in group:
+            _check(ti.is_cuda and ti.device == dev and ti.is_contiguous() and ti.dtype == torch.uint8)
+            _check_archive_aligned(ti)
+            ins.append(ti)
+    g, n = len(ts_out), len(ins)
+    st_ptr, _ = _validate_status(out_status, None, n, dev)
+    ft = FP8_TYPES[archive_dtype]
+    L = capi.lib()
+    sizes = capi.u32_array([t.numel() for t in ts_out])
+    with torch.cuda.device(dev):
+        if sq_norm_out is not None:
+            tmp = _Temp(temp_mem, L.dgb_float_decompress_reduce_norm_temp_bytes(ft, g, width, sizes), dev)
+            entry, extra = L.dgb_float_decompress_reduce_scaled_dev_norm, (sq_norm_out.data_ptr(),)
+        else:
+            tmp = _Temp(temp_mem, L.dgb_float_decompress_temp_bytes(ft, n, 0), dev)
+            entry, extra = L.dgb_float_decompress_reduce_scaled_dev, ()
+        rc = entry(tmp.ptr, tmp.bytes, ft, capi.FLOAT32, prob_bits, g, width,
+                   capi.ptr_array([t.data_ptr() for t in ins]), capi.ptr_array([t.data_ptr() for t in ts_out]), sizes,
+                   int(bool(accumulate)), scale_tensor.data_ptr(),
+                   None if found_inf is None else found_inf.data_ptr(), *extra, st_ptr, _stream())
     capi.check(rc, "decompress_data_reduce")
     return tmp.need
 

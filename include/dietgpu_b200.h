@@ -69,6 +69,12 @@ extern "C" {
  * plane and a compacted u8 plane.  Same 32 B header and block table as the 16-bit sparse types (DESIGN.md
  * section 0).  7 stays unassigned. */
 #define DGB_FLOAT32_SPARSE 8
+/* fp8 words (OCP FP8: E4M3 with no infinities and max 448, E5M2 with max 57344).  An fp8 archive is an ordinary
+ * byte archive (dgb_ans_encode_pointer of the fp8 bytes; the 256-symbol coder codes each word whole), so there is no
+ * float header for these types: only dgb_float_cast_fp8 and the device-scale decode-and-sum entries take them, and
+ * every other float entry refuses them.  9 stays unassigned. */
+#define DGB_FLOAT8_E4M3 10
+#define DGB_FLOAT8_E5M2 11
 
 /* ans/GpuANSCodec.h:16,20 */
 #define DGB_ANS_REQUIRED_ALIGNMENT 4
@@ -175,6 +181,27 @@ int dgb_float_compress_pointer(void* temp_dev, size_t temp_bytes, int float_type
                                int use_checksum, uint32_t num_in_batch, const void* const* in,
                                const uint32_t* in_size, void* const* out, uint32_t* out_size_dev,
                                void* stream);
+
+/* Scaled fp8 cast with a fused histogram (new; no reference counterpart), the first half of an fp8 compress.
+ * in_float_type: DGB_FLOAT32 or DGB_BFLOAT16; fp8_type: DGB_FLOAT8_E4M3 or DGB_FLOAT8_E5M2; any other pair returns
+ * DGB_ERR_INVALID_ARG before any CUDA call.  in[i] (aligned to its word size) holds in_size[i] words; out[i]
+ * receives in_size[i] bytes, q = cvt.rn.satfinite.fp8(fp32(x) * s), with s = *scale_dev (4 B aligned; NULL means
+ * 1.0f), the product one round-to-nearest-even fp32 multiply (never contracted) and the bf16 widening exact.  For
+ * every x whose product is not NaN this is torch's (x.float() * s).clamp(-M, M).to(fp8) byte for byte (M = 448 for
+ * E4M3, 57344 for E5M2): out-of-range products and infinities saturate to +-M, products too small for the fp8
+ * type's subnormals round to +-0 and keep their sign.  A NaN product gives the byte 0x7F whatever its sign (the
+ * H100's F2FP.SATFINITE writes the positive canonical NaN).
+ * histogram_dev (may be NULL): num_in_batch x 256 u32 counts, overwritten (not accumulated) with the histogram of
+ * each out[i]: exactly what the byte encoder's statistics pass counts, so that
+ *   dgb_float_cast_fp8(..., out, hist, stream); dgb_ans_encode_pointer(..., out, in_size, hist, archives, ...)
+ * is the fp8 compress, whose archives are byte archives of q, bit-identical to dgb_ans_encode_pointer of q without a
+ * histogram.  With the histogram and no checksum the encoder skips its own statistics pass, so the input is read once
+ * and q is written once and read once.  out[i] may have any alignment, but the byte encoder wants it 4 B aligned
+ * (DGB_ANS_REQUIRED_ALIGNMENT).  in and out must not overlap.  Never synchronises; capturable into a CUDA graph (a
+ * replay reads *scale_dev's value then). */
+int dgb_float_cast_fp8(int in_float_type, int fp8_type, uint32_t num_in_batch, const void* const* in,
+                       const uint32_t* in_size, const float* scale_dev, void* const* out, uint32_t* histogram_dev,
+                       void* stream);
 
 /* Compress with a narrowing cast (new; no reference counterpart).  The allowed pairs (in_float_type, float_type)
  * are (DGB_FLOAT16, DGB_FLOAT16), (DGB_BFLOAT16, DGB_BFLOAT16) and (DGB_FLOAT32, DGB_FLOAT32), which are exactly
@@ -330,7 +357,15 @@ int dgb_float_decompress_reduce_scaled(void* temp_dev, size_t temp_bytes, int fl
  * sum that overflows and a non-finite running value taken in by accumulate all set it, since no later term turns
  * inf or NaN finite.
  * DGB_ERR_INVALID_ARG before any CUDA call: scale_dev NULL or not 4 B aligned, found_inf_dev not 4 B aligned, and
- * every argument dgb_float_decompress_reduce_scaled refuses. */
+ * every argument dgb_float_decompress_reduce_scaled refuses.
+ * fp8 sums: this entry and dgb_float_decompress_reduce_scaled_dev_norm also take the pairs (DGB_FLOAT8_E4M3,
+ * DGB_FLOAT32) and (DGB_FLOAT8_E5M2, DGB_FLOAT32), which no other decode-and-sum entry takes.  Their archives are
+ * byte archives (dgb_float_cast_fp8 + dgb_ans_encode_pointer) of out_size[g] fp8 words; one is valid iff its ANS
+ * header has the magic, prob_bits, ceil(out_size[g] / 4096) blocks and out_size[g] uncompressed bytes.  The term is
+ * fp32(q) * s (the fp8 word widened exactly, one fp32 multiply), so out[g] = (accumulate ? out[g] : term(q(g,0))) +
+ * term(q(g,1)) + ... in fp32 in archive order: torch's acc = q0.float() * d; acc = acc + q1.float() * d; ... bit for
+ * bit.  Statuses, found_inf_dev, groups left unwritten, graph capture and num_groups = 0 are as above; the scratch
+ * is dgb_float_decompress_temp_bytes(fp8 type, G * W, 0). */
 int dgb_float_decompress_reduce_scaled_dev(void* temp_dev, size_t temp_bytes, int float_type, int out_float_type,
                                            int prob_bits, uint32_t num_groups, uint32_t archives_per_group,
                                            const void* const* in, void* const* out, const uint32_t* out_size,
@@ -406,7 +441,8 @@ int dgb_float_decompress_reduce_narrow_norm(void* temp_dev, size_t temp_bytes, i
 
 /* Scratch of the two entries above: dgb_float_decompress_temp_bytes(float_type, G * W, 0) plus the squared norm's own
  * part, 8 B per 4096-word block of every group (8 * sum of ceil(out_size[g] / 4096)) and 12 B per group for the block
- * offsets, sizes and validity flags, each rounded up to 256 B.  0 for an invalid float_type. */
+ * offsets, sizes and validity flags, each rounded up to 256 B.  0 for an invalid float_type (the fp8 types are
+ * valid here). */
 size_t dgb_float_decompress_reduce_norm_temp_bytes(int float_type, uint32_t num_groups, uint32_t archives_per_group,
                                                    const uint32_t* out_size);
 
